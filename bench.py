@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- the headline measurement (contract: task brief "Measurement").
+"""bench.py -- the headline measurement.
 
 Workload = BASELINE.json configs[2], the configuration its metric is quoted on: the FULL TURN of the cascade on one GPU,
     Whisper-small STT (10 s / 16 kHz utterance, 128 tokens)  ->  Llama-3-8B bf16 (64-token prompt, 128-token reply)
@@ -101,7 +101,7 @@ def decode_bytes_llama(g, n_steps, B, past) -> float:
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons DURING the timed region."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -269,7 +269,7 @@ def reference_arm(args, rank, world):
     print(json.dumps(line), flush=True)
 
 
-# =============================================================================================== B200 arm
+# =============================================================================================== GPU arm
 _T0 = time.perf_counter()
 
 
@@ -305,6 +305,12 @@ class Stack:
         self.post = TTSPostProcessor(dev)
         self.torch = torch
 
+    def close(self) -> None:
+        """Free the lane's engines (the handler section builds its own: both sets of Llama-3-8B weights do not fit in 80 GB)."""
+        self.whisper.close()
+        self.llm.close()
+        self.tts.close()
+
 
 class TtsProfileWindow:
     """cudaProfilerStart/Stop around chunks [first, first + n) of the second utterance's frame loop (all lanes): an ncu launch
@@ -330,8 +336,11 @@ class TtsProfileWindow:
                     self.torch.cuda.cudart().cudaProfilerStop()
 
 
-def wave_device(st: Stack, pcm_dev, ev, tts_prof: "TtsProfileWindow | None" = None) -> None:
-    """One wave of S full turns as an engine-level launch sequence; stage boundaries marked with CUDA events."""
+def wave_device(st: Stack, pcm_dev, ev, tts_prof: "TtsProfileWindow | None" = None, out: "dict | None" = None) -> None:
+    """One wave of S full turns as an engine-level launch sequence; stage boundaries marked with CUDA events.  `out`: a dict
+    that receives what the wave hands its callers (device tensors, no synchronisation): STT ids, LLM tokens, TTS codes and
+    the int16 16 kHz audio of every chunk."""
+    keep = (lambda key, v: out.setdefault(key, []).append(v)) if out is not None else (lambda key, v: None)
     torch, S = st.torch, st.S
     dev = f"cuda:{st.dev}"
     ev["t0"].record()
@@ -341,7 +350,7 @@ def wave_device(st: Stack, pcm_dev, ev, tts_prof: "TtsProfileWindow | None" = No
         st.whisper.encode(nb)
         wa, wb_ = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         wa.record()
-        st.whisper.decode(nb, st.opts)
+        keep("stt", st.whisper.decode(nb, st.opts))
         wb_.record()
         ev["whisper_mark"].append((wa, wb_))
     ev["stt"].record()
@@ -355,7 +364,8 @@ def wave_device(st: Stack, pcm_dev, ev, tts_prof: "TtsProfileWindow | None" = No
     first = torch.cat(firsts)
     for b0 in range(0, S, st.llm_b):                                      # ---- LLM decode, llm_b sessions per launch
         sl = list(range(b0, min(S, b0 + st.llm_b)))
-        st.llm.decode(sl, first[b0:b0 + len(sl)].contiguous(), MAX_NEW - 1)
+        keep("llm", st.llm.decode(sl, first[b0:b0 + len(sl)].contiguous(), MAX_NEW - 1))
+    keep("llm_first", first)
     ev["llm"].record()
     eng = st.tts.engine
     text1, text2 = [3] * FIRST_SENTENCE, [5] * (MAX_NEW - FIRST_SENTENCE)
@@ -368,13 +378,13 @@ def wave_device(st: Stack, pcm_dev, ev, tts_prof: "TtsProfileWindow | None" = No
             if tts_prof is not None and text is text2:
                 tts_prof.chunk_begin(ci)
             for b0 in range(0, S, st.tts_b):
-                eng.decode_frames(list(range(b0, min(S, b0 + st.tts_b))), n)
+                keep("codes", eng.decode_frames(list(range(b0, min(S, b0 + st.tts_b))), n))
             ev["frames_mark"].append((torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)))
             a, b = ev["frames_mark"][-1]
             a.record()
             for b0 in range(0, S, st.tts_b):
                 for wav in eng.decode_audio_batch(list(range(b0, min(S, b0 + st.tts_b))), n, LEFT_CTX):
-                    st.post.to_int16_device(wav)
+                    keep("pcm16", st.post.to_int16_device(wav))
             b.record()
             if tts_prof is not None and text is text2:
                 tts_prof.chunk_end(ci)
@@ -383,7 +393,7 @@ def wave_device(st: Stack, pcm_dev, ev, tts_prof: "TtsProfileWindow | None" = No
     ev["tts"].record()
 
 
-def run_wave(stacks, pcm_dev, evs, tts_prof=None):
+def run_wave(stacks, pcm_dev, evs, tts_prof=None, outs=None):
     """One wave on every lane at once: a host thread per lane issues the lane's launch sequence on the lane's stream; the step is
     timed on the calling stream, from an event every lane waits for to an event that waits for every lane."""
     torch = stacks[0].torch
@@ -391,7 +401,7 @@ def run_wave(stacks, pcm_dev, evs, tts_prof=None):
     start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     start.record(cur)
     if len(stacks) == 1:
-        wave_device(stacks[0], pcm_dev, evs[0], tts_prof)
+        wave_device(stacks[0], pcm_dev, evs[0], tts_prof, outs[0] if outs else None)
     else:
         errs, Sl = [], stacks[0].S
 
@@ -401,7 +411,7 @@ def run_wave(stacks, pcm_dev, evs, tts_prof=None):
                 torch.cuda.set_device(st.dev)
                 with st.E.lane_context(st.dev, st.lane, st.lanes):
                     torch.cuda.current_stream().wait_event(start)
-                    wave_device(st, pcm_dev[i * Sl:(i + 1) * Sl], evs[i], tts_prof)
+                    wave_device(st, pcm_dev[i * Sl:(i + 1) * Sl], evs[i], tts_prof, outs[i] if outs else None)
                     evs[i]["done"].record()
             except BaseException as e:  # noqa: BLE001
                 errs.append(e)
@@ -500,6 +510,36 @@ LLM_STREAM_CHUNK = 4     # tokens per decode launch in the handler path: the TTS
                          # first-sentence TTS request waits behind at most 4 LLM steps on the lane's stream
 
 
+DUMP_PCM_SAMPLES = 1 << 20      # int16 samples of the turn's audio written by --dump-outputs (a fixed, seeded sample)
+
+
+def dump_outputs(outs, stacks, path: str) -> dict:
+    """What the last timed wave handed its callers, session-major over all lanes, as float64 (ids) / float32 (audio) .npy files.
+    Chunks of one session are concatenated in order; the audio of all sessions is sampled at fixed seeded positions."""
+    os.makedirs(path, exist_ok=True)
+    ids, lens, llm_first, llm_ids, codes, pcm = [], [], [], [], [], []
+    for st, o in zip(stacks, outs):
+        S, n_chunks = st.S, len(o["pcm16"]) // st.S
+        ids += [i.cpu().numpy() for i, _ in o["stt"]]
+        lens += [n.cpu().numpy() for _, n in o["stt"]]
+        llm_first += [f.cpu().numpy() for f in o["llm_first"]]
+        llm_ids += [i.cpu().numpy() for i, _ in o["llm"]]
+        cs = [c.cpu().numpy() for c in o["codes"]]                         # per chunk: launch groups of [B, n, groups]
+        groups = len(cs) // n_chunks
+        codes.append(np.concatenate([np.concatenate(cs[c * groups:(c + 1) * groups], axis=0) for c in range(n_chunks)], axis=1))
+        chunks = [p.cpu().numpy() for p in o["pcm16"]]                     # chunk-major, session-minor
+        pcm.append(np.stack([np.concatenate(chunks[s::S]) for s in range(S)]))
+    pcm_all = np.concatenate(pcm).astype(np.float32)
+    idx = np.sort(np.random.default_rng(0).choice(pcm_all.size, min(DUMP_PCM_SAMPLES, pcm_all.size), replace=False))
+    arrays = {"stt_ids": np.concatenate(ids).astype(np.float64), "stt_lens": np.concatenate(lens).astype(np.float64),
+              "llm_first_ids": np.concatenate(llm_first).astype(np.float64), "llm_ids": np.concatenate(llm_ids).astype(np.float64),
+              "tts_codes": np.concatenate(codes).astype(np.float64),
+              "tts_pcm16_sample": pcm_all.reshape(-1)[idx], "tts_pcm16_sample_index": idx.astype(np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(path, f"{name}.npy"), a)
+    return {name: list(a.shape) for name, a in arrays.items()} | {"tts_pcm16_shape": list(pcm_all.shape)}
+
+
 def make_handlers(S: int, dev: int, lanes: int = 1):
     """S pipeline units' worth of handler instances; the units of a lane share one engine per stage (gen_kwargs / kwargs of the
     reference slots)."""
@@ -548,6 +588,9 @@ def main():
                     help="cudaProfilerStart/Stop around this many 8-frame chunks (frames + codec + post-processing) of the TTS stage only")
     ap.add_argument("--profile-region", action="store_true",
                     help="cudaProfilerStart/Stop around the device-timed region (use with ncu --profile-from-start off)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (STT ids, LLM tokens, TTS codes, a seeded "
+                         "sample of the int16 audio) as DIR/<name>.npy")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -563,6 +606,7 @@ def main():
     from speech_to_speech_b200 import engine as E, shard
 
     assert args.warmup >= 3, "timing rules: at least 3 warm-up steps"
+    assert args.steps >= 1, "--steps: at least one timed step"
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device(f"cuda:{local_rank}"))
@@ -588,7 +632,7 @@ def main():
     xe[1].record()
     torch.cuda.synchronize()
     scatter_ms = xe[0].elapsed_time(xe[1])
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)       # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)       # > 50 MB L2
 
     def barrier():
         if world > 1:
@@ -614,7 +658,7 @@ def main():
     if rank == 0:
         sampler.start()
     E.launch_count(local_rank, reset=True)
-    evs, spans = [], []
+    evs, spans, outs = [], [], None
     barrier()
     if args.profile_region:
         torch.cuda.cudart().cudaProfilerStart()
@@ -623,7 +667,8 @@ def main():
         flush.fill_(i & 0xFF)                 # L2 flush between timed steps (not timed)
         ev = new_events()
         prof = TtsProfileWindow(torch, L, args.profile_tts_chunks) if args.profile_tts_chunks > 0 and i == 0 else None
-        spans.append(run_wave(stacks, pcm_dev, ev, prof))
+        outs = [{} for _ in range(L)] if i == args.steps - 1 else None
+        spans.append(run_wave(stacks, pcm_dev, ev, prof, outs))
         evs.append(ev[0])                     # stage boundaries: lane 0's (the lanes run the same sequence side by side)
     barrier()
     if args.profile_region:
@@ -631,6 +676,11 @@ def main():
     wall_s = time.perf_counter() - t_wall
     launches = E.launch_count(local_rank, reset=True)
     log(f"timed region done: {wall_s:.2f} s for {args.steps} wave(s), {launches} launches")
+    dumped = None
+    if args.dump_outputs and rank == 0:
+        dumped = dump_outputs(outs, stacks, args.dump_outputs)
+        log(f"outputs of the last timed step written to {args.dump_outputs}: {dumped}")
+    outs = None
 
     def stage(ev, a, b):
         return ev[a].elapsed_time(ev[b])
@@ -661,6 +711,10 @@ def main():
             # ~70 Python threads (two per session + the batchers' engine threads) hand work to each other through the GIL: the
             # default 5 ms switch interval is longer than a whole batch window
             sys.setswitchinterval(0.0005)
+            for s_ in stacks:
+                s_.close()
+            del flush
+            torch.cuda.empty_cache()
             handlers = make_handlers(S, local_rank, L)
             log("handler instances built and warmed up")
             auds = [pcm_dev[i].cpu().numpy() for i in range(S)]
@@ -716,7 +770,7 @@ def main():
         if os.path.exists(peaks_path):
             peak, peak_src = json.load(open(peaks_path))["hbm_gbs"], "MEASURED_PEAKS.json hbm_gbs (measured)"
         else:
-            peak, peak_src = 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+            peak, peak_src = 3350.0, "H100 SXM data sheet, 3.35 TB/s HBM3 (not measured)"
         # dominant stage of the step and its kernel's roofline
         shares = {k: v / ms_per_step for k, v in stages.items() if k in ("stt_ms", "llm_prefill_ms", "llm_decode_ms", "tts_talker_predictor_ms", "tts_codec_postproc_ms")}
         Sl = S // L                                                   # sessions of one lane
@@ -740,13 +794,9 @@ def main():
         n_frame_launch = (Sl + st.tts_b - 1) // st.tts_b
         frame_ms = stages["tts_talker_predictor_ms"] / (F1 + F2) / n_frame_launch
         ach_tts = L * frame_bytes / 1e9 / (frame_ms / 1e3)
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "ncu_traffic_r2.json")
-        if os.path.exists(tpath):
-            traffic = json.load(open(tpath)).get("llama_decode", {}).get("dram_bytes_per_launch")
         roofline = {"kernel": f"llama_decode_kernel (persistent, {min(Sl, st.llm_b)} sessions x {MAX_NEW - 1} steps per launch, Llama-3-8B bf16; "
                               f"{L} launch(es) run concurrently, one per lane of {lane_ctas} CTAs)",
-                    "bound": "hbm", "achieved": ach_llm, "peak": peak, "unit": "GB/s", "frac": ach_llm / peak, "traffic": traffic,
+                    "bound": "hbm", "achieved": ach_llm, "peak": peak, "unit": "GB/s", "frac": ach_llm / peak,
                     "achieved_note": f"sum over the {L} concurrent launches (each streams its own copy of the weights): "
                                      f"{L} x algorithmic_bytes_per_launch / launch_ms; achieved_per_launch is one launch alone",
                     "achieved_per_launch": ach_llm_launch, "concurrent_launches": L,
@@ -757,7 +807,7 @@ def main():
             "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "f16 (Whisper, codec-decoder contractions) / bf16 (Llama, talker, code predictor) operands, f32 accumulate and residual streams", "data": "synthetic",
             "config": workload_config(world, S),
-            "l2": "flushed between timed steps (256 MiB write); every stage streams > 126 MB of weights per launch",
+            "l2": "flushed between timed steps (256 MiB write); every stage streams > 50 MB of weights per launch",
             "lanes": {"per_gpu": L, "ctas_per_lane": lane_ctas, "sessions_per_lane": Sl,
                       "note": "SM partitions with their own engines and CUDA streams; stage_ms are lane 0's (all lanes run the same "
                               "sequence side by side), ms_per_step spans all lanes"},
@@ -773,7 +823,7 @@ def main():
                                              f"{min(Sl, st.tts_b)} sessions per launch, {L} concurrent", "bound": "hbm",
                                    "algorithmic_bytes_per_frame": frame_bytes, "ms_per_frame": frame_ms, "achieved": ach_tts, "peak": peak,
                                    "unit": "GB/s", "frac": ach_tts / peak,
-                                   "note": "latency-bound: ~630 grid-barrier phases of 5-10 us per frame (profiles/r2/tts_phase_trace.txt); "
+                                   "note": "latency-bound: ~630 grid-barrier phases per frame; "
                                            "weights are KV-free attention-light (<= 512 positions), KV bytes not counted"},
             "stt_only_sessions": world * S * AUDIO_S / (stages["stt_ms"] / 1e3),
         }
@@ -808,6 +858,8 @@ def main():
                                     "'latency_ms_at_70pct_load' / 'latency_ms_at_30pct_load' = turn ends evenly spread at 70 % / 30 % of the rate the loaded wave sustains")
         elif e2e:
             line["e2e"] = e2e
+        if dumped is not None:
+            line["dumped_outputs"] = {"dir": args.dump_outputs, "shapes": dumped}
         if world == 1 and not args.no_cpu_baseline:
             log("cpu baseline (child process)")
             line["cpu_baseline"] = cpu_baseline_subprocess(args.cpu_baseline_turns)

@@ -1,5 +1,5 @@
 /*
- * s2s_b200.h -- C ABI of libs2s_b200.so, the B200 (sm_100a) engine behind
+ * s2s_b200.h -- C ABI of libs2s_b200.so, the H100 (sm_90a) engine behind
  * huggingface/speech-to-speech's STT / LLM / TTS handler slots.
  *
  * The reference has no FFI of its own (pure Python); the calls this library replaces are
@@ -8,7 +8,7 @@
  *   s2s_whisper_*   <- processor(...) + model.generate(...)            S/STT/whisper_stt_handler.py:83-87, 166-197, 243
  *   s2s_llama_*     <- pipeline("text-generation")(prompt, ...)        S/LLM/language_model.py:800-892
  *   s2s_tts_*       <- _resample_to_pipeline_sr/_to_int16/_stream      S/TTS/qwen3_tts_handler.py:612-613, 674-680, 695-749
- *   (S/ = /root/reference/src/speech_to_speech)
+ *   (S/ = src/speech_to_speech of huggingface/speech-to-speech)
  *
  * Conventions: plain pointers and sizes only; every call returns 0 on success or a negative
  * S2S_ERR_* code (message via s2s_last_error(), thread-local).  Pointers suffixed _d are
@@ -46,7 +46,7 @@ typedef struct s2s_llama s2s_llama;
 int s2s_init(int device, s2s_ctx** out);
 int s2s_destroy(s2s_ctx* ctx);
 /* SM partition ("lane") of a context: the persistent cooperative decode kernels of the models created on `ctx` use `ctas`
- * CTAs (0 = one per SM, the default).  Contexts with disjoint partitions (e.g. two of 74 CTAs on a 148-SM B200), driven
+ * CTAs (0 = one per SM, the default).  Contexts with disjoint partitions (e.g. two of 66 CTAs on a 132-SM H100), driven
  * from different CUDA streams, run their decode launches concurrently; a decode step is a chain of latency-bound phases, so
  * two half-grid launches take about as long as one whole-grid launch.  No reference counterpart (the reference runs one
  * session per model call). */
@@ -124,7 +124,7 @@ int s2s_whisper_transcribe(s2s_whisper* m, const s2s_whisper_decode_opts* opts, 
                            int32_t* len_out_h, void* stream);
 
 /* ---- generic GEMM (exposed for tests / roofline benches) --------------------------------
- * C[M,N] = A[M,K] * W[N,K]^T (+bias), tcgen05 + TMA; dtype S2S_F16 or S2S_BF16, fp32 accumulate.
+ * C[M,N] = A[M,K] * W[N,K]^T (+bias), wgmma + TMA; dtype S2S_F16 or S2S_BF16, fp32 accumulate.
  * out_dtype: S2S_F32 or same as dtype.  act: 0 none, 1 exact GELU.                          */
 int s2s_gemm(s2s_ctx* ctx, const void* a_d, const void* w_d, const float* bias_d, void* c_d, int32_t M,
              int32_t N, int32_t K, int32_t dtype, int32_t out_dtype, int32_t act, void* stream);

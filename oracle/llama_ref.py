@@ -1,6 +1,6 @@
 """numpy restatement of the Llama-family arithmetic on the reference's LLM path (TEST INFRASTRUCTURE).
 
-The reference (`/root/reference/src/speech_to_speech/LLM/language_model.py:800-892`) runs
+The reference (`speech_to_speech/LLM/language_model.py:800-892`) runs
 `pipeline("text-generation")` over `AutoModelForCausalLM`; the math lives in transformers
 (TF = site-packages/transformers/models/llama/modeling_llama.py):
 

@@ -1,5 +1,5 @@
 """TTS post-processing oracle (TEST INFRASTRUCTURE): the exact calls Qwen3TTSHandler._stream makes
-(/root/reference/src/speech_to_speech/TTS/qwen3_tts_handler.py:612-613, 674-680, 695-749) -- scipy's
+(speech_to_speech/TTS/qwen3_tts_handler.py:612-613, 674-680, 695-749) -- scipy's
 resample_poly is the reference implementation itself, so this oracle is pinned by construction; the
 restatement `resample_direct` documents the arithmetic the CUDA kernel follows and is checked against scipy."""
 from __future__ import annotations

@@ -1,6 +1,6 @@
 """numpy restatement of the Whisper arithmetic on the reference's STT path (TEST INFRASTRUCTURE).
 
-The reference (`/root/reference/src/speech_to_speech/STT/whisper_stt_handler.py:83-87, 225-282`)
+The reference (`speech_to_speech/STT/whisper_stt_handler.py:83-87, 225-282`)
 delegates to `transformers` (pinned >=4.57; 5.5.0 installed).  Each function cites the
 transformers file it restates (TF = site-packages/transformers/models/whisper):
 

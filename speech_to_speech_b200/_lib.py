@@ -88,7 +88,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise ImportError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a).  speech_to_speech_b200 has no CPU fallback."
+            "(nvcc, sm_90a).  speech_to_speech_b200 has no CPU fallback."
         )
     lib = C.CDLL(LIB_PATH)
     lib.s2s_last_error.restype = C.c_char_p

@@ -3,7 +3,7 @@ requests are merged into one launch.
 
 Why (SURVEY.md §8f rank 1): the reference gives every pipeline unit its own handler threads and its own model copy
 (`s2s_pipeline.py:554-565`, `--num_pipelines`, `arguments_classes/module_arguments.py:85-93`), so N sessions cost
-N weight sets and N independent per-token weight streams.  On the B200 path the decode kernel processes up to 16
+N weight sets and N independent per-token weight streams.  On the GPU path the decode kernel processes up to 16
 sessions per persistent launch at almost the cost of one (the batch is the m dimension of the tensor-core tile,
 csrc/decode_common.cuh): measured 1030 concurrent real-time Whisper-small sessions per GPU at 16 per launch
 against 121 one at a time.  The batcher is the host piece that makes that reachable from the handler slots:

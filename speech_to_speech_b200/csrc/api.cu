@@ -34,8 +34,8 @@ int s2s_init(int device, s2s_ctx** out) {
   S2S_CHECK_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   S2S_CHECK_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    s2s_set_error("s2s_init: device %d is sm_%d%d; this library is built for sm_100a (B200) only", device, prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    s2s_set_error("s2s_init: device %d is sm_%d%d; this library is built for sm_90a (Hopper, H100) only", device, prop.major,
                   prop.minor);
     return S2S_ERR_UNSUPPORTED;
   }
@@ -83,7 +83,7 @@ int s2s_attention(s2s_ctx* ctx, const void* q_d, const void* k_d, const void* v_
                   int32_t Tk, int32_t heads, int32_t kv_heads, int32_t hd, int64_t ldq, int64_t ldk, int64_t ldv,
                   int64_t ldo, float scale, int32_t causal, int32_t dtype, void* stream) {
   S2S_REQUIRE(ctx && q_d && k_d && v_d && o_d, "s2s_attention: null argument");
-  // test / bench entry point: the V^T scratch of the tcgen05 kernel is allocated per call here (the models own theirs)
+  // test / bench entry point: the V^T scratch of the attention kernel is allocated per call here (the models own theirs)
   const size_t elems = attention_tc_scratch_elems(B, Tk, kv_heads, hd);
   void* vt = nullptr;
   S2S_CHECK_CUDA(cudaMalloc(&vt, elems * 2));

@@ -1,26 +1,27 @@
-// attention_tc.cu -- fused softmax(Q K^T) V on the 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// attention_tc.cu -- fused softmax(Q K^T) V on Hopper tensor cores (wgmma + TMA).
 //
-// One CTA = 128 query rows of one head.  Per 64-key tile:
-//   S = Q K^T        tcgen05.mma  M=128 N=64  K=hd     (Q, K tiles in shared memory via TMA, S in TMEM cols [0,64))
-//   softmax          4 warps, one query row per thread: tcgen05.ld S -> registers, mask, online max/sum (exp2, fp32),
-//                    P (16-bit) written to shared memory in the K-major 128-byte-swizzled operand layout,
-//                    O (TMEM cols [64, 64+hd)) rescaled in place with tcgen05.ld / tcgen05.st
-//   O += P V         tcgen05.mma  M=128 N=hd  K=64      (V^T tile [hd, 64 keys] in shared memory via TMA)
-// Warp roles (192 threads): warps 0-3 softmax/epilogue (TMEM lane group = warp id), warp 4 TMA producer,
-// warp 5 TMEM allocator + MMA issuer.  K/V tiles are double buffered; S(t+1) is issued while softmax(t) runs.
-// V is consumed as V^T (K-major B operand), produced once per call by a small transpose kernel into a
-// caller-owned scratch [B, kv_heads, hd, Tpad].
+// One CTA = 128 query rows of one head; two MMA warpgroups own 64 query rows each.  Per 64-key tile:
+//   S = Q K^T        wgmma m64 n64 k16 x hd/16, Q and K tiles in shared memory (TMA, 128-byte swizzle), S in registers
+//   softmax          in registers: a query row lives in one quad of lanes (online max/sum in fp32, exp2), the
+//                    accumulators O are rescaled in place
+//   O += P V         wgmma m64 n=hd k16 x 4 with P (16-bit) as the register A operand and the V^T tile
+//                    [hd, 64 keys] in shared memory (TMA)
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = MMA + softmax + epilogue.
+// K/V tiles are double buffered.  V is consumed as V^T (K-major B operand), produced once per call by a small
+// transpose kernel into a caller-owned scratch [B, kv_heads, hd, Tpad].
 // Reference ops: transformers modeling_whisper.py:215-239 (eager_attention_forward, encoder: non-causal 1500x1500),
 // modeling_llama.py:187-222 (causal GQA, prefill).
 #include "common.cuh"
 #include "gemm_tc.cuh"
 #include "kernels.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int QM = 128;  // queries per CTA
 constexpr int KN = 64;   // keys per tile
-constexpr int ATC_THREADS = 192;
+constexpr int ATC_THREADS = 384;
+constexpr int ATC_CONSUMERS = 256;
 
 struct AtcParams {
   void* o;
@@ -30,28 +31,13 @@ struct AtcParams {
   int causal_off;  // query i sees keys <= i + causal_off
 };
 
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
 template <int HD> struct AtcSmem {
   static constexpr int Q_BYTES = QM * HD * 2;
   static constexpr int K_BYTES = KN * HD * 2;   // per stage
   static constexpr int V_BYTES = HD * KN * 2;   // per stage
-  static constexpr int P_BYTES = QM * KN * 2;
   static constexpr int OFF_K = Q_BYTES;
   static constexpr int OFF_V = OFF_K + 2 * K_BYTES;
-  static constexpr int OFF_P = OFF_V + 2 * V_BYTES;
-  static constexpr int OFF_BAR = OFF_P + P_BYTES;
+  static constexpr int OFF_BAR = OFF_V + 2 * V_BYTES;
   static constexpr int TOTAL = OFF_BAR + 256 + 1024;
 };
 
@@ -66,18 +52,12 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
   uint8_t* sQ = smem;
   uint8_t* sK = smem + L::OFF_K;
   uint8_t* sV = smem + L::OFF_V;
-  uint8_t* sP = smem + L::OFF_P;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L::OFF_BAR);
   uint64_t* q_full = bars + 0;
   uint64_t* kv_full = bars + 1;   // [2]
   uint64_t* kv_empty = bars + 3;  // [2]
-  uint64_t* s_full = bars + 5;
-  uint64_t* s_free = bars + 6;
-  uint64_t* p_ready = bars + 7;
-  uint64_t* o_done = bars + 8;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int q0 = blockIdx.x * QM, h = blockIdx.y, b = blockIdx.z;
   const int kvh = h / (p.heads / p.kv_heads);
 
@@ -88,28 +68,18 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
     if (n_tiles < 1) n_tiles = 1;
   }
 
-  if (warp == 4 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_q); tma_prefetch_desc(&map_k); tma_prefetch_desc(&map_vt);
     mbar_init(q_full, 1);
     mbar_init(&kv_full[0], 1); mbar_init(&kv_full[1], 1);
-    mbar_init(&kv_empty[0], 1); mbar_init(&kv_empty[1], 1);
-    mbar_init(s_full, 1);
-    mbar_init(s_free, 128);
-    mbar_init(p_ready, 128);
-    mbar_init(o_done, 1);
+    mbar_init(&kv_empty[0], ATC_CONSUMERS); mbar_init(&kv_empty[1], ATC_CONSUMERS);
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc<256>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base;        // columns [0, 64)
-  const uint32_t tmem_O = tmem_base + 64;   // columns [64, 64 + HD)
 
-  if (warp == 4) {
+  if (wg == 0) {
     // ============================== TMA producer ==============================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       mbar_expect_tx(q_full, L::Q_BYTES);
 #pragma unroll
       for (int kk = 0; kk < KK; ++kk) tma_load_2d(sQ + kk * (QM * 128), &map_q, q_full, h * HD + kk * 64, b * p.Tq + q0);
@@ -123,137 +93,97 @@ attn_tc_kernel(const __grid_constant__ CUtensorMap map_q, const __grid_constant_
         tma_load_3d(sV + s * L::V_BYTES, &map_vt, &kv_full[s], t * KN, 0, b * p.kv_heads + kvh);
       }
     }
-  } else if (warp == 5) {
-    // ============================== MMA issuer (one thread) ==============================
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = umma_idesc_f16(DT<T>::umma_fmt, QM, KN);
-      constexpr uint32_t idesc_o = umma_idesc_f16(DT<T>::umma_fmt, QM, HD);
-      auto issue_s = [&](int t) {
-        const int s = t & 1;
-        mbar_wait(&kv_full[s], (t >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < KK; ++kk) {
-          const uint64_t ad = umma_smem_desc_sw128(smem_u32(sQ + kk * (QM * 128)));
-          const uint64_t bd = umma_smem_desc_sw128(smem_u32(sK + s * L::K_BYTES + kk * (KN * 128)));
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma_f16(tmem_S, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc_s, (kk | k) != 0);
-        }
-        umma_commit(s_full);
-      };
-      mbar_wait(q_full, 0);
-      issue_s(0);
-      for (int t = 0; t < n_tiles; ++t) {
-        const int s = t & 1;
-        if (t + 1 < n_tiles) {
-          mbar_wait(s_free, t & 1);  // softmax(t) holds S(t) in registers: the S columns may be overwritten
-          issue_s(t + 1);
-        }
-        mbar_wait(p_ready, t & 1);   // P(t) is in shared memory, O has been rescaled
-        tc_fence_after();
-        const uint64_t ad = umma_smem_desc_sw128(smem_u32(sP));
-        const uint64_t bd = umma_smem_desc_sw128(smem_u32(sV + s * L::V_BYTES));
-#pragma unroll
-        for (int k = 0; k < 4; ++k) umma_f16(tmem_O, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc_o, (t | k) != 0);
-        umma_commit(o_done);
-        umma_commit(&kv_empty[s]);
-      }
-    }
-  } else {
-    // ============================== softmax + epilogue: one query row per thread ==============================
-    const int row = warp * 32 + lane;          // TMEM lane == query row inside the tile
-    const int q = q0 + row;                    // query index inside the sequence
-    const uint32_t lane_sel = (uint32_t)(warp * 32) << 16;
-    float m = -INFINITY, l = 0.f;
-    for (int t = 0; t < n_tiles; ++t) {
-      mbar_wait(s_full, t & 1);
-      tc_fence_after();
-      uint32_t sr[2][32];
-      tmem_ld_32x32(tmem_S + lane_sel + 0, sr[0]);
-      tmem_ld_32x32(tmem_S + lane_sel + 32, sr[1]);
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(s_free);
-      float mx = -INFINITY;
-      const int kbase = t * KN;
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const int key = kbase + hh * 32 + j;
-          bool ok = key < p.Tk;
-          if (CAUSAL) ok = ok && (key <= q + p.causal_off);
-          const float v = ok ? __uint_as_float(sr[hh][j]) * p.scale_log2 : -INFINITY;
-          sr[hh][j] = __float_as_uint(v);
-          mx = fmaxf(mx, v);
-        }
-      const float m_new = fmaxf(m, mx);
-      const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-      const float corr = exp2f(m - m_use);  // m = -inf -> 0
-      float rs = 0.f;
-      uint32_t pk[32];  // 64 probabilities packed 2 x 16-bit
-#pragma unroll
-      for (int hh = 0; hh < 2; ++hh)
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          const float p0 = exp2f(__uint_as_float(sr[hh][j]) - m_use);
-          const float p1 = exp2f(__uint_as_float(sr[hh][j + 1]) - m_use);
-          rs += p0 + p1;
-          pk[hh * 16 + (j >> 1)] = DT<T>::pack2(p0, p1);
-        }
-      l = l * corr + rs;
-      m = m_new;
-      if (t > 0) {
-        mbar_wait(o_done, (t - 1) & 1);  // PV(t-1) finished: P buffer free, O stable
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < HD / 32; ++c) {
-          uint32_t orr[32];
-          tmem_ld_32x32(tmem_O + lane_sel + c * 32, orr);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) orr[j] = __float_as_uint(__uint_as_float(orr[j]) * corr);
-          tmem_st_32x32(tmem_O + lane_sel + c * 32, orr);
-        }
-        tmem_st_wait();
-      }
-      // P row -> shared memory, K-major 128-byte swizzle: 16-byte chunk c of row r lives at chunk (c ^ (r & 7))
-      uint8_t* prow = sP + row * 128;
-#pragma unroll
-      for (int c = 0; c < 8; ++c)
-        *reinterpret_cast<uint4*>(prow + ((c ^ (row & 7)) << 4)) = make_uint4(pk[c * 4], pk[c * 4 + 1], pk[c * 4 + 2], pk[c * 4 + 3]);
-      fence_proxy_async();  // generic-proxy writes -> visible to the tensor core's async-proxy reads
-      tc_fence_before();
-      mbar_arrive(p_ready);
-    }
-    // ---- epilogue: O / l -> 16-bit global ----
-    mbar_wait(o_done, (n_tiles - 1) & 1);
-    tc_fence_after();
-    const float inv = l > 0.f ? 1.f / l : 0.f;
-    T* orow = reinterpret_cast<T*>(p.o) + ((long long)b * p.Tq + q) * p.ldo + (long long)h * HD;
-#pragma unroll 1
-    for (int c = 0; c < HD / 32; ++c) {
-      uint32_t orr[32];
-      tmem_ld_32x32(tmem_O + lane_sel + c * 32, orr);
-      tmem_ld_wait();
-      if (q < p.Tq) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 8) {
-          uint4 w;
-          w.x = DT<T>::pack2(__uint_as_float(orr[j]) * inv, __uint_as_float(orr[j + 1]) * inv);
-          w.y = DT<T>::pack2(__uint_as_float(orr[j + 2]) * inv, __uint_as_float(orr[j + 3]) * inv);
-          w.z = DT<T>::pack2(__uint_as_float(orr[j + 4]) * inv, __uint_as_float(orr[j + 5]) * inv);
-          w.w = DT<T>::pack2(__uint_as_float(orr[j + 6]) * inv, __uint_as_float(orr[j + 7]) * inv);
-          *reinterpret_cast<uint4*>(orow + c * 32 + j) = w;
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc<256>(tmem_base);
+
+  // ============================== MMA warpgroups: query rows [64 cw, 64 cw + 64) ==============================
+  const int cw = wg - 1;
+  const int tid = threadIdx.x & 127, w = tid >> 5, l = tid & 31;
+  const int r0 = q0 + cw * 64 + w * 16 + (l >> 2);  // this thread's two query rows: r0 and r0 + 8
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, lsum[2] = {0.f, 0.f};  // lsum: this thread's share of the row sum
+  mbar_wait(q_full, 0);
+  for (int t = 0; t < n_tiles; ++t) {
+    const int s = t & 1;
+    mbar_wait(&kv_full[s], (t >> 1) & 1);
+    // ---- S = Q K^T ----
+    float sacc[KN / 2];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < KK; ++kk) {
+      const uint64_t ad = wgmma_desc_sw128(smem_u32(sQ + kk * (QM * 128) + cw * (64 * 128)));
+      const uint64_t bd = wgmma_desc_sw128(smem_u32(sK + s * L::K_BYTES + kk * (KN * 128)));
+#pragma unroll
+      for (int k = 0; k < 4; ++k) wgmma_ss<T, KN>(sacc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), (kk | k) != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(sacc);
+    // ---- online softmax ----
+    const int kbase = t * KN + 2 * (l & 3);
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < KN / 2; ++i) {
+      const int key = kbase + (i >> 2) * 8 + (i & 1), hr = (i >> 1) & 1;
+      bool ok = key < p.Tk;
+      if (CAUSAL) ok = ok && (key <= r0 + hr * 8 + p.causal_off);
+      sacc[i] = ok ? sacc[i] * p.scale_log2 : -INFINITY;
+      mx[hr] = fmaxf(mx[hr], sacc[i]);
+    }
+    float corr[2], m_use[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 1));
+      mx[hr] = fmaxf(mx[hr], __shfl_xor_sync(0xffffffffu, mx[hr], 2));
+      const float m_new = fmaxf(m[hr], mx[hr]);
+      m_use[hr] = (m_new == -INFINITY) ? 0.f : m_new;
+      corr[hr] = exp2f(m[hr] - m_use[hr]);  // m = -inf -> 0
+      m[hr] = m_new;
+      lsum[hr] *= corr[hr];
+    }
+    uint32_t pk[KN / 4];  // P packed 2 x 16-bit, in the accumulator order = the A-operand order of the next product
+#pragma unroll
+    for (int i = 0; i < KN / 2; i += 2) {
+      const int hr = (i >> 1) & 1;
+      const float p0 = exp2f(sacc[i] - m_use[hr]), p1 = exp2f(sacc[i + 1] - m_use[hr]);
+      lsum[hr] += p0 + p1;
+      pk[i >> 1] = DT<T>::pack2(p0, p1);
+    }
+#pragma unroll
+    for (int i = 0; i < HD / 2; ++i) o[i] *= corr[(i >> 1) & 1];
+    // ---- O += P V ----
+    const uint64_t vd = wgmma_desc_sw128(smem_u32(sV + s * L::V_BYTES));
+    wgmma_fence_operand(o);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KN / 16; ++k) {
+      const uint32_t a[4] = {pk[4 * k], pk[4 * k + 1], pk[4 * k + 2], pk[4 * k + 3]};
+      wgmma_rs<T, HD>(o, a, vd + (uint64_t)(k * 2), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_operand(o);
+    mbar_arrive(&kv_empty[s]);
+  }
+  // ---- epilogue: O / l -> 16-bit global ----
+  float inv[2];
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    float lt = lsum[hr];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    inv[hr] = lt > 0.f ? 1.f / lt : 0.f;
+  }
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int q = r0 + hr * 8;
+    if (q >= p.Tq) continue;
+    T* orow = reinterpret_cast<T*>(p.o) + ((long long)b * p.Tq + q) * p.ldo + (long long)h * HD + 2 * (l & 3);
+#pragma unroll
+    for (int j = 0; j < HD / 8; ++j)
+      *reinterpret_cast<uint32_t*>(orow + j * 8) = DT<T>::pack2(o[4 * j + 2 * hr] * inv[hr], o[4 * j + 2 * hr + 1] * inv[hr]);
   }
 }
 

@@ -18,7 +18,7 @@
 //   transposed conv, k = s           : a 1-tap contraction with N = s * C_out
 //   linear layers (transformer, ConvNeXt MLP): 1 tap.
 // fp32 CUDA-core FMA with shared-memory tiles: the decoder is held to 1e-4-level waveform parity with the fp32 oracle;
-// its cost is ~5 GFLOP per frame (DESIGN.md), far from the B200's limits at the session counts the talker sustains.
+// its cost is ~5 GFLOP per frame (DESIGN.md), far from the H100's limits at the session counts the talker sustains.
 #include <math.h>
 #include <string.h>
 
@@ -112,7 +112,7 @@ __global__ void __launch_bounds__(CV_THREADS) conv1d_f32_kernel(const ConvArgs a
 // mma.sync.m16n8k16, CTA tile 128 (time) x 64 (channels) x 32 (k), 8 warps as 4 x 2, warp tile 32 x 32.  The codec
 // decoder is ~5 GFLOP per frame and every chunk re-decodes its 25 frames of left context (chunked_decode): on the CUDA
 // cores it was the largest share of a turn (bench.py stage_ms), here it is weight- and activation-stream bound.
-// tcgen05 is not used: the operand is a strided gather of fp32 rows (dilated taps, causal zero rows) that has to be
+// wgmma is not used: the operand is a strided gather of fp32 rows (dilated taps, causal zero rows) that has to be
 // converted on the way in, which the generic-proxy staging path does and a TMA descriptor does not.
 constexpr int TC_BM = 128, TC_BN = 64, TC_BK = 32, TC_THREADS = 256;
 constexpr int TC_APAD = 8;     // halves: row stride 40 halves = 80 B -> conflict-free 32-bit fragment loads
@@ -560,7 +560,12 @@ int conv1d_f32_launch(const ConvArgs& a, cudaStream_t st) {
   const int batch = a.batch > 0 ? a.batch : 1;
   const int mt = (a.T_out - a.t0 + CV_BM - 1) / CV_BM;
   // few time tiles (transformer / first decoder stages): narrower n tiles put more SMs on the weight stream
-  if ((long long)mt * ((a.N + 63) / 64) * batch < 148) {
+  static const int num_sms = [] {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) n = 0;
+    return n;
+  }();
+  if ((long long)mt * ((a.N + 63) / 64) * batch < num_sms) {
     dim3 grid((a.N + 31) / 32, mt, batch);
     conv1d_f32_kernel<32><<<grid, CV_THREADS, 0, st>>>(a);
   } else {

@@ -1,4 +1,4 @@
-// common.cuh -- shared device/host helpers for libs2s_b200 (sm_100a only).
+// common.cuh -- shared device/host helpers for libs2s_b200 (sm_90a, Hopper).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
@@ -50,7 +50,7 @@ struct s2s_ctx {
   int device;
   int num_sms;
   // SM partition ("lane"): the persistent cooperative decode kernels launched through this context use this many CTAs
-  // (0 = one per SM).  Two contexts of 74 CTAs each run their decode launches side by side on one GPU: the phases of a
+  // (0 = one per SM).  Two contexts of half the SMs each run their decode launches side by side on one GPU: the phases of a
   // decode step are latency-bound, so two half-grid launches finish in about the time of one whole-grid launch.
   int decode_ctas;
   // cuTensorMapEncodeTiled resolved through the runtime (no link-time libcuda dependency)
@@ -86,7 +86,6 @@ inline int dec_grid(const s2s_ctx* c) { return (c->decode_ctas > 0 && c->decode_
 template <typename T> struct DT;
 template <> struct DT<__half> {
   static constexpr int code = S2S_F16;
-  static constexpr uint32_t umma_fmt = 0;  // F16
   static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   __device__ __forceinline__ static float to_f(__half v) { return __half2float(v); }
   __device__ __forceinline__ static __half from_f(float v) { return __float2half_rn(v); }
@@ -100,7 +99,6 @@ template <> struct DT<__half> {
 };
 template <> struct DT<__nv_bfloat16> {
   static constexpr int code = S2S_BF16;
-  static constexpr uint32_t umma_fmt = 1;  // BF16
   static constexpr CUtensorMapDataType tma = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
   __device__ __forceinline__ static float to_f(__nv_bfloat16 v) { return __bfloat162float(v); }
   __device__ __forceinline__ static __nv_bfloat16 from_f(float v) { return __float2bfloat16_rn(v); }
@@ -146,7 +144,7 @@ __device__ __forceinline__ uint4 ld_stream16(const void* p) {
 }
 
 // ------------------------------------------------------------------------------------------
-// mbarrier / TMA / tcgen05 PTX wrappers (sm_100a)
+// mbarrier / TMA PTX wrappers (sm_90a)
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
@@ -196,62 +194,4 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const void* desc, ui
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
       ::"r"(smem_u32(smem_dst)), "l"(desc), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
       : "memory");
-}
-
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-template <int NCOLS> __device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS> __device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem]^T ; kind::f16 covers fp16 and bf16 operands with fp32 accumulate
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// mbarrier arrives when all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp gets lane (base_lane + i)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// K-major, 128-byte-swizzled shared-memory operand descriptor (tile rows are 128 B = 64 x 16-bit,
-// 8-row groups 1024 B apart).  Field layout: cute/arch/mma_sm100_desc.hpp SmemDescriptor.
-__device__ __forceinline__ uint64_t umma_smem_desc_sw128(uint32_t smem_addr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);  // start address, bits [0,14)
-  d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
-  d |= (uint64_t)(1024u >> 4) << 32;             // stride byte offset: 8 rows x 128 B
-  d |= (uint64_t)1 << 46;                        // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                        // SWIZZLE_128B
-  return d;
-}
-// Instruction descriptor for kind::f16, fp32 accumulate, both operands K-major (InstrDescriptor).
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t fmt, uint32_t M, uint32_t N) {
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
 }

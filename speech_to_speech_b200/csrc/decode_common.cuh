@@ -38,10 +38,10 @@ __device__ __forceinline__ unsigned int ld_relaxed_gpu(const unsigned int* p) {
   asm volatile("ld.relaxed.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
-// Polling the counter costs one L2 round trip (~0.7 us) per sample; with a single load in flight the release is
+// Polling the counter costs one L2 round trip per sample; with a single load in flight the release is
 // noticed on average half a round trip late.  Thread 0 therefore keeps FOUR relaxed loads in flight, issued a
 // quarter round trip apart; the pipeline is self-clocking (each consumed load is re-issued at once), so the counter
-// is sampled every ~0.18 us.  After the successful sample thread 0 executes fence.acq_rel.gpu: relaxed load + fence is
+// is sampled several times per round trip.  After the successful sample thread 0 executes fence.acq_rel.gpu: relaxed load + fence is
 // the PTX acquire pattern, it synchronises with every producer's red.release, and the bar.sync that follows extends
 // the ordering to the CTA's other threads (causality order is transitive over barriers).  `relaxed` != 0 skips the
 // fence (A/B measurements only, S2S_SYNC_RELAXED=1): without it the cross-CTA reads race under the PTX memory model
@@ -354,7 +354,7 @@ struct GemvArgs {
 // epilogue of the row pair (row0, row0 + 1), row0 even, for session b.  v already carries the bias.
 // LLAMA selects which modes exist in the instantiation (smaller code per model family).  Kept inline: with ~220 KB of
 // the SM's 256 KB configured as shared memory the L1 data cache is tiny, so the stack traffic of a call (argument
-// struct, saved registers) goes to L2 -- measured +1 us per phase for a non-inlined epilogue / argument builder.
+// struct, saved registers) goes to L2 on every phase for a non-inlined epilogue / argument builder.
 template <typename T, bool LLAMA>
 __device__ __forceinline__ void gemv_pair_epilogue(const GemvArgs& a, int mode, int row0, int b, float v0, float v1,
                                                    float r0, float r1, int sup0, int sup1, float& best_v, int& best_i) {
@@ -411,7 +411,7 @@ __device__ __forceinline__ void gemv_pair_epilogue(const GemvArgs& a, int mode, 
 // ---- weight streaming through a per-warp shared-memory ring filled by the bulk-copy engine ---------------
 // Each warp owns `slots` slots of GV_ROWS x GV_UK 16-bit weights.  Lane 0 issues ONE cp.async.bulk per unit
 // (global -> shared, completion on the slot's mbarrier; one request per 4 KB keeps the per-SM copy engine far from
-// its request-rate limit -- 512-byte row copies measured 25 % slower); the warp then feeds the tensor core from
+// its request-rate limit, which 512-byte row copies approach); the warp then feeds the tensor core from
 // shared memory.  Bytes in flight are bounded by shared memory (16 KB per warp), not by registers, and the copies
 // are not droppable hints.  The warp is its own producer and consumer, so no cross-warp synchronisation is needed:
 // slot reuse is ordered by program order + __syncwarp + fence.proxy.async.

@@ -1,28 +1,27 @@
-// gemm_tc.cu -- C = A * W^T on Blackwell 5th-gen tensor cores.
+// gemm_tc.cu -- C = A * W^T on Hopper tensor cores (wgmma).
 //
 //   * operands: 16-bit (fp16 / bf16), K-major, staged global->shared by TMA (cp.async.bulk.tensor,
 //     128-byte swizzle) through a STAGES-deep mbarrier ring;
-//   * math: tcgen05.mma.cta_group::1.kind::f16, M=128 x N=BN x K=16 per instruction, issued by ONE
-//     thread; the fp32 accumulator tile lives in TMEM (BN columns x 128 lanes);
-//   * epilogue: 4 warps read TMEM with tcgen05.ld (32 lanes x 32 columns per instruction) and fuse
-//     bias, exact GELU, fp32 residual add (in-place residual stream or broadcast positional table)
-//     and the 16-bit / fp32 stores.
+//   * math: wgmma.mma_async m64 x N=BN x k16 from shared-memory descriptors, fp32 accumulators in registers;
+//     each of the two consumer warpgroups owns 64 rows of the 128-row tile and keeps one k-block of MMAs in flight;
+//   * epilogue: straight from the accumulator registers, fused bias, exact GELU, SwiGLU, fp32 residual add
+//     (in-place residual stream or broadcast positional table) and the 16-bit / fp32 stores.
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2..5 = epilogue (TMEM lane group = warp_id % 4).
+// Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = MMA + epilogue.
 //
 // Used for every GEMM-shaped op with M >= 64 on the hot path: Whisper conv1/conv2 (as strided-window
 // GEMMs, no im2col), QKV / out-proj / fc1 / fc2 of the encoder, the cross-attention K/V projection and
 // the LLM prefill projections.  (Reference ops: transformers modeling_whisper.py:284-357,380-414,619-625;
 // modeling_llama.py:171-289.)
 #include "gemm_tc.cuh"
+#include "wgmma.cuh"
 
 namespace {
 
 constexpr int BM = 128;
 constexpr int BK = 64;  // 64 x 16-bit = 128 B = one swizzle atom
-constexpr int UMMA_K = 16;
-constexpr int NTHREADS = 192;
+constexpr int NTHREADS = 384;
+constexpr int CONSUMERS = 256;  // threads of the two MMA warpgroups
 
 template <int BN> struct TileCfg {
   static constexpr int STAGES = (BN == 64) ? 8 : 6;
@@ -30,7 +29,6 @@ template <int BN> struct TileCfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static constexpr int TMEM_COLS = (BN < 32) ? 32 : BN;
 };
 
 struct EpiParams {
@@ -49,43 +47,68 @@ struct EpiParams {
   int M, N, K;
 };
 
+// two adjacent output columns (n, n + 1) of row m
+template <typename T>
+__device__ __forceinline__ void epilogue_pair(const EpiParams& ep, int batch, int m, int n, float v0, float v1) {
+  if (m >= ep.M) return;
+  const long long orow = (long long)batch * ep.out_batch_rows + ep.out_row_offset + m;
+  if (ep.bias) {
+    const float2 b2 = *reinterpret_cast<const float2*>(ep.bias + n);
+    v0 += b2.x; v1 += b2.y;
+  }
+  if (ep.act == 1) { v0 = gelu_erf(v0); v1 = gelu_erf(v1); }
+  if (ep.act == 2) {
+    // SwiGLU over interleaved (gate, up) columns: out[n/2] = silu(v[n]) * v[n+1]; 16-bit output, ld = N/2
+    reinterpret_cast<T*>(ep.out_h)[orow * ep.ldo_h + (n >> 1)] = DT<T>::from_f((v0 / (1.0f + __expf(-v0))) * v1);
+    return;
+  }
+  if (ep.out_f) {
+    if (ep.resid) {
+      const long long rrow = (ep.resid_mode == 2) ? (long long)m : orow;
+      const float2 q = *reinterpret_cast<const float2*>(ep.resid + rrow * ep.ld_resid + n);
+      v0 += q.x; v1 += q.y;
+    }
+    *reinterpret_cast<float2*>(ep.out_f + orow * ep.ldo_f + n) = make_float2(v0, v1);
+  }
+  if (ep.out_h) {
+    T* dst = reinterpret_cast<T*>(ep.out_h) + orow * ep.ldo_h + n;
+    if (ep.head_major_rows > 0) {
+      const long long ob = orow / ep.head_major_rows, ot = orow - ob * ep.head_major_rows;
+      dst = reinterpret_cast<T*>(ep.out_h) + ((ob * (ep.N >> 6) + (n >> 6)) * ep.head_major_rows + ot) * 64 + (n & 63);
+    }
+    *reinterpret_cast<uint32_t*>(dst) = DT<T>::pack2(v0, v1);
+  }
+}
+
 template <typename T, int BN>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
                const EpiParams ep) {
   using Cfg = TileCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
-  // 1024-byte alignment is required by the 128-byte swizzle pattern (TMA and UMMA must agree)
+  // 1024-byte alignment is required by the 128-byte swizzle pattern (TMA and wgmma must agree)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + Cfg::STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
   const int n_tile = blockIdx.x, m_tile = blockIdx.y, batch = blockIdx.z;
   const int num_kb = (ep.K + BK - 1) / BK;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_w);
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], CONSUMERS);
     }
-    mbar_init(tmem_full_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
+  if (wg == 0) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
+    if (threadIdx.x == 0) {
       for (int kb = 0; kb < num_kb; ++kb) {
         const int s = kb % Cfg::STAGES;
         const uint32_t ph = (kb / Cfg::STAGES) & 1;
@@ -97,116 +120,41 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         tma_load_2d(sb, &map_w, &full_bar[s], kb * BK, n_tile * BN);
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one thread) =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc = umma_idesc_f16(DT<T>::umma_fmt, BM, BN);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % Cfg::STAGES;
-        const uint32_t ph = (kb / Cfg::STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES);
-        const uint32_t sb = sa + Cfg::A_BYTES;
-        const uint64_t adesc = umma_smem_desc_sw128(sa);
-        const uint64_t bdesc = umma_smem_desc_sw128(sb);
-#pragma unroll
-        for (int k = 0; k < BK / UMMA_K; ++k) {
-          // advancing K inside the 128-byte swizzle atom = +32 B on the start address (>>4 => +2)
-          umma_f16(tmem_base, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), idesc, (kb | k) != 0);
-        }
-        umma_commit(&empty_bar[s]);  // frees the smem stage when these MMAs retire
-      }
-      umma_commit(tmem_full_bar);    // accumulator complete
-    }
-  } else {
-    // ===================== epilogue: TMEM -> registers -> global =====================
-    const int lg = warp & 3;  // TMEM lane group this warp may access
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const int m = m_tile * BM + lg * 32 + lane;
-    const bool valid = m < ep.M;
-    const long long orow = (long long)batch * ep.out_batch_rows + ep.out_row_offset + m;
-    const long long rrow = (ep.resid_mode == 2) ? (long long)m : orow;
-#pragma unroll 1
-    for (int c = 0; c < BN / 32; ++c) {
-      uint32_t r[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(lg * 32) << 16) + (uint32_t)(c * 32), r);
-      tmem_ld_wait();
-      const int n0 = n_tile * BN + c * 32;
-      if (valid) {
-        float v[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-        if (ep.bias) {
-#pragma unroll
-          for (int j = 0; j < 32; j += 4) {
-            const float4 b4 = *reinterpret_cast<const float4*>(ep.bias + n0 + j);
-            v[j] += b4.x; v[j + 1] += b4.y; v[j + 2] += b4.z; v[j + 3] += b4.w;
-          }
-        }
-        if (ep.act == 1) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = gelu_erf(v[j]);
-        }
-        if (ep.act == 2) {
-          // SwiGLU over interleaved (gate, up) columns: out[n/2] = silu(v[2i]) * v[2i+1]; 16-bit output, ld = N/2
-          T* dst = reinterpret_cast<T*>(ep.out_h) + orow * ep.ldo_h + (n0 >> 1);
-          float o[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const float gte = v[2 * j];
-            o[j] = (gte / (1.0f + __expf(-gte))) * v[2 * j + 1];
-          }
-#pragma unroll
-          for (int j = 0; j < 16; j += 8) {
-            uint4 q;
-            q.x = DT<T>::pack2(o[j], o[j + 1]);
-            q.y = DT<T>::pack2(o[j + 2], o[j + 3]);
-            q.z = DT<T>::pack2(o[j + 4], o[j + 5]);
-            q.w = DT<T>::pack2(o[j + 6], o[j + 7]);
-            *reinterpret_cast<uint4*>(dst + j) = q;
-          }
-          continue;
-        }
-        if (ep.out_f) {
-          float* dst = ep.out_f + orow * ep.ldo_f + n0;
-          if (ep.resid) {
-            const float* rs = ep.resid + rrow * ep.ld_resid + n0;
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-              const float4 q = *reinterpret_cast<const float4*>(rs + j);
-              v[j] += q.x; v[j + 1] += q.y; v[j + 2] += q.z; v[j + 3] += q.w;
-            }
-          }
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(dst + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-        }
-        if (ep.out_h) {
-          T* dst = reinterpret_cast<T*>(ep.out_h) + orow * ep.ldo_h + n0;
-          if (ep.head_major_rows > 0) {
-            const long long ob = orow / ep.head_major_rows, ot = orow - ob * ep.head_major_rows;
-            dst = reinterpret_cast<T*>(ep.out_h) + ((ob * (ep.N >> 6) + (n0 >> 6)) * ep.head_major_rows + ot) * 64 + (n0 & 63);
-          }
-#pragma unroll
-          for (int j = 0; j < 32; j += 8) {
-            uint4 q;
-            q.x = DT<T>::pack2(v[j], v[j + 1]);
-            q.y = DT<T>::pack2(v[j + 2], v[j + 3]);
-            q.z = DT<T>::pack2(v[j + 4], v[j + 5]);
-            q.w = DT<T>::pack2(v[j + 6], v[j + 7]);
-            *reinterpret_cast<uint4*>(dst + j) = q;
-          }
-        }
-      }
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+
+  // ===================== MMA warpgroups: rows [64 cw, 64 cw + 64) of the tile =====================
+  const int cw = wg - 1;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  for (int kb = 0; kb < num_kb; ++kb) {
+    const int s = kb % Cfg::STAGES;
+    mbar_wait(&full_bar[s], (kb / Cfg::STAGES) & 1);
+    const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128);
+    const uint32_t sb = smem_u32(smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+    const uint64_t adesc = wgmma_desc_sw128(sa);
+    const uint64_t bdesc = wgmma_desc_sw128(sb);
+    wgmma_fence_operand(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) wgmma_ss<T, BN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1u);
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage may be refilled
+    wgmma_fence_operand(acc);
+    if (kb > 0) mbar_arrive(&empty_bar[(kb - 1) % Cfg::STAGES]);
+  }
+  wgmma_wait<0>();
+  wgmma_fence_operand(acc);
+
+  // ===================== epilogue: registers -> global =====================
+  const int t = threadIdx.x & 127, w = t >> 5, l = t & 31;
+  const int m0 = m_tile * BM + cw * 64 + w * 16 + (l >> 2);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = n_tile * BN + j * 8 + 2 * (l & 3);
+    epilogue_pair<T>(ep, batch, m0, n, acc[4 * j], acc[4 * j + 1]);
+    epilogue_pair<T>(ep, batch, m0 + 8, n, acc[4 * j + 2], acc[4 * j + 3]);
   }
 }
 
@@ -282,7 +230,7 @@ int gemm_tc_launch(s2s_ctx* ctx, const GemmProblem& p, int dtype, cudaStream_t s
   S2S_REQUIRE((reinterpret_cast<uintptr_t>(p.a) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.w) & 15) == 0,
               "gemm: operands must be 16-byte aligned");
   S2S_REQUIRE(p.M > 0 && p.batch > 0, "gemm: empty problem");
-  // Pick the N tile so the grid covers the 148 SMs when the problem allows it.
+  // Pick the N tile so the grid covers every SM when the problem allows it.
   const long long tiles128 = (long long)(p.N / 128) * ((p.M + BM - 1) / BM) * p.batch;
   const bool use128 = (p.N % 128 == 0) && tiles128 >= ctx->num_sms;
   if (dtype == S2S_F16) {

@@ -1,8 +1,8 @@
-// gemm_tc.cuh -- host interface of the tcgen05 + TMA GEMM (see gemm_tc.cu).
+// gemm_tc.cuh -- host interface of the wgmma + TMA GEMM (see gemm_tc.cu).
 #pragma once
 #include "common.cuh"
 
-// C[b, m, n] = epilogue( sum_k A[b, m, k] * W[n, k] ), A and W K-major 16-bit, fp32 accumulate in TMEM.
+// C[b, m, n] = epilogue( sum_k A[b, m, k] * W[n, k] ), A and W K-major 16-bit, fp32 accumulate in registers.
 // A is addressed through a 3-D TMA map (k, row, batch) so that convolution windows
 // (overlapping rows: row stride < row length) need no im2col.
 struct GemmProblem {

@@ -14,7 +14,7 @@ int logmel_launch(const LogmelTables& tb, const float* pcm_d, long long pcm_stri
 int logmel_finalize_launch(const float* src, const float* mel_max, int normalize, int B, int n_mels, float* dst_f32,
                            void* mel_t, int dtype, cudaStream_t stream);
 
-// ---- attention_tc.cu (tcgen05 / TMEM / TMA) ----
+// ---- attention_tc.cu (wgmma / TMA) ----
 size_t attention_tc_scratch_elems(int B, int Tk, int kv_heads, int hd);  // 16-bit elements of V^T scratch
 int attention_tc_launch(s2s_ctx* ctx, const void* q, const void* k, const void* v, void* o, int B, int Tq, int Tk,
                         int heads, int kv_heads, int hd, long long ldq, long long ldk, long long ldv, long long ldo,

@@ -1,5 +1,5 @@
 // llama.cu -- Llama-family LLM model object behind the C ABI: weight arena (transformers state-dict names ->
-// kernel layouts), per-session KV cache, prefill launch sequence (tcgen05 GEMMs + causal GQA attention) and
+// kernel layouts), per-session KV cache, prefill launch sequence (wgmma GEMMs + causal GQA attention) and
 // the persistent greedy decode.  Replaces the device work of LanguageModelHandler._generate
 // (reference S/LLM/language_model.py:832-892: tokenizer -> pipeline("text-generation") -> streamer).
 //
@@ -264,7 +264,7 @@ GemmProblem lgemm(const void* a, int64_t lda, const void* w, int64_t ldw, int64_
 }  // namespace
 
 int llama_max_decode_batch_of(const s2s_llama* m) {
-  return std::min(MAX_DEC_B, llama_decode_max_batch(m->cfg.d_model, m->cfg.ffn, m->cfg.heads * m->cfg.head_dim));
+  return std::min(MAX_DEC_B, llama_decode_max_batch(m->cfg.d_model, m->cfg.ffn, m->cfg.heads * m->cfg.head_dim, dec_grid(m->ctx)));
 }
 
 void llama_fill_dec_params(s2s_llama* m, LlamaDecParams& p) {

@@ -10,7 +10,7 @@
 //   then 5L: final RMSNorm + lm_head + per-CTA argmax      5L+1: global argmax, EOS bookkeeping, next embedding
 // Qwen3 family (qk_norm, transformers modeling_qwen3.py Qwen3Attention): phase 0 stores RAW q / k; the per-head
 // RMSNorm(head_dim) + RoPE is folded into the attention items of phase 1 (ld_qk_prepare), so the phase count stays 5 per
-// layer (it was a sixth phase until round 2: ~10 us per layer and step of pure barrier latency in the TTS frame loop).
+// layer (a sixth phase would add one grid barrier per layer and step to the TTS frame loop).
 // Projections are swap-AB tensor-core GEMVs (sessions on m) fed from per-warp bulk-copy rings of fragment-major weights
 // (decode_common.cuh, weight_tiles.cu); HBM-bound: 15.0 GB / token for Llama-3-8B (SURVEY.md Appendix A).
 #include <algorithm>
@@ -455,9 +455,9 @@ bool llama_decode_plan(int B, int d, int ffn, int qd, int grid, int* kmax, int* 
   return false;
 }
 
-int llama_decode_max_batch(int d, int ffn, int qd) {
+int llama_decode_max_batch(int d, int ffn, int qd, int grid) {
   int kmax, rg, kc, slots;
   for (int B = DEC_MAX_B; B >= 1; --B)
-    if (llama_decode_plan(B, d, ffn, qd, 148, &kmax, &rg, &kc, &slots)) return B;
+    if (llama_decode_plan(B, d, ffn, qd, grid, &kmax, &rg, &kc, &slots)) return B;
   return 0;
 }

@@ -64,8 +64,8 @@ struct LlamaDecParams {
 };
 
 int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int debug_phases, cudaStream_t stream);
-// largest batch per launch that keeps >= 2 weight-ring slots per warp in shared memory
-int llama_decode_max_batch(int d, int ffn, int qd);
+// largest batch per launch on `grid` CTAs that keeps >= 2 weight-ring slots per warp in shared memory
+int llama_decode_max_batch(int d, int ffn, int qd, int grid);
 // shared-memory plan of a batch: kmax = widest operand staged whole, rg = statistics rows per group, kc = down-projection chunk
 // (0 = unchunked); returns false when the batch does not fit
 bool llama_decode_plan(int B, int d, int ffn, int qd, int grid, int* kmax, int* rg, int* kc, int* ring_slots);

@@ -7,7 +7,7 @@
 //
 // Both models are Qwen3-style decoders, i.e. the Llama-family engine of llama.cu with qk_norm:
 //   talker    : s2s_llama over the codec vocabulary, driven by EMBEDDINGS: the prompt rows are prefilled through the
-//               tcgen05 GEMM path (llama_prefill_rows), every frame is one step of the persistent decode kernel with
+//               wgmma GEMM path (llama_prefill_rows), every frame is one step of the persistent decode kernel with
 //               x_in = sum of the previous frame's 16 code embeddings + the next text embedding;
 //   predictor : s2s_llama with one embedding table / output head per residual codebook (multi-table mode): one persistent
 //               launch of n_groups steps per frame: [talker hidden, embed(code0)] then one step per residual codebook.

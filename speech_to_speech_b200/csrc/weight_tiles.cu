@@ -3,7 +3,7 @@
 //   element (row 8*tile + g, k 32*w + 8*t + e)  ->  ((tile * K/32 + w) * 32 + 4*g + t) * 8 + e
 // so that (a) any run of k windows of a tile is one contiguous block = one cp.async.bulk, and (b) the 16-byte
 // fragment loads of a warp read 512 consecutive bytes of shared memory.  Rows N..roundup8(N) are zero.  Done once
-// at finalize; the row-major copy stays for the TMA/tcgen05 GEMMs (prefill, encoder) and the embedding lookup.
+// at finalize; the row-major copy stays for the TMA/wgmma GEMMs (prefill, encoder) and the embedding lookup.
 #include <algorithm>
 
 #include "kernels.cuh"
@@ -29,7 +29,7 @@ size_t tiled_weight_elems(int N, int K) { return (size_t)((N + 7) / 8) * 8 * (si
 int tile_weights_launch(const void* W, int N, int K, void* Wt, cudaStream_t stream) {
   S2S_REQUIRE(K % 32 == 0, "tile_weights: K=%d must be a multiple of 32", K);
   const long long n_vec = (long long)tiled_weight_elems(N, K) / 8;
-  const int blocks = (int)std::min<long long>((n_vec + 255) / 256, 148 * 16);
+  const int blocks = (int)std::min<long long>((n_vec + 255) / 256, 132 * 16);
   tile_weights_kernel<<<blocks, 256, 0, stream>>>(reinterpret_cast<const uint4*>(W), N, K, reinterpret_cast<uint4*>(Wt), n_vec);
   S2S_LAUNCH_CHECK();
   return S2S_OK;

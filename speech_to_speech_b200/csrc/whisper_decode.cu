@@ -6,7 +6,7 @@
 // reference launches ~10 tiny kernels per layer per token and syncs with the host every token for the EOS
 // check; here the host launches once per utterance batch and reads the ids at the end.
 //
-// One CTA per SM (148), 256 threads, 1-16 sessions per launch.  A token step is a fixed sequence of phases separated by
+// One CTA per SM (132 on an H100), 256 threads, 1-16 sessions per launch.  A token step is a fixed sequence of phases separated by
 // a grid barrier:
 //   per layer  0: LN1 + QKV projection (+ self-KV append)   1: self-attention items (32-key blocks, last split merges)
 //              2: out-projection + residual                 3: LN2 + cross-q projection
@@ -366,10 +366,10 @@ whisper_decode_kernel(const WhisperDecParams p, int step_begin, int step_end, in
 // =====================================================================================================================
 // Cluster variant for 1-2 sessions per launch: FOUR grid-wide phases per layer instead of eight.
 //
-// At batch 1 the step time is the number of grid-wide dependency hops (grid barrier + L2 round trip, ~5.5 us each),
+// At batch 1 the step time is the number of grid-wide dependency hops (grid barrier + L2 round trip),
 // not bytes.  Launched with thread-block clusters of CS CTAs, one cluster per attention head, the chain
 //   LN + q/k/v rows of the head -> attention of the head -> the head's slice of the out-projection
-// never leaves the cluster: its two internal hand-offs use barrier.cluster (hardware, ~0.3 us) + L2 instead of the
+// never leaves the cluster: its two internal hand-offs use barrier.cluster (hardware) + L2 instead of the
 // grid barrier.  Each head leaves a PARTIAL out-projection [B, d] (its 64 columns of W_o); the next phase sums the
 // H partials in fixed order while staging its input (stage_rows_norm_sum: deterministic, no atomics), and one CTA
 // writes the summed residual stream back for the later phases:
@@ -397,7 +397,7 @@ __device__ __forceinline__ unsigned int cluster_nctaid_x() {
 // all threads of all CTAs of the cluster; release/acquire at cluster scope covers the global-memory hand-offs
 // ONE thread publishes the CTA's writes (bar.sync + fence by thread 0: cumulative, like grid_arrive); the hardware barrier
 // itself is relaxed -- barrier.cluster.arrive.release makes EVERY thread execute MEMBAR.ALL.GPU, which serialises
-// (measured 6 us per barrier with 256 threads).  Readers use L2 accesses (ld.global.cg) after the wait.
+// with 256 threads.  Readers use L2 accesses (ld.global.cg) after the wait.
 __device__ __forceinline__ void cluster_barrier(int relaxed) {
   __syncthreads();
   if (threadIdx.x == 0) asm volatile("fence.acq_rel.gpu;" ::: "memory");
@@ -597,8 +597,8 @@ whisper_decode_cluster_kernel(const WhisperDecParams p, int step_begin, int step
   __shared__ GemvRing s_rings[DEC_WARPS];
   WdcCtx cx;
   // Cluster identity comes from the hardware registers only: whatever cluster shape the launch really got (a tool that
-  // intercepts the launch may drop or change the cluster attribute -- round 1's ncu-wrapped run returned wrong ids
-  // because the size was taken from the parameter block), rank / size / id stay mutually consistent and the head -> cluster
+  // intercepts the launch may drop or change the cluster attribute -- a size taken from the parameter block would then
+  // give wrong ids), rank / size / id stay mutually consistent and the head -> cluster
   // assignment stays correct; a shape with fewer clusters than heads is caught below.
   cx.cid = (int)cluster_id_x(); cx.rank = (int)cluster_ctarank(); cx.cs = (int)cluster_nctaid_x();
   if ((int)(gridDim.x / cx.cs) < p.heads) __trap();
@@ -788,8 +788,8 @@ int launch_cluster_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, 
 
 template <typename T>
 int launch_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, cudaStream_t stream) {
-  // single sessions: the cluster kernel (measured 520 vs 534 us/token for Whisper-small); batches use the 8-phase kernel,
-  // whose weight stream and attention items spread over all 148 SMs
+  // single sessions: the cluster kernel (fewer grid-wide hops per token); batches use the 8-phase kernel,
+  // whose weight stream and attention items spread over all SMs
   if (p.cluster_size != 0 && p.B == 1 && p.x_alt && p.part_x0 && p.part_x1) {
     int used = 0;
     S2S_CHECK(launch_cluster_t<T>(ctx, p, debug_phases, stream, &used));

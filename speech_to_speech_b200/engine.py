@@ -24,7 +24,7 @@ def get_context(device: int = 0, lane: int = 0, lanes: int = 1) -> C.c_void_p:
     decode kernels of the engines built on lane i use num_sms // lanes CTAs (s2s_set_sm_partition), so the lanes' decode
     launches -- issued from different CUDA streams (lane_stream) -- run side by side on one GPU."""
     if not torch.cuda.is_available():
-        raise S2SError("speech_to_speech_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise S2SError("speech_to_speech_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     if not (lanes >= 1 and 0 <= lane < lanes):
         raise ValueError(f"lane {lane} not in [0, {lanes})")
     lib = _lib.load()
@@ -108,7 +108,7 @@ class WhisperDecodeOptions:
 
 
 class WhisperEngine:
-    """Whisper STT on one B200: log-mel -> encoder -> greedy decoder, batched over utterances."""
+    """Whisper STT on one H100: log-mel -> encoder -> greedy decoder, batched over utterances."""
 
     def __init__(self, geometry: Mapping[str, int], dtype: str = "float16", max_batch: int = 1, device: int = 0,
                  lane: int = 0, lanes: int = 1):
@@ -250,7 +250,7 @@ class WhisperEngine:
 # ---------------------------------------------------------------------------------------------
 def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, act: str = "none",
          out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
-    """C = A @ W^T (+bias) through the tcgen05 kernel; a [M,K], w [N,K] fp16/bf16 cuda tensors."""
+    """C = A @ W^T (+bias) through the wgmma kernel; a [M,K], w [N,K] fp16/bf16 cuda tensors."""
     assert a.is_cuda and w.is_cuda and a.dtype == w.dtype and a.is_contiguous() and w.is_contiguous()
     dev = a.device.index or 0
     M, K = a.shape
@@ -285,7 +285,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, kv_
 
 
 class LlamaEngine:
-    """Llama-family LLM on one B200: tcgen05 prefill + persistent greedy decode with a per-session KV cache."""
+    """Llama-family LLM on one H100: wgmma prefill + persistent greedy decode with a per-session KV cache."""
 
     def __init__(self, geometry: Mapping[str, float], dtype: str = "bfloat16", max_sessions: int = 1,
                  max_positions: int = 2048, max_prefill: int = 512, device: int = 0, lane: int = 0, lanes: int = 1):
@@ -417,7 +417,7 @@ def codec_config(g: Mapping, max_frames: int = 40, precision: int = 1, max_batch
 
 
 class CodecEngine:
-    """Codebook ids -> 24 kHz waveform on one B200 (the codec-decoder half of the TTS slot; csrc/codec_decode.cu)."""
+    """Codebook ids -> 24 kHz waveform on one H100 (the codec-decoder half of the TTS slot; csrc/codec_decode.cu)."""
 
     def __init__(self, geometry: Mapping, max_frames: int = 40, device: int = 0, precision: int = 1, _handle=None, _owner=None):
         self.lib = _lib.load()
@@ -471,7 +471,7 @@ class CodecEngine:
 
 
 class Qwen3TTSEngine:
-    """Talker + code predictor + codec decoder of the TTS slot on one B200 (csrc/qwen3tts.cu).  Geometry mapping =
+    """Talker + code predictor + codec decoder of the TTS slot on one H100 (csrc/qwen3tts.cu).  Geometry mapping =
     oracle.qwen3tts_ref.TTSGeometry.to_dict(); codec geometry = oracle.code2wav_ref.Code2WavGeometry.to_dict()."""
 
     def __init__(self, geometry: Mapping, codec_geometry: Mapping, dtype: str = "bfloat16", max_sessions: int = 4,

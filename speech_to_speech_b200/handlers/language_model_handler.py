@@ -1,6 +1,6 @@
 """B200LanguageModelHandler -- the reference's `transformers` LLM slot with prefill + decode on libs2s_b200.so.
 
-Mirrors LanguageModelHandler (/root/reference/src/speech_to_speech/LLM/language_model.py:785-972): it implements the
+Mirrors LanguageModelHandler (speech_to_speech/LLM/language_model.py:785-972): it implements the
 two hooks the reference's BaseLanguageModelHandler leaves abstract, `_load_model(model_name, device, torch_dtype,
 gen_kwargs)` (:217-224) and `_generate(chat, language_code, gen, ctx, runtime_config, response)` (:238-247), and
 reuses the reference's own `_stream_tokens` / sentence batching / cancel logic unchanged (:309-560).  Where the
@@ -232,7 +232,7 @@ def geometry_from_hf_config(c: Any, max_positions: int) -> dict:
     rope = getattr(c, "rope_parameters", None) or getattr(c, "rope_scaling", None) or {}
     rtype = (rope.get("rope_type") or rope.get("type") or "default") if isinstance(rope, dict) else "default"
     if rtype != "default":
-        raise ValueError(f"rope scaling {rtype!r} is not implemented by the sm_100a RoPE table (plain theta^(-2j/hd) only)")
+        raise ValueError(f"rope scaling {rtype!r} is not implemented by the sm_90a RoPE table (plain theta^(-2j/hd) only)")
     theta = float((rope.get("rope_theta") if isinstance(rope, dict) else None) or getattr(c, "rope_theta", 10000.0))
     for flag in ("attention_bias", "mlp_bias"):
         if getattr(c, flag, False):
@@ -274,7 +274,7 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
 
     def _load_model(self, model_name: str, device: str, torch_dtype: str, gen_kwargs: dict[str, Any]) -> None:
         if not str(device).startswith("cuda"):
-            raise ValueError(f"B200LanguageModelHandler runs on CUDA (sm_100a) only, got device={device!r}; there is no CPU fallback")
+            raise ValueError(f"B200LanguageModelHandler runs on CUDA (sm_90a) only, got device={device!r}; there is no CPU fallback")
         from .. import engine as E
         dev = int(device.split(":")[1]) if ":" in device else 0
         self.gen_kwargs = dict(gen_kwargs)

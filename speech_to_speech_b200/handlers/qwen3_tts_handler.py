@@ -2,7 +2,7 @@
 post-processing on libs2s_b200.so.
 
 Drop-in shape: when `speech_to_speech` is importable this is a subclass of the reference's own `Qwen3TTSHandler`
-(/root/reference/src/speech_to_speech/TTS/qwen3_tts_handler.py) and inherits `setup()` with all its kwargs (:106-211),
+(speech_to_speech/TTS/qwen3_tts_handler.py) and inherits `setup()` with all its kwargs (:106-211),
 `process` (:812-865), sentence coalescing (:751-810), `_estimate_max_new_tokens` (:615-658), `_stream` (:695-749) and the
 session-voice logic unchanged; on a machine without the reference it subclasses the minimal mirror
 (`host/mirror_tts.py`).  Three hooks change:
@@ -68,7 +68,7 @@ class B200Qwen3TTSHandler(_Base):  # type: ignore[misc, valid-type]
         import torch
         device = str(getattr(self, "device", "cuda"))
         if device.startswith("cpu") or not torch.cuda.is_available():
-            raise ValueError("B200Qwen3TTSHandler has no CPU path: qwen3_tts_device must be a CUDA device (sm_100a)")
+            raise ValueError("B200Qwen3TTSHandler has no CPU path: qwen3_tts_device must be a CUDA device (sm_90a)")
         if dtype in ("auto", None):
             self.dtype = torch.bfloat16
         else:

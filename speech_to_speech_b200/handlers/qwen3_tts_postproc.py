@@ -3,7 +3,7 @@
 Scope note (DESIGN.md "TTS"): the Qwen3-TTS talker / codec arithmetic lives in `faster-qwen3-tts`, which is absent
 from the reference tree, this container and the wheelhouse, so its parity is unpinned and it is NOT rebuilt here.
 What the reference itself computes per audio chunk -- `_resample_to_pipeline_sr` (scipy resample_poly 24 kHz ->
-16 kHz) + `_to_int16` (/root/reference/src/speech_to_speech/TTS/qwen3_tts_handler.py:612-613, 674-680) -- is fused
+16 kHz) + `_to_int16` (speech_to_speech/TTS/qwen3_tts_handler.py:612-613, 674-680) -- is fused
 into one CUDA kernel (`s2s_tts_postproc`), bit-exact against scipy.  `patch_handler_class()` swaps those two
 methods on the reference's Qwen3TTSHandler, leaving `_stream`'s trim / 512-sample blocking (:695-749) untouched."""
 from __future__ import annotations

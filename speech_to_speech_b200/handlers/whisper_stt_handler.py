@@ -1,6 +1,6 @@
 """B200WhisperSTTHandler -- the reference's WhisperSTTHandler slot with the forward pass on libs2s_b200.so.
 
-Mirrors /root/reference/src/speech_to_speech/STT/whisper_stt_handler.py: same `setup()` kwargs (:53-61), same
+Mirrors speech_to_speech/STT/whisper_stt_handler.py: same `setup()` kwargs (:53-61), same
 `process(VADAudio) -> Iterator[PartialTranscription | Transcription]` contract (:225-282) including the
 language bookkeeping ("-auto" suffix, sticky last_language restricted to SUPPORTED_LANGUAGES, progressive mode).
 What changes is what the handler calls: `processor(...)` + `model.generate(...)` become ONE call into the C ABI
@@ -132,7 +132,7 @@ class _EngineBundle:
 
 
 class B200WhisperSTTHandler(_api.BaseSTTHandler):
-    """Speech-to-text on the B200 engine.  `model_name`: a local transformers Whisper checkpoint directory / hub id
+    """Speech-to-text on the H100 engine.  `model_name`: a local transformers Whisper checkpoint directory / hub id
     (weights are read once on the CPU and copied into the engine), or "random:<geometry>[:seed]" for seeded
     random-init weights at a reference geometry (tiny/small/large-v3) -- used by the tests and benches because no
     checkpoints exist offline."""
@@ -143,7 +143,7 @@ class B200WhisperSTTHandler(_api.BaseSTTHandler):
               compile_mode: Optional[str] = None, language: Optional[str] = None, gen_kwargs: dict[str, Any] = {},
               max_batch: int = 1, batch_wait_ms: float = 6.0, lane: Optional[int] = None, lanes: int = 1, batch_gap_ms: float = 0.8) -> None:
         if not str(device).startswith("cuda"):
-            raise ValueError(f"B200WhisperSTTHandler runs on CUDA (sm_100a) only, got device={device!r}; there is no CPU fallback")
+            raise ValueError(f"B200WhisperSTTHandler runs on CUDA (sm_90a) only, got device={device!r}; there is no CPU fallback")
         from .. import engine as E  # raises ImportError if libs2s_b200.so is not built
 
         self.device = device

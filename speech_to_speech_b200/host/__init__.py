@@ -3,9 +3,8 @@
 `resolve()` returns the reference's own stage-runtime types when `speech_to_speech` is importable (the
 drop-in case: our handlers then subclass the reference's BaseHandler / BaseSTTHandler and are driven by its
 unchanged thread loop), and otherwise a minimal mirror of that interface (same names, argument meaning and
-error behaviour; reference: /root/reference/src/speech_to_speech/baseHandler.py:24-187,
-pipeline/messages.py:45-223) so that the handlers can be exercised on a machine that only has this repo
-(the GPU box has no /root/reference)."""
+error behaviour; reference: speech_to_speech/baseHandler.py:24-187,
+pipeline/messages.py:45-223) so that the handlers can be exercised on a machine that only has this repo."""
 from __future__ import annotations
 
 import importlib

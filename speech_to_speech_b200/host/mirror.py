@@ -1,4 +1,4 @@
-"""Minimal mirror of the reference's stage runtime for machines without /root/reference.
+"""Minimal mirror of the reference's stage runtime for machines without the upstream speech_to_speech package.
 
 Same constructor, hook names and loop semantics as the reference BaseHandler
 (S/baseHandler.py:24-187): `setup(*setup_args, **setup_kwargs)` runs in the constructor, `run()` pulls from

@@ -1,4 +1,4 @@
-"""Minimal mirror of the reference's Qwen3-TTS handler slot for machines without /root/reference (the GPU box).
+"""Minimal mirror of the reference's Qwen3-TTS handler slot for machines without the upstream speech_to_speech package.
 
 When `speech_to_speech` is importable the B200 handler subclasses the reference's own `Qwen3TTSHandler` and inherits all
 of this unchanged; this mirror restates only what the hot path needs, with the same method names, argument meaning and

@@ -1,5 +1,5 @@
-"""Registration of the B200 handlers in the reference's backend registry
-(/root/reference/src/speech_to_speech/backend_registry.py:77-100 BackendSpec, :151-161 registry dicts, :206-233
+"""Registration of the H100 handlers in the reference's backend registry
+(speech_to_speech/backend_registry.py:77-100 BackendSpec, :151-161 registry dicts, :206-233
 `_simple_handler_factory`).  Two ways in, both leaving the registry module unmodified:
 
   register()            adds the specs "b200-whisper" (stt), "b200-transformers" (llm) and "b200-qwen3" (tts) next to the

@@ -1,7 +1,7 @@
 """B200Qwen3TTS -- the object the TTS handler slot holds in `self.model`, on libs2s_b200.so.
 
 It stands where the reference puts `FasterQwen3TTS.from_pretrained(model_name, device=, dtype=, attn_implementation=,
-backend=, ...)` (/root/reference/src/speech_to_speech/TTS/qwen3_tts_handler.py:213-249) and offers the calls the handler
+backend=, ...)` (speech_to_speech/TTS/qwen3_tts_handler.py:213-249) and offers the calls the handler
 makes on it: `warmup(prefill_len=100)` (:555-572), `generate_custom_voice_streaming(text, speaker, language, instruct,
 chunk_size, max_new_tokens, non_streaming_mode)` (:946-978) yielding `(audio_f32, 24000, timing)` per chunk -- the tuple
 contract the reference's tests pin with fakes (T/test_qwen3_tts_handler_backend.py:756-762) -- `get_supported_speakers()`
@@ -64,7 +64,7 @@ DEFAULT_SPEAKERS = {"aiden": 2301, "ethan": 2302, "chelsie": 2303}   # codec-voc
 class DeviceAudio:
     """A chunk of 24 kHz fp32 audio that is still on the GPU.  `np.asarray(chunk)` copies it to the host, so a consumer
     that only knows the `(np.float32[n], sr, timing)` contract (the reference's `_prepare_audio_chunk`, :682-693) works
-    unchanged; the B200 handler keeps it on the device and runs resample + int16 there."""
+    unchanged; the GPU handler keeps it on the device and runs resample + int16 there."""
 
     __slots__ = ("tensor",)
 

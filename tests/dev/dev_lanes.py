@@ -33,7 +33,7 @@ def timed(jobs, reps=3):
 
 frames = lambda i: (lambda: lanes[i].decode_frames(list(range(B)), NF))
 codec = lambda i: (lambda: lanes[i].decode_audio_batch(list(range(B)), 8, 25))
-for ctas in (148, 74, 96, 52):
+for ctas in (132, 66, 88, 44):
     os.environ["S2S_DECODE_CTAS"] = str(ctas)
     one = timed([(0, frames(0))])
     two = timed([(0, frames(0)), (1, frames(1))])
@@ -43,5 +43,5 @@ os.environ["S2S_DECODE_CTAS"] = "74"
 c1 = timed([(1, codec(1))])
 mix = timed([(0, frames(0)), (1, codec(1))])
 print(f"codec chunk alone {c1:.2f} ms; {NF} frames (74 CTAs) alone {timed([(0, frames(0))]):.2f} ms; both concurrently {mix:.2f} ms")
-os.environ["S2S_DECODE_CTAS"] = "148"
+os.environ["S2S_DECODE_CTAS"] = "132"
 print(f"full grid: frames {timed([(0, frames(0))]):.2f} ms, codec {timed([(1, codec(1))]):.2f} ms, sequential sum is the baseline")

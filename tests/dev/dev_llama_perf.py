@@ -1,4 +1,4 @@
-"""Developer aid: Llama-3-8B prefill/decode timing on one B200 (random-init weights)."""
+"""Developer aid: Llama-3-8B prefill/decode timing on one H100 (random-init weights)."""
 import os, sys, time, json
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))); sys.path.insert(0, ROOT)

@@ -45,7 +45,7 @@ int main() {
                            {7168, 1024}, {1024, 3584}, {32064, 1024}};
   int bad = 0;
   for (auto& s : shapes)
-    for (int grid : {148, 144, 132, 120, 112}) {
+    for (int grid : {148, 144, 132, 120, 112, 66}) {
       char what[64]; snprintf(what, sizeof what, "[%d,%d] grid %d", s[0], s[1], grid);
       bad += check((s[0] + 7) / 8, s[1], grid, 0, 30, 0, what);
     }
@@ -71,7 +71,7 @@ int main() {
   for (int BH : {2, 6, 12, 20, 24, 32, 48, 96, 128, 192, 320, 512})
     for (int nb : {1, 2, 5, 14, 47, 64, 256})
       for (int smax : {4, 24, 128}) {
-        const int p = attn_plan(BH, nb, smax, 148), S = p & 0x7f;
+        const int p = attn_plan(BH, nb, smax, 132), S = p & 0x7f;
         if (S < 1 || S > nb || S > smax || S > ((p & ATTN_WARP_LEVEL) ? 32 : 16)) { printf("attn_plan(%d,%d,%d) = %d\n", BH, nb, smax, p); ++bad; }
       }
   // K-chunked projections (gemv_mma_chunked): for every accepted shape each (tile, k) of every chunk is covered exactly once by
@@ -79,7 +79,7 @@ int main() {
   {
     const int cases[][3] = {{4096, 14336, 4096}, {2560, 9728, 4096}, {1024, 3584, 1024}, {4096, 14336, 2048}, {256, 1536, 256}};
     for (auto& cse : cases)
-      for (int grid : {148, 132}) {
+      for (int grid : {132, 66}) {
         const int N = cse[0], K = cse[1], kc = cse[2];
         if (!gemv_chunk_ok(N, K, kc, grid)) continue;
         const int n_tiles = (N + 7) / 8, n_chunks = (K + kc - 1) / kc;
@@ -107,7 +107,8 @@ int main() {
           if (pos != K) { printf("chunk tile %d covers %d of %d\n", kv.first, pos, K); ++bad; }
         }
       }
-    if (!gemv_chunk_ok(4096, 14336, 4096, 148)) { printf("Llama-3-8B down-projection must be chunkable\n"); ++bad; }
+    for (int grid : {132, 66})  // a whole H100, and one of two SM partitions
+      if (!gemv_chunk_ok(4096, 14336, 4096, grid)) { printf("Llama-3-8B down-projection must be chunkable on %d CTAs\n", grid); ++bad; }
   }
   printf(bad ? "FAILED %d\n" : "OK\n", bad);
   return bad ? 1 : 0;

@@ -1,5 +1,5 @@
-// Developer microbenchmark (not part of the library): HBM read bandwidth of GEMV-like access patterns on B200.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o stream_bw stream_bw.cu && ./stream_bw
+// Developer microbenchmark (not part of the library): HBM read bandwidth of GEMV-like access patterns on H100.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o stream_bw stream_bw.cu && ./stream_bw
 #include <cstdio>
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -66,7 +66,8 @@ int main() {
   const long long bytes = 2LL << 30;  // 2 GiB >> L2
   char* buf; cudaMalloc(&buf, bytes); cudaMemset(buf, 1, bytes);
   unsigned* sink; cudaMalloc(&sink, 4);
-  int sms = 148;
+  int sms = 0;
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
   for (int K : {4096, 14336, 768}) {
     const long long n_rows = bytes / (K * 2);
     for (int threads : {256, 512}) for (int mult : {1, 2}) {

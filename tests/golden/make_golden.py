@@ -333,9 +333,14 @@ def qwen3tts_golden(name: str = "micro", text_len: int = 6, max_frames: int = 10
         codes = torch.stack([h[-1] for h in res.hidden_states if h[-1] is not None], dim=1)[0].numpy()   # [F, 16]
         t_scores = torch.stack([s[0] for s in res.scores]).numpy()
     path = os.path.join(OUT, f"qwen3tts_{name}.npz")
+    # the predictor logits are large: a fixed half of the vocabulary columns, and the top two of every row (the margins)
+    p_scores = np.stack(pred_scores).astype(np.float32)
+    cols = np.sort(np.random.default_rng(0).choice(p_scores.shape[-1], p_scores.shape[-1] // 2, replace=False)).astype(np.int32)
+    top2 = np.sort(np.where(np.isfinite(p_scores), p_scores, -1e30), axis=-1)[..., -2:].astype(np.float32)
     np.savez_compressed(path, text_ids=np.asarray(text_ids, np.int32), speaker=speaker, codes=codes.astype(np.int32),
                         code0_all=res.sequences[0].numpy().astype(np.int32), talker_logits=t_scores.astype(np.float32),
-                        predictor_logits=np.stack(pred_scores).astype(np.float32), prompt_embeds=embeds[0].numpy().astype(np.float32),
+                        predictor_logits=np.ascontiguousarray(p_scores[..., cols]), predictor_logits_cols=cols, predictor_top2=top2,
+                        prompt_embeds=embeds[0].numpy().astype(np.float32),
                         trailing=trailing[0].numpy().astype(np.float32), max_frames=max_frames,
                         transformers_version=__import__("transformers").__version__)
     print("wrote", path, codes.shape, codes[:2].tolist(), "code0", res.sequences[0].tolist())

@@ -23,7 +23,7 @@ def E(monkeypatch):
             return 0
     monkeypatch.setattr(_lib, "load", lambda: FakeLib())
     monkeypatch.setattr(torch.cuda, "is_available", lambda: True)
-    monkeypatch.setattr(torch.cuda, "get_device_properties", lambda d: types.SimpleNamespace(multi_processor_count=148))
+    monkeypatch.setattr(torch.cuda, "get_device_properties", lambda d: types.SimpleNamespace(multi_processor_count=132))
     monkeypatch.setattr(torch.cuda, "Stream", lambda device=None: types.SimpleNamespace(kind="lane", device=device))
     monkeypatch.setattr(torch.cuda, "default_stream", lambda d=None: types.SimpleNamespace(kind="default", device=d))
     monkeypatch.setattr(engine, "_ctx_by_device", {})
@@ -38,8 +38,8 @@ def test_one_context_per_device_and_lane_with_its_sm_partition(E):
     whole = E.get_context(0)
     assert whole.value not in (a.value, b.value)
     parts = [c for c in E._test_calls if c[0] == "partition"]
-    assert [p[2] for p in parts] == [74, 74] and {p[1] for p in parts} == {a.value, b.value}      # 148 SMs // 2 lanes; none for one lane
-    assert E.get_context(0, 2, 3) is not None and [c for c in E._test_calls if c[0] == "partition"][-1][2] == 49
+    assert [p[2] for p in parts] == [66, 66] and {p[1] for p in parts} == {a.value, b.value}      # 132 SMs // 2 lanes; none for one lane
+    assert E.get_context(0, 2, 3) is not None and [c for c in E._test_calls if c[0] == "partition"][-1][2] == 44
     with pytest.raises(ValueError):
         E.get_context(0, 2, 2)
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (B200) of the TTS codec decoder (csrc/codec_decode.cu) through the C ABI against the numpy oracle
+"""GPU parity tests (H100) of the TTS codec decoder (csrc/codec_decode.cu) through the C ABI against the numpy oracle
 (oracle/code2wav_ref.py) and the golden vectors generated from transformers' Qwen3OmniMoeCode2Wav.  fp32 arithmetic on
 both sides: pre-transformer output within 2e-4, waveform (values in [-1, 1]) within 1e-3 (stated tolerance; measured far
 below).  Parity with the real Qwen3-TTS codec stays unpinned (upstream absent)."""

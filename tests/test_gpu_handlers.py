@@ -1,4 +1,4 @@
-"""GPU: the handlers end to end on a B200 (mirror runtime when the reference tree is absent), and the TTS
+"""GPU: the handlers end to end on an H100 (mirror runtime when the reference tree is absent), and the TTS
 post-processing kernel against scipy (bit-exact int16)."""
 from queue import Queue
 from threading import Event, Thread

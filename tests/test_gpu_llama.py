@@ -1,4 +1,4 @@
-"""GPU parity tests (B200) for the Llama-family path through the C ABI, against the numpy oracle and the
+"""GPU parity tests (H100) for the Llama-family path through the C ABI, against the numpy oracle and the
 transformers goldens.  bf16 weights/operands, fp32 accumulate/residual: logits tolerance 3e-2 (values O(1));
 token ids exact wherever the oracle's top-1 margin exceeds 4x that tolerance."""
 import os

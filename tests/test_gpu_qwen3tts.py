@@ -1,4 +1,4 @@
-"""GPU parity tests (B200) of the TTS talker + code predictor (csrc/qwen3tts.cu) through the C ABI: codebook ids
+"""GPU parity tests (H100) of the TTS talker + code predictor (csrc/qwen3tts.cu) through the C ABI: codebook ids
 bit-exact against the numpy oracle (oracle/qwen3tts_ref.py) and the golden codes generated from the transformers
 cousin; sessions batched in one launch equal the single-session results.  Unpinned vs faster-qwen3-tts (absent)."""
 import os
@@ -63,7 +63,7 @@ def test_codes_match_transformers_golden(E, golden_dir, dtype):
     codes every safe decision is bit-exact; the free run equals the golden codes up to the first unsafe decision."""
     g, cg, w, cw, eng = _engine(E, dtype)
     G = np.load(os.path.join(golden_dir, "qwen3tts_micro.npz"))
-    gold, tl, pl = G["codes"], G["talker_logits"], G["predictor_logits"]
+    gold, tl, pl = G["codes"], G["talker_logits"], G["predictor_top2"]   # the margins need only each row's top two
     F = len(gold)
     eng.prefill(0, G["text_ids"].tolist(), int(G["speaker"]))
     _check_forced(eng, [(gold, tl, pl)], [0], TOL[dtype], 0.6 if dtype == "float16" else 0.2)

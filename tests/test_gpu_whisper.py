@@ -1,4 +1,4 @@
-"""GPU parity tests (B200): the CUDA path, called through the C ABI, against the numpy oracle and the
+"""GPU parity tests (H100): the CUDA path, called through the C ABI, against the numpy oracle and the
 transformers-generated golden vectors.
 
 Tolerances (stated, per BASELINE.json north_star "token ids bit-exact, logits/mel within a stated fp tolerance"):
@@ -47,6 +47,7 @@ def _opts(E, G, max_new=None):
 @pytest.mark.parametrize("shape", [(128, 64, 64), (1500, 768, 768), (200, 64, 240), (3000, 2304, 768), (333, 512, 3072),
                                    (1, 128, 8), (129, 192, 72)])
 def test_gemm_tcgen05_matches_fp32_matmul(E, dt, shape):
+    """The tensor-core GEMM (csrc/gemm_tc.cu, wgmma on sm_90a) against an fp32 matmul."""
     M, N, K = shape
     gen = torch.Generator(device="cuda").manual_seed(M * 7 + N)
     a = (torch.randn(M, K, device="cuda", generator=gen) * 0.5).to(dt)

@@ -11,9 +11,12 @@ from types import SimpleNamespace
 
 import pytest
 
-REF_SRC = "/root/reference/src"
-HAVE_REF = os.path.isdir(REF_SRC)
-pytestmark = pytest.mark.skipif(not HAVE_REF, reason="reference tree not present (GPU box)")
+from oracle import upstream
+
+REF_SRC = upstream.reference_src()   # the upstream huggingface/speech-to-speech `src` tree, "" when absent
+HAVE_REF = bool(REF_SRC) and os.path.isdir(REF_SRC)
+# the tests that drive a request through process() need the reference's Chat and message types
+needs_ref = pytest.mark.skipif(not HAVE_REF, reason="upstream source tree not found (oracle/upstream.py)")
 if HAVE_REF and REF_SRC not in sys.path:
     sys.path.insert(0, REF_SRC)
 
@@ -117,6 +120,7 @@ def _request(text="tell me something", **kw):
     return GenerateResponseRequest(runtime_config=RuntimeConfig(chat=chat), **kw), chat
 
 
+@needs_ref
 def test_request_flows_through_process_in_the_reference_order(monkeypatch):
     from speech_to_speech.pipeline.messages import EndOfResponse, LLMResponseChunk, TokenUsage
     h, tok, eng = _handler(monkeypatch, "Hello there. How are you today?")
@@ -141,6 +145,7 @@ def test_request_flows_through_process_in_the_reference_order(monkeypatch):
     assert eng.decode_calls >= 3       # the reply was produced in chunks of 2 tokens
 
 
+@needs_ref
 def test_cancel_scope_stops_generation_between_chunks(monkeypatch):
     from speech_to_speech.pipeline.cancel_scope import CancelScope
     from speech_to_speech.pipeline.messages import EndOfResponse, LLMResponseChunk
@@ -158,6 +163,7 @@ def test_cancel_scope_stops_generation_between_chunks(monkeypatch):
     assert 1 <= n_chunks < 8 and eng.decode_calls < 8
 
 
+@needs_ref
 def test_prefetch_abort_is_registered_and_stops_the_stream(monkeypatch):
     h, tok, eng = _handler(monkeypatch, "A b c d e f g h i j k l m n o p.")
     from speech_to_speech.LLM.language_model import StreamContext

@@ -1,6 +1,6 @@
-"""CPU contract tests of the B200 TTS handler slot with a fake model object (the reference's own test strategy: bypass the
+"""CPU contract tests of the TTS handler slot with a fake model object (the reference's own test strategy: bypass the
 device, inject fakes -- T/test_qwen3_tts_handler_backend.py:18-19, 756-762).  Both base classes are exercised: the reference's
-Qwen3TTSHandler when importable, and the mirror used on machines without /root/reference."""
+Qwen3TTSHandler when its source tree is found (oracle/upstream.py), and the mirror used without it."""
 import importlib
 import os
 import sys
@@ -10,7 +10,9 @@ from threading import Event
 import numpy as np
 import pytest
 
-REF_SRC = "/root/reference/src"
+from oracle import upstream
+
+REF_SRC = upstream.reference_src()   # the upstream huggingface/speech-to-speech `src` tree, "" when absent
 LONG = " ".join(["This is a deliberately long sentence for the Qwen3 TTS budget estimator."] * 12)
 CJK_SHORT = "我懂，心情不好时会让人特别疲惫。"
 CJK_LONG = ("上海是一座充满活力的现代化大都市，既有繁华的金融中心和摩天大楼，也有老城厢的弄堂风情"
@@ -46,10 +48,10 @@ def _handler_module(use_reference: bool):
     """Import handlers.qwen3_tts_handler against the reference base or the mirror base."""
     for m in [k for k in sys.modules if k.startswith("speech_to_speech_b200.handlers.qwen3_tts_handler")]:
         del sys.modules[m]
-    had = REF_SRC in sys.path
+    had = bool(REF_SRC) and REF_SRC in sys.path
     if use_reference:
-        if not os.path.isdir(REF_SRC):
-            pytest.skip("reference tree not present")
+        if not REF_SRC or not os.path.isdir(REF_SRC):
+            pytest.skip("upstream source tree not found (oracle/upstream.py)")
         if not had:
             sys.path.insert(0, REF_SRC)
     else:
@@ -154,25 +156,36 @@ def test_token_budget_goldens_of_the_reference(monkeypatch, use_reference):
 
 
 def test_mirror_budget_equals_the_reference_function_on_random_text():
-    if not os.path.isdir(REF_SRC):
-        pytest.skip("reference tree not present")
-    sys.path.insert(0, REF_SRC)
-    try:
-        from speech_to_speech.TTS.qwen3_tts_handler import Qwen3TTSHandler
-    except Exception as e:
-        pytest.skip(f"reference handler not importable: {e}")
-    finally:
-        sys.path.remove(REF_SRC)
+    """The mirror's estimator against the reference's `_estimate_max_new_tokens` on 600 seeded random texts: the reference's
+    answers are stored in tests/golden/reference_tts_helpers.npz, and asked live too when its source tree is found."""
     from speech_to_speech_b200.host.mirror_tts import MirrorQwen3TTSHandler
-    a, b = object.__new__(Qwen3TTSHandler), object.__new__(MirrorQwen3TTSHandler)
+    a = None
+    if REF_SRC and os.path.isdir(REF_SRC):
+        sys.path.insert(0, REF_SRC)
+        try:
+            from speech_to_speech.TTS.qwen3_tts_handler import Qwen3TTSHandler
+            a = object.__new__(Qwen3TTSHandler)
+        except Exception:
+            a = None
+        finally:
+            sys.path.remove(REF_SRC)
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_tts_helpers.npz"))
+    b = object.__new__(MirrorQwen3TTSHandler)
     rng = np.random.default_rng(0)
     alphabet = list("abcdefghij klmnop, qrst. uvw! xyz? 上海是一座城市，。") + [" "] * 6
+    k = 0
     for chunk, cap in ((8, 1536), (4, 700), (1, 5000)):
-        a.streaming_chunk_size = b.streaming_chunk_size = chunk
-        a.max_new_tokens = b.max_new_tokens = cap
+        b.streaming_chunk_size, b.max_new_tokens = chunk, cap
+        if a is not None:
+            a.streaming_chunk_size, a.max_new_tokens = chunk, cap
         for _ in range(200):
             text = "".join(rng.choice(alphabet, int(rng.integers(0, 900))))
-            assert a._estimate_max_new_tokens(text) == b._estimate_max_new_tokens(text), text
+            assert (g["budget_chunk"][k], g["budget_cap"][k], g["budget_len"][k]) == (chunk, cap, len(text))
+            assert b._estimate_max_new_tokens(text) == g["budget_tokens"][k], text
+            if a is not None:
+                assert a._estimate_max_new_tokens(text) == g["budget_tokens"][k], text
+            k += 1
+    assert k == len(g["budget_tokens"])
 
 
 @pytest.mark.parametrize("use_reference", [True, False])
