@@ -155,22 +155,44 @@ int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, co
                           int32_t ndim, int32_t dtype);
 int s2s_llama_init_random(s2s_llama* m, uint64_t seed);
 int s2s_llama_finalize(s2s_llama* m);
-/* Reset a KV-cache slot (new response). */
+/* Reset a KV-cache slot (new response).  Also empties the slot's seen-id set (repetition penalty), on the stream of the
+ * slot's next prefill or decode. */
 int s2s_llama_session_reset(s2s_llama* m, int32_t slot);
+/* Token choice of a slot, in transformers' logits-processor order (generation/utils.py _get_logits_processor):
+ * repetition penalty over every id the slot has seen (prompt and generated), EOS ids masked until min_new_tokens tokens were
+ * produced since the slot's last prefill, then only when do_sample: temperature, top-k (0 = off), top-p (1 = off) and a
+ * Gumbel-max draw whose uniforms come from Philox4x64-10 keyed by `seed` with counter (token id, position of the predicted
+ * token) -- numpy.random.Philox(key=seed, counter=[id, position, 0, 0]), first output -- so a token depends only on (seed,
+ * position, logits).  NULL = greedy argmax, which is also the state after create.  Every prefill adds its prompt ids to the
+ * seen set; a token joins it when it is fed to a decode launch of a slot with a penalty (the choice after an intermediate
+ * chunk of a long prompt does not).  Set it before the prefill of a response.                                          */
+typedef struct {
+  int32_t do_sample;
+  float temperature;          /* > 0 when do_sample */
+  int32_t top_k;              /* >= 0; 0 or >= vocab = off */
+  float top_p;                /* (0, 1]; 1 = off */
+  float repetition_penalty;   /* > 0; 1 = off */
+  int32_t min_new_tokens;     /* >= 0 */
+  int32_t n_eos;              /* <= 8 */
+  int32_t eos_ids[8];
+  uint64_t seed;
+} s2s_sampling;
+int s2s_llama_set_sampling(s2s_llama* m, int32_t slot, const s2s_sampling* s);
 /* Prefill `n` prompt tokens (host ids) into `slot`; logits_out_d optional [n, vocab] f32;
- * next_id_d optional [1] i32 = argmax of the last position.                                 */
+ * next_id_d optional [1] i32 = the token chosen from the last position (argmax, or the slot's s2s_llama_set_sampling). */
 int s2s_llama_prefill(s2s_llama* m, int32_t slot, const int32_t* ids_h, int32_t n, float* logits_out_d,
                       int32_t* next_id_d, void* stream);
 /* Prefill of B sessions in ONE pass over the weights (the reference prefills one request per pipeline call,
  * LLM/language_model.py:883-888): ids_h holds the sessions' new prompt tokens back to back (n_h[b] tokens for slot slots_h[b],
  * sum <= max_prefill, B <= 16); the projections and the MLP run over all rows at once, RoPE / KV append / causal attention per
- * session.  next_ids_d [B] receives each session's greedy next token.  Rows of a session produce the same values as
+ * session.  next_ids_d [B] receives each session's next token (chosen as by s2s_llama_prefill).  Rows of a session produce the same values as
  * s2s_llama_prefill up to the tile shape the GEMM picks for the row count. */
 int s2s_llama_prefill_batch(s2s_llama* m, const int32_t* slots_h, int32_t B, const int32_t* ids_h, const int32_t* n_h,
                             int32_t* next_ids_d, void* stream);
 
-/* Greedy decode for B (<= s2s_llama_max_decode_batch: 16, 4 for Llama-3-8B) sessions in one persistent launch.  slots_h[B]; first_ids_d[B] are the tokens to
- * feed first (the prefill argmax); ids_out_d [B, n_steps] receives the n_steps tokens generated AFTER them; eos stops
+/* Decode for B (<= s2s_llama_max_decode_batch: 16, 4 for Llama-3-8B) sessions in one persistent launch, each token chosen as
+ * its slot's s2s_llama_set_sampling says (argmax by default).  slots_h[B]; first_ids_d[B] are the tokens to
+ * feed first (the prefill's choice); ids_out_d [B, n_steps] receives the n_steps tokens generated AFTER them; eos stops
  * a row (eos_id < 0 disables); forced_d optional [B, n_steps] teacher-forced feedback; logits_out_d optional
  * [n_steps, B, vocab].                                                                              */
 int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int32_t* first_ids_d,
@@ -180,8 +202,8 @@ int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int3
 int s2s_llama_set_trace(s2s_llama* m, uint64_t* trace_d, int32_t capacity);
 /* Largest B accepted by s2s_llama_decode for this geometry (shared-memory budget of the decode kernel, <= 16). */
 int32_t s2s_llama_max_decode_batch(s2s_llama* m);
-/* End-to-end with HOST buffers: (chunked) prefill + greedy decode, synchronous.  ids_out_h[0] is the argmax of the
- * prompt's last position, n_steps tokens in total (generate() semantics of the reference's pipeline call). */
+/* End-to-end with HOST buffers: (chunked) prefill + decode with the slot's token choice, synchronous.  ids_out_h[0] is
+ * the token chosen from the prompt's last position, n_steps tokens in total (generate() semantics of the reference's pipeline call). */
 int s2s_llama_generate(s2s_llama* m, int32_t slot, const int32_t* prompt_h, int32_t n_prompt, int32_t n_steps,
                        int32_t eos_id, int32_t* ids_out_h, int32_t* len_out_h, void* stream);
 

@@ -19,7 +19,7 @@ EXPORTED = [
     "s2s_whisper_detect_language", "s2s_whisper_transcribe", "s2s_whisper_set_trace", "s2s_whisper_max_decode_batch",
     "s2s_gemm", "s2s_attention",
     "s2s_llama_create", "s2s_llama_destroy", "s2s_llama_bind_tensor", "s2s_llama_init_random",
-    "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
+    "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_set_sampling", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
     "s2s_tts_postproc",
     "s2s_codec_create", "s2s_codec_destroy", "s2s_codec_bind_tensor", "s2s_codec_init_random", "s2s_codec_finalize",
     "s2s_codec_decode", "s2s_codec_samples", "s2s_codec_total_upsample",
@@ -51,6 +51,14 @@ class LlamaConfig(C.Structure):
         ("rope_theta", C.c_float), ("rms_eps", C.c_float),
         ("compute_dtype", C.c_int32), ("max_sessions", C.c_int32), ("max_positions", C.c_int32),
         ("max_prefill", C.c_int32), ("qk_norm", C.c_int32), ("n_tables", C.c_int32),
+    ]
+
+
+class Sampling(C.Structure):
+    _fields_ = [
+        ("do_sample", C.c_int32), ("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float),
+        ("repetition_penalty", C.c_float), ("min_new_tokens", C.c_int32), ("n_eos", C.c_int32), ("eos_ids", C.c_int32 * 8),
+        ("seed", C.c_uint64),
     ]
 
 
@@ -119,6 +127,7 @@ def load() -> C.CDLL:
     lib.s2s_llama_init_random.argtypes = [vp, C.c_uint64]
     lib.s2s_llama_finalize.argtypes = [vp]
     lib.s2s_llama_session_reset.argtypes = [vp, i32]
+    lib.s2s_llama_set_sampling.argtypes = [vp, i32, C.POINTER(Sampling)]
     lib.s2s_llama_prefill.argtypes = [vp, i32, C.POINTER(i32), i32, vp, vp, vp]
     lib.s2s_llama_prefill_batch.argtypes = [vp, C.POINTER(i32), i32, C.POINTER(i32), C.POINTER(i32), vp, vp]
     lib.s2s_llama_decode.argtypes = [vp, C.POINTER(i32), i32, vp, i32, i32, vp, vp, vp, vp, vp]

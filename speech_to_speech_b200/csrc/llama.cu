@@ -108,6 +108,20 @@ __global__ void argmax_row_kernel(const float* __restrict__ logits, int n, int* 
   }
 }
 
+// sampling.cuh's choice for one row (prefill).  The chosen id joins the seen set only when it is fed (the decode launch):
+// the choice after an intermediate chunk of a long prompt is discarded.
+__global__ void __launch_bounds__(1024) sample_row_kernel(const float* __restrict__ row, int n, const SampSlot s,
+                                                          const unsigned int* seen, int pred_pos, int* __restrict__ out) {
+  __shared__ SampShared sh;
+  const int tok = sample_row(row, n, s, seen, pred_pos, sh);
+  if (threadIdx.x == 0) *out = tok;
+}
+
+__global__ void seen_set_kernel(const int* __restrict__ ids, int n, unsigned int* seen) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) atomicOr(seen + (ids[i] >> 5), 1u << (ids[i] & 31));
+}
+
 inline uint16_t f2h(float f) { __half h = __float2half_rn(f); uint16_t u; memcpy(&u, &h, 2); return u; }
 inline uint16_t f2bf(float f) {
   uint32_t u; memcpy(&u, &f, 4);
@@ -251,6 +265,12 @@ int build(s2s_llama* m) {
   S2S_CHECK(lalloc(m, &m->sync_counter, 16));
   S2S_CHECK(lalloc(m, &m->kraw, (size_t)MAX_DEC_B * kvd * 4));
   S2S_CHECK(lalloc(m, &m->qn, (size_t)MAX_DEC_B * qd * 4));
+  m->samp.assign(c.max_sessions, samp_greedy());
+  m->seen_words = (c.vocab + 31) / 32;
+  m->seen_stale.assign(c.max_sessions, 0);
+  S2S_CHECK(lalloc(m, &m->samp_d, MAX_DEC_B * sizeof(SampSlot)));
+  S2S_CHECK(lalloc(m, &m->samp_rows, (size_t)MAX_DEC_B * c.vocab * 4));
+  S2S_CHECK(lalloc(m, &m->seen, (size_t)c.max_sessions * m->seen_words * 4));
   return S2S_OK;
 }
 
@@ -278,6 +298,35 @@ void llama_fill_dec_params(s2s_llama* m, LlamaDecParams& p) {
   p.done = m->done; p.n_done = m->n_done; p.cand_val = m->cand_val; p.cand_idx = m->cand_idx; p.sync_counter = m->sync_counter;
   p.trace = m->trace; p.trace_cap = m->trace_cap;
   p.qk_norm = c.qk_norm ? 1 : 0; p.kraw = m->kraw; p.qn = m->qn;
+  p.samp_rows = m->samp_rows; p.seen = m->seen; p.seen_words = m->seen_words;
+}
+
+// The seen set of a slot that was reset is emptied on the stream of the slot's next launch (session_reset takes no stream).
+static int seen_clear_if_reset(s2s_llama* m, int slot, cudaStream_t st) {
+  if (!m->seen_stale[slot]) return S2S_OK;
+  S2S_CHECK_CUDA(cudaMemsetAsync(m->seen + (size_t)slot * m->seen_words, 0, (size_t)m->seen_words * 4, st));
+  m->seen_stale[slot] = 0;
+  return S2S_OK;
+}
+
+// Repetition penalty: the n prompt ids (device) of a prefill join the slot's seen set, whatever its current settings, so
+// that a penalty set later in the response still sees the whole prompt.
+static int seen_add(s2s_llama* m, int slot, const int* ids_d, int n, cudaStream_t st) {
+  S2S_CHECK(seen_clear_if_reset(m, slot, st));
+  seen_set_kernel<<<(n + 255) / 256, 256, 0, st>>>(ids_d, n, m->seen + (size_t)slot * m->seen_words);
+  S2S_LAUNCH_CHECK();
+  return S2S_OK;
+}
+
+// The token predicted from the logits row that follows a prefill of `slot`, at position pred_pos: argmax for a greedy slot,
+// sampling.cuh's choice otherwise.  The slot's new-token count restarts here.
+static int prefill_choose(s2s_llama* m, int slot, const float* row, int pred_pos, int32_t* out_d, cudaStream_t st) {
+  SampSlot& s = m->samp[slot];
+  s.base = pred_pos;
+  if (!s.active) argmax_row_kernel<<<1, 1024, 0, st>>>(row, m->cfg.vocab, out_d);
+  else sample_row_kernel<<<1, 1024, 0, st>>>(row, m->cfg.vocab, s, m->seen + (size_t)slot * m->seen_words, pred_pos, out_d);
+  S2S_LAUNCH_CHECK();
+  return S2S_OK;
 }
 
 // One pass of all decoder layers over R = sum of the segments' rows, already embedded in m->x.  A segment is the new rows of
@@ -369,8 +418,7 @@ int llama_prefill_rows(s2s_llama* m, int slot, int n, float* logits_out_d, int32
       S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
       last = m->last_logits;
     }
-    argmax_row_kernel<<<1, 1024, 0, st>>>(last, c.vocab, next_id_d);
-    S2S_LAUNCH_CHECK();
+    S2S_CHECK(prefill_choose(m, slot, last, past + n, next_id_d, st));
   }
   m->len[slot] = past + n;
   return S2S_OK;
@@ -411,8 +459,8 @@ int llama_prefill_batch(s2s_llama* m, const int32_t* slots_h, int B, const int32
     S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
   }
   for (int b = 0; b < B; ++b) {
-    argmax_row_kernel<<<1, 1024, 0, st>>>(m->batch_logits + (size_t)b * c.vocab, c.vocab, next_ids_d + b);
-    S2S_LAUNCH_CHECK();
+    S2S_CHECK(seen_add(m, slots_h[b], m->ids_d + segs[b].off, n_h[b], st));
+    S2S_CHECK(prefill_choose(m, slots_h[b], m->batch_logits + (size_t)b * c.vocab, segs[b].past + n_h[b], next_ids_d + b, st));
   }
   for (int b = 0; b < B; ++b) m->len[slots_h[b]] += n_h[b];
   return S2S_OK;
@@ -567,6 +615,32 @@ int s2s_llama_finalize(s2s_llama* m) {
 int s2s_llama_session_reset(s2s_llama* m, int32_t slot) {
   S2S_REQUIRE(m && slot >= 0 && slot < m->cfg.max_sessions, "llama session_reset: bad slot %d", slot);
   m->len[slot] = 0;
+  m->seen_stale[slot] = 1;
+  return S2S_OK;
+}
+
+int s2s_llama_set_sampling(s2s_llama* m, int32_t slot, const s2s_sampling* s) {
+  S2S_REQUIRE(m && slot >= 0 && slot < m->cfg.max_sessions, "llama set_sampling: bad slot %d", slot);
+  SampSlot t = samp_greedy();
+  if (s) {
+    S2S_REQUIRE(!s->do_sample || s->temperature > 0.f, "llama set_sampling: do_sample needs temperature > 0 (got %g)", (double)s->temperature);
+    S2S_REQUIRE(s->top_p > 0.f && s->top_p <= 1.f, "llama set_sampling: top_p %g outside (0, 1]", (double)s->top_p);
+    S2S_REQUIRE(s->top_k >= 0, "llama set_sampling: top_k %d < 0", s->top_k);
+    S2S_REQUIRE(s->repetition_penalty > 0.f, "llama set_sampling: repetition_penalty %g <= 0", (double)s->repetition_penalty);
+    S2S_REQUIRE(s->min_new_tokens >= 0, "llama set_sampling: min_new_tokens %d < 0", s->min_new_tokens);
+    S2S_REQUIRE(s->n_eos >= 0 && s->n_eos <= 8, "llama set_sampling: %d EOS ids (at most 8)", s->n_eos);
+    for (int e = 0; e < s->n_eos; ++e)
+      S2S_REQUIRE(s->eos_ids[e] >= 0 && s->eos_ids[e] < m->cfg.vocab, "llama set_sampling: EOS id %d outside the vocabulary", s->eos_ids[e]);
+    t.do_sample = s->do_sample ? 1 : 0;
+    t.temperature = s->do_sample ? s->temperature : 1.f;
+    t.top_k = s->top_k; t.top_p = s->top_p; t.penalty = s->repetition_penalty;
+    t.min_new = s->min_new_tokens; t.n_eos = s->n_eos;
+    for (int e = 0; e < s->n_eos; ++e) t.eos[e] = s->eos_ids[e];
+    t.seed = s->seed;
+    t.active = t.do_sample || t.penalty != 1.f || (t.min_new > 0 && t.n_eos > 0);
+  }
+  t.base = m->samp[slot].base;
+  m->samp[slot] = t;
   return S2S_OK;
 }
 
@@ -584,6 +658,7 @@ int s2s_llama_prefill(s2s_llama* m, int32_t slot, const int32_t* ids_h, int32_t 
   if (c.compute_dtype == S2S_BF16) embed_gather_kernel<__nv_bfloat16><<<n, 256, 0, st>>>(m->ids_d, (const __nv_bfloat16*)m->embed, m->x, c.d_model);
   else embed_gather_kernel<__half><<<n, 256, 0, st>>>(m->ids_d, (const __half*)m->embed, m->x, c.d_model);
   S2S_LAUNCH_CHECK();
+  S2S_CHECK(seen_add(m, slot, m->ids_d, n, st));
   return llama_prefill_rows(m, slot, n, logits_out_d, next_id_d, nullptr, st);
 }
 
@@ -634,12 +709,20 @@ int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int3
   }
   S2S_CHECK_CUDA(cudaMemcpyAsync(m->slot_d, slots_h, B * 4, cudaMemcpyHostToDevice, st));
   S2S_CHECK_CUDA(cudaMemcpyAsync(m->pos_d, pos_h, B * 4, cudaMemcpyHostToDevice, st));
+  SampSlot samp_h[MAX_DEC_B];
+  bool any_samp = false;
+  for (int b = 0; b < B; ++b) {
+    samp_h[b] = m->samp[slots_h[b]];
+    any_samp |= samp_h[b].active != 0;
+    S2S_CHECK(seen_clear_if_reset(m, slots_h[b], st));
+  }
+  if (any_samp) S2S_CHECK_CUDA(cudaMemcpyAsync(m->samp_d, samp_h, B * sizeof(SampSlot), cudaMemcpyHostToDevice, st));
   S2S_CHECK_CUDA(cudaStreamSynchronize(st));
   LlamaDecParams p{};
   llama_fill_dec_params(m, p);
   p.B = B; p.slot = m->slot_d; p.pos = m->pos_d; p.max_len = max_len;
   p.first_ids = first_ids_d; p.n_steps = n_steps; p.eos = eos_id; p.out_ids = ids_out_d; p.out_len = len_out_d;
-  p.forced = forced_d; p.logits_out = logits_out_d;
+  p.forced = forced_d; p.logits_out = logits_out_d; p.samp = any_samp ? m->samp_d : nullptr;
   S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->debug_phases, st));
   for (int b = 0; b < B; ++b) m->len[slots_h[b]] += n_steps;
   return S2S_OK;
@@ -669,7 +752,7 @@ int s2s_llama_generate(s2s_llama* m, int32_t slot, const int32_t* prompt_h, int3
     const bool last = o + n >= n_prompt;
     S2S_CHECK(s2s_llama_prefill(m, slot, prompt_h + o, n, nullptr, last ? m->next_id : nullptr, stream));
   }
-  // ids_out[0] = argmax of the prompt's last position; the decode kernel then feeds it and produces the rest
+  // ids_out[0] = the token chosen from the prompt's last position; the decode kernel then feeds it and produces the rest
   int first = 0;
   S2S_CHECK_CUDA(cudaMemcpyAsync(&first, m->next_id, 4, cudaMemcpyDeviceToHost, st));
   int n_dec = 0;

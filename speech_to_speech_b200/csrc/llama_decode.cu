@@ -8,6 +8,8 @@
 //   0: RMSNorm + QKV projection + RoPE + KV append   1: GQA attention items (32-key blocks, last split merges)
 //   2: o_proj + residual                             3: RMSNorm + gate/up projection + SwiGLU     4: down + residual
 //   then 5L: final RMSNorm + lm_head + per-CTA argmax      5L+1: global argmax, EOS bookkeeping, next embedding
+// Sessions with sampling parameters (sampling.cuh) have their logits row stored in phase 5L and chosen from it by the CTA
+// that owns the session in phase 5L+1: no extra phase, no extra grid barrier.
 // Qwen3 family (qk_norm, transformers modeling_qwen3.py Qwen3Attention): phase 0 stores RAW q / k; the per-head
 // RMSNorm(head_dim) + RoPE is folded into the attention items of phase 1 (ld_qk_prepare), so the phase count stays 5 per
 // layer (a sixth phase would add one grid barrier per layer and step to the TTS frame loop).
@@ -139,17 +141,28 @@ __device__ __forceinline__ bool ld_has_gemv(const LlamaDecParams& p, int step, i
   return k == 0 || k == 2 || k == 3 || k == 4 || (k == 6 && ld_has_head(p, step));
 }
 
+// s_samp: the tail-round reduction buffer of the projections, idle in this phase (the look-ahead issued between the
+// previous barrier's arrive and wait only fills the weight ring and the norm-weight buffer)
 template <typename T>
-__device__ __noinline__ void ld_select(const LlamaDecParams& p, int step, float* s_aux) {
+__device__ __noinline__ void ld_select(const LlamaDecParams& p, int step, float* s_aux, SampShared& s_samp) {
   const int d = p.d, B = p.B;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int* s_feed = reinterpret_cast<int*>(s_aux);
 #pragma unroll 1
   for (int b = blockIdx.x; b < B; b += gridDim.x) {
     __syncthreads();
+    const SampSlot* sc = p.samp ? p.samp + b : nullptr;
+    const bool sampled = sc && sc->active && ld_has_head(p, step);
+    int stok = 0;
+    if (sampled) {   // the whole CTA selects from the step's logits row; pos[b] + 1 = position of the predicted token
+      const float* row = p.logits_out ? p.logits_out + ((long long)step * B + b) * p.vocab : p.samp_rows + (long long)b * p.vocab;
+      stok = sample_row(row, p.vocab, *sc, p.seen + (long long)p.slot[b] * p.seen_words, p.pos[b] + 1, s_samp);
+    }
     if (warp == 0) {
       float bv = -INFINITY; int bi = 0x7fffffff;
-      if (ld_has_head(p, step)) {
+      if (sampled) {
+        bi = stok;
+      } else if (ld_has_head(p, step)) {
 #pragma unroll 1
         for (int c = lane; c < (int)gridDim.x; c += 32) {
           const float v = __ldcg(p.cand_val + b * gridDim.x + c); const int i = __ldcg(p.cand_idx + b * gridDim.x + c);
@@ -174,6 +187,10 @@ __device__ __noinline__ void ld_select(const LlamaDecParams& p, int step, float*
         }
         if (p.forced && step == p.n_steps - 1) p.out_len[b] = p.n_steps;
         *s_feed = p.forced ? p.forced[b * p.n_steps + step] : tok;
+        if (sc && sc->penalty != 1.f) {
+          const int f = *s_feed;
+          atomicOr(p.seen + (long long)p.slot[b] * p.seen_words + (f >> 5), 1u << (f & 31));
+        }
         p.pos[b] = p.pos[b] + 1;  // the fed token sits at the next position
       }
     }
@@ -217,7 +234,10 @@ __device__ __forceinline__ bool ld_gemv_args(const LlamaDecParams& p, int step, 
   if (kind == 6 && ld_has_head(p, step)) {
     a.W = ld_multi(p) ? reinterpret_cast<const T*>(p.lm_head) + (long long)(step - 1) * p.head_stride : p.lm_head;
     a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 4; a.suppress = p.suppress;
-    a.logits_out = p.logits_out ? p.logits_out + (long long)step * B * p.vocab : nullptr; a.logits_ld = p.vocab;
+    // sessions that sample read their row back in the select phase: from logits_out when the caller asked for it, else from
+    // the row scratch (every row of such a launch is stored, a few MB against the step's weight stream)
+    a.logits_out = p.logits_out ? p.logits_out + (long long)step * B * p.vocab : p.samp ? p.samp_rows : nullptr;
+    a.logits_ld = p.vocab;
     return true;
   }
   return false;
@@ -268,7 +288,8 @@ __device__ __forceinline__ void ld_phase(const LlamaDecParams& p, int step, int 
     gemv_mma<T, true>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
     gemv_argmax_candidates(best_v, best_i, B, sm.sv, sm.si, p.cand_val, p.cand_idx);
   } else {
-    ld_select<T>(p, step, sm.sv);
+    static_assert(sizeof(SampShared) <= 2 * DEC_THREADS * 16, "sampling scratch must fit the tail-round buffer");
+    ld_select<T>(p, step, sm.sv, *reinterpret_cast<SampShared*>(sm.red));
   }
 }
 
@@ -379,6 +400,12 @@ __global__ void llama_decode_init_kernel(const LlamaDecParams p) {
     p.out_len[b] = 0;
     if (b == 0) { *p.n_done = 0; *p.sync_counter = 0; }
     for (int h = 0; h < p.heads; ++h) p.attn_cnt[b * p.heads + h] = 0u;
+    // the first fed id is in the sequence now: it joins the seen set of a session with a repetition penalty (the select
+    // phase adds the ids fed after it)
+    if (p.samp && p.samp[b].active && p.samp[b].penalty != 1.f) {
+      const int f = p.first_ids[b];
+      atomicOr(p.seen + (long long)p.slot[b] * p.seen_words + (f >> 5), 1u << (f & 31));
+    }
   }
   for (int i = threadIdx.x; i < p.n_steps; i += blockDim.x) p.out_ids[b * p.n_steps + i] = p.eos;
 }

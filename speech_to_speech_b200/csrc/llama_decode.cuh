@@ -1,6 +1,7 @@
 // llama_decode.cuh -- parameters of the persistent Llama-family greedy-decode kernel.
 #pragma once
 #include "common.cuh"
+#include "sampling.cuh"
 
 struct LlamaDecLayer {          // device pointers; 16-bit weights [out, in]: TILED layout (weight_tiles.cu) in the kernel's table
   const void* w_qkv;            // [(H + 2 KV) * hd, d]; q and k rows stored pair-adjacent for RoPE (see llama.cu)
@@ -61,6 +62,11 @@ struct LlamaDecParams {
   unsigned long long* trace;    // optional [cap][3] globaltimer stamps of CTA 0 (phase begin, body end, barrier exit)
   int trace_cap;
   int sync_relaxed;             // 1: barrier waits without the acquire fence (A/B measurement aid)
+  // ---- per-session token choice (sampling.cuh); samp == null: every session takes the argmax-candidate path ----
+  const SampSlot* samp;         // [B] or null
+  float* samp_rows;             // [B][vocab] fp32 logits rows of the step (used when logits_out is null)
+  unsigned int* seen;           // [slots][seen_words] ids seen by each slot (repetition penalty)
+  int seen_words;
 };
 
 int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int debug_phases, cudaStream_t stream);

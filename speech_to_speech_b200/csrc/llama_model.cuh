@@ -59,6 +59,13 @@ struct s2s_llama {
   size_t embed_table_elems = 0, head_table_elems = 0, head_t_table_elems = 0;
   float* qn = nullptr;                   // qk_norm: normalised q rows of the decode step [B][H*hd]
   float* kraw = nullptr;                 // qk_norm: raw k rows of the decode step [B][KV*hd]
+  // token choice per slot (s2s_llama_set_sampling); active == 0: argmax
+  std::vector<SampSlot> samp;            // [max_sessions]
+  SampSlot* samp_d = nullptr;            // [MAX_DEC_B] the launch's packed parameters
+  float* samp_rows = nullptr;            // [MAX_DEC_B][vocab]
+  unsigned int* seen = nullptr;          // [max_sessions][seen_words]
+  int seen_words = 0;
+  std::vector<char> seen_stale;          // [max_sessions] reset since the seen set was last emptied
 };
 
 

@@ -285,7 +285,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, kv_
 
 
 class LlamaEngine:
-    """Llama-family LLM on one H100: wgmma prefill + persistent greedy decode with a per-session KV cache."""
+    """Llama-family LLM on one H100: wgmma prefill + persistent decode (greedy, or sampled per slot) with a per-session KV cache."""
 
     def __init__(self, geometry: Mapping[str, float], dtype: str = "bfloat16", max_sessions: int = 1,
                  max_positions: int = 2048, max_prefill: int = 512, device: int = 0, lane: int = 0, lanes: int = 1):
@@ -322,6 +322,18 @@ class LlamaEngine:
 
     def reset(self, slot: int = 0) -> None:
         check(self.lib.s2s_llama_session_reset(self.handle, slot), "s2s_llama_session_reset")
+
+    def set_sampling(self, slot: int, *, do_sample: bool = False, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
+                     repetition_penalty: float = 1.0, min_new_tokens: int = 0, eos_ids: Sequence[int] = (), seed: int = 0) -> None:
+        """Token choice of `slot` for the following prefill and decode calls (include/s2s_b200.h s2s_llama_set_sampling):
+        repetition penalty and min_new_tokens apply to greedy slots too; temperature / top_k / top_p only with do_sample.
+        The defaults are greedy argmax.  Set it before the response's prefill."""
+        eos = [int(e) for e in eos_ids]
+        if len(eos) > 8:
+            raise ValueError(f"at most 8 EOS ids, got {len(eos)}")
+        s = _lib.Sampling(int(bool(do_sample)), float(temperature), int(top_k), float(top_p), float(repetition_penalty),
+                          int(min_new_tokens), len(eos), (C.c_int32 * 8)(*eos), int(seed) & 0xFFFFFFFFFFFFFFFF)
+        check(self.lib.s2s_llama_set_sampling(self.handle, slot, C.byref(s)), "s2s_llama_set_sampling")
 
     def prefill(self, slot: int, ids: Sequence[int], return_logits: bool = False):
         """Append `ids` to the session.  Returns (next_id cuda int32[1], logits cuda f32[n, vocab] or None)."""

@@ -16,6 +16,8 @@ from __future__ import annotations
 
 import contextlib
 import logging
+import os
+import random
 import threading
 from typing import Any, Callable, Iterator, Optional, Sequence
 
@@ -37,14 +39,55 @@ LLAMA_GEOMETRIES = {
 }
 
 
+# GenerationConfig fields the device sampler does not implement, with the value at which they do nothing
+_UNSUPPORTED_GENERATION = {"min_p": 0.0, "typical_p": 1.0, "epsilon_cutoff": 0.0, "eta_cutoff": 0.0, "num_beams": 1,
+                           "no_repeat_ngram_size": 0}
+
+
+def resolve_generation(gen_kwargs: dict, generation_config: Any = None) -> dict:
+    """The token-choice options of a response, resolved the way transformers' generate() resolves them: its defaults
+    (GenerationConfig._get_default_generation_params), overlaid by the checkpoint's generation_config, overlaid by gen_kwargs.
+    Returns the keyword arguments of LlamaEngine.set_sampling (without eos_ids / seed).  Raises ValueError for what the
+    kernels do not implement instead of silently decoding differently."""
+    from transformers import GenerationConfig
+    eff = dict(GenerationConfig._get_default_generation_params())
+    if generation_config is not None:
+        src = generation_config.to_dict() if hasattr(generation_config, "to_dict") else dict(generation_config)
+        eff.update({k: v for k, v in src.items() if v is not None})
+    eff.update({k: v for k, v in gen_kwargs.items() if v is not None})
+    for k, off in _UNSUPPORTED_GENERATION.items():
+        v = eff.get(k)
+        if v is not None and v != off and not (k == "num_beams" and int(v) <= 1):
+            raise ValueError(f"`{k}` (={v}) is not supported by B200LanguageModelHandler: its sampler implements repetition_penalty, "
+                             f"min_new_tokens, temperature, top_k and top_p only")
+    do_sample = bool(eff.get("do_sample") or False)
+    temperature = float(eff.get("temperature") if eff.get("temperature") is not None else 1.0)
+    top_k = int(eff.get("top_k") or 0)
+    top_p = float(eff.get("top_p") if eff.get("top_p") is not None else 1.0)
+    penalty = float(eff.get("repetition_penalty") if eff.get("repetition_penalty") is not None else 1.0)
+    if do_sample and not temperature > 0.0:
+        raise ValueError(f"`temperature` (={temperature}) has to be a strictly positive float, otherwise your next token scores will be "
+                         "invalid. If you're looking for greedy decoding strategies, set `do_sample=False`.")
+    if do_sample and not 0.0 < top_p <= 1.0:
+        raise ValueError(f"`top_p` has to be a float > 0 and < 1, but is {top_p}")
+    if do_sample and top_k < 0:
+        raise ValueError(f"`top_k` has to be a strictly positive integer, but is {top_k}")
+    if not penalty > 0.0:
+        raise ValueError(f"`penalty` has to be a strictly positive float, but is {penalty}")
+    return dict(do_sample=do_sample, temperature=temperature if do_sample else 1.0, top_k=top_k if do_sample else 0,
+                top_p=top_p if do_sample else 1.0, repetition_penalty=penalty, min_new_tokens=int(eff.get("min_new_tokens") or 0))
+
+
 class TokenStreamer:
-    """Greedy generation as an iterator of text fragments (the role TextIteratorStreamer plays in the reference)."""
+    """Generation as an iterator of text fragments (the role TextIteratorStreamer plays in the reference)."""
 
     def __init__(self, engine: Any, decode_text: Callable[[Sequence[int]], str], eos_ids: Sequence[int], chunk: int = 8, slot: int = 0,
                  decode_chunk: Optional[Callable[[int, int, int, int], list]] = None, lock: Optional[Any] = None,
-                 context: Optional[Callable[[], Any]] = None, prefill: Optional[Callable[[int, Sequence[int]], int]] = None):
+                 context: Optional[Callable[[], Any]] = None, prefill: Optional[Callable[..., int]] = None,
+                 sampling: Optional[Callable[[], dict]] = None):
         import contextlib
         self._context = context or contextlib.nullcontext   # the lane's CUDA stream for this thread's GPU calls
+        self._sampling = sampling   # -> LlamaEngine.set_sampling kwargs of the next response (None: leave the slot as it is)
         self.engine, self.decode_text, self.eos_ids, self.chunk, self.slot = engine, decode_text, set(int(e) for e in eos_ids), max(1, chunk), slot
         self.generated: list[int] = []
         self._po = self._ro = 0   # incremental detokenisation window
@@ -86,11 +129,14 @@ class TokenStreamer:
             prompt_ids = prompt_ids[-(room - 1):]
         max_new_tokens = max(1, min(int(max_new_tokens), room - len(prompt_ids)))
         nxt = None
+        sampling = self._sampling() if self._sampling is not None else None
         if self._prefill is not None:
-            tok = int(self._prefill(self.slot, prompt_ids))
+            tok = int(self._prefill(self.slot, prompt_ids, sampling) if sampling is not None else self._prefill(self.slot, prompt_ids))
         else:
             with self._lock, self._context():
                 eng.reset(self.slot)
+                if sampling is not None:
+                    eng.set_sampling(self.slot, **sampling)
                 for o in range(0, len(prompt_ids), max_prefill):
                     nxt, _ = eng.prefill(self.slot, list(prompt_ids[o:o + max_prefill]))
                 tok = int(nxt[0])
@@ -129,8 +175,9 @@ class _LlamaBundle:
     by a lock, decode chunks of concurrent sessions merged into one launch by the SessionBatcher."""
 
     def __init__(self, engine: Any, tokenizer: Any, eos_ids: list, max_sessions: int, batch_wait_s: float, lane: int = 0, lanes: int = 1,
-                 batch_gap_s: Optional[float] = None):
+                 batch_gap_s: Optional[float] = None, generation_config: Any = None):
         self.engine, self.tokenizer, self.eos_ids = engine, tokenizer, eos_ids
+        self.generation_config = generation_config   # the checkpoint's (None for random weights)
         self.lane, self.lanes = lane, lanes
         self.lock = threading.Lock()
         self._free = list(range(max_sessions))
@@ -156,7 +203,7 @@ class _LlamaBundle:
             self._free.append(slot)
 
     def _run_prefill(self, items: list) -> list:
-        """items: (slot, prompt ids).  Fresh prompts that fit one pass together are prefilled by ONE s2s_llama_prefill_batch
+        """items: (slot, prompt ids[, set_sampling kwargs]).  Each slot is reset and gets its token choice first.  Fresh prompts that fit one pass together are prefilled by ONE s2s_llama_prefill_batch
         call (one pass over the weights for all of them); the rest go one by one, over-long prompts in max_prefill chunks."""
         eng = self.engine
         cap = int(eng.cfg.max_prefill)
@@ -178,8 +225,11 @@ class _LlamaBundle:
                         nx, _ = eng.prefill(items[i][0], list(items[i][1][o:o + cap]))
                     out[i] = int(nx[0])
                 group, rows = [], 0
-            for i, (slot, ids) in enumerate(items):
+            for i, it in enumerate(items):
+                slot, ids = it[0], it[1]
                 eng.reset(slot)
+                if len(it) > 2 and it[2] is not None:
+                    eng.set_sampling(slot, **it[2])
                 if len(ids) > cap:
                     flush()
                     group = [i]
@@ -192,11 +242,12 @@ class _LlamaBundle:
             flush()
         return out
 
-    def prefill(self, slot: int, ids: Sequence[int]) -> int:
-        """Reset the session and run its prompt; concurrent sessions' prompts share one pass over the weights."""
+    def prefill(self, slot: int, ids: Sequence[int], sampling: Optional[dict] = None) -> int:
+        """Reset the session, set its token choice (under the lock, on the lane's stream) and run its prompt; concurrent
+        sessions' prompts share one pass over the weights."""
         if self.batcher is None:
-            return self._run_prefill([(slot, list(ids))])[0]
-        return self.batcher.call(("prefill",), (slot, list(ids)))
+            return self._run_prefill([(slot, list(ids), sampling)])[0]
+        return self.batcher.call(("prefill",), (slot, list(ids), sampling))
 
     def _run_batch(self, key: tuple, items: list) -> list:
         import torch
@@ -278,10 +329,9 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
         from .. import engine as E
         dev = int(device.split(":")[1]) if ":" in device else 0
         self.gen_kwargs = dict(gen_kwargs)
-        if self.gen_kwargs.get("do_sample") or float(self.gen_kwargs.get("temperature") or 0.0) > 0.0:
-            logger.warning("B200LanguageModelHandler decodes greedily on the device: do_sample / temperature are ignored")
-        if int(self.gen_kwargs.get("min_new_tokens") or 0) > 0:
-            logger.warning("B200LanguageModelHandler: min_new_tokens is ignored (EOS always ends the reply)")
+        seed = self.gen_kwargs.pop("seed", None)
+        # one 64-bit sampling seed per response, drawn from a generator seeded by gen_kwargs["seed"] (OS entropy when absent)
+        self._seed_rng = random.Random(int(seed) if seed is not None else int.from_bytes(os.urandom(8), "little"))
         self.stream_chunk_tokens = int(self.gen_kwargs.pop("stream_chunk_tokens", 8))
         max_pos = int(self.gen_kwargs.pop("max_positions", 4096))
         max_sessions = max(1, int(self.gen_kwargs.pop("max_sessions", 1)))
@@ -302,7 +352,13 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
                 engine = E.LlamaEngine(geom, dtype=torch_dtype, max_sessions=max_sessions, max_positions=max_pos, max_prefill=512, device=dev, lane=lane, lanes=lanes)
                 engine.init_random(int(parts[2]) if len(parts) > 2 else 0)
                 return _LlamaBundle(engine, _IdTokenizer(geom["vocab"]), [geom["vocab"] - 1], max_sessions, batch_wait_s, lane, lanes, batch_gap_s)
-            from transformers import AutoModelForCausalLM, AutoTokenizer
+            # the checkpoint is read before the weights are loaded so that unsupported options fail fast
+            from transformers import AutoModelForCausalLM, AutoTokenizer, GenerationConfig
+            try:
+                ckpt_gen = GenerationConfig.from_pretrained(model_name)
+            except OSError:
+                ckpt_gen = None
+            resolve_generation(self.gen_kwargs, ckpt_gen)
             tokenizer = AutoTokenizer.from_pretrained(model_name)
             hf = AutoModelForCausalLM.from_pretrained(model_name)
             c = hf.config
@@ -312,15 +368,24 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
             eos = hf.generation_config.eos_token_id
             eos_ids = list(eos) if isinstance(eos, (list, tuple)) else [int(eos)]
             del hf
-            return _LlamaBundle(engine, tokenizer, eos_ids, max_sessions, batch_wait_s, lane, lanes, batch_gap_s)
+            return _LlamaBundle(engine, tokenizer, eos_ids, max_sessions, batch_wait_s, lane, lanes, batch_gap_s, ckpt_gen)
 
+        if model_name.startswith("random:"):
+            resolve_generation(self.gen_kwargs)
         self._shared_key = ("llama", model_name, torch_dtype, dev, max_sessions, max_pos, lane, lanes) if max_sessions > 1 else None
         self.bundle = acquire_shared(self._shared_key, build, lambda b: b.close()) if self._shared_key else build()
         self.engine, self.tokenizer, self.eos_ids = self.bundle.engine, self.bundle.tokenizer, self.bundle.eos_ids
+        self.sampling = resolve_generation(self.gen_kwargs, getattr(self.bundle, "generation_config", None))
         self.slot = self.bundle.acquire_slot()
         self.streamer = TokenStreamer(self.engine, lambda ids: self.tokenizer.decode(list(ids), skip_special_tokens=True),
                                       self.eos_ids, self.stream_chunk_tokens, slot=self.slot, decode_chunk=self.bundle.decode_chunk,
-                                      lock=self.bundle.lock, context=self.bundle.lane_context, prefill=self.bundle.prefill)
+                                      lock=self.bundle.lock, context=self.bundle.lane_context, prefill=self.bundle.prefill,
+                                      sampling=self.next_sampling)
+
+    def next_sampling(self) -> dict:
+        """LlamaEngine.set_sampling kwargs of the next response: the resolved options, the model's EOS ids (for
+        min_new_tokens) and a fresh 64-bit seed."""
+        return dict(self.sampling, eos_ids=list(self.eos_ids)[:8], seed=self._seed_rng.getrandbits(64))
 
     def generate_text_stream(self, prompt_ids: Sequence[int], max_new_tokens: Optional[int] = None,
                              should_stop: Callable[[], bool] = lambda: False) -> Iterator[str]:
