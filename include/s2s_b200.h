@@ -244,7 +244,8 @@ int32_t s2s_codec_total_upsample(s2s_codec* m);       /* samples per frame (1920
  * instruct, chunk_size, max_new_tokens, non_streaming_mode)` (S/TTS/qwen3_tts_handler.py:946-978; warm-up :555-572).
  * The package is absent everywhere; the arithmetic is pinned to the published cousin, the Qwen3-Omni talker in
  * transformers (modeling_qwen3_omni_moe.py: talker :3029-3281, code predictor :2550-2731, prompt layout :3842-3905) with
- * a dense talker MLP and greedy selection (oracle/qwen3tts_ref.py) -- UNPINNED against the real Qwen3-TTS.
+ * a dense talker MLP (oracle/qwen3tts_ref.py) -- UNPINNED against the real Qwen3-TTS.  Codes are chosen greedily unless
+ * s2s_qwen3tts_set_sampling asks for the cousin's sampling.
  * One frame = 1 talker step (first codebook, special ids suppressed) + n_groups code-predictor steps (residual
  * codebooks) + the next talker input (sum of the frame's code embeddings + the next text embedding / tts_pad). */
 typedef struct {
@@ -273,9 +274,20 @@ int s2s_qwen3tts_bind_tensor(s2s_qwen3tts* m, const char* name, const void* data
 int s2s_qwen3tts_init_random(s2s_qwen3tts* m, uint64_t seed);
 int s2s_qwen3tts_finalize(s2s_qwen3tts* m);
 /* Start an utterance in `slot`: builds the prompt ([im_start, assistant, newline] + text, codec prefix with the speaker
- * id), prefills the talker and stages the first frame's input.  text_ids_h: >= 1 text token ids. */
+ * id), prefills the talker and stages the first frame's input.  text_ids_h: >= 1 text token ids.  Resets the slot's
+ * token choice to greedy and empties its repetition-penalty set. */
 int s2s_qwen3tts_prefill(s2s_qwen3tts* m, int32_t slot, const int32_t* text_ids_h, int32_t n_text, int32_t speaker_id,
                          void* stream);
+/* Token choice of the utterance just prefilled in `slot` (call it after s2s_qwen3tts_prefill); NULL = greedy argmax.
+ * The fields and range checks are those of s2s_llama_set_sampling, in the same logits-processor order (the talker's
+ * suppressed special ids are -inf before any of it).  min_new_tokens must be 0 and the EOS ids are ignored: codec_eos is
+ * the only stop.  The code predictor has no repetition penalty (anything but 1 is rejected).  The talker's penalty acts on
+ * the first codes of the frames kept since prefill (the forced ones under teacher forcing), not on the prompt's codec ids
+ * (the cousin's talker.generate gets no input_ids).  Draws: Philox4x64-10 keyed by the struct's seed (pass the same seed to
+ * both) with counter [id, position, stream, 0] -- talker: stream 0, position of the predicted code in the talker's
+ * sequence; predictor: stream 1 + the frame's index since prefill, position of the predicted code in the predictor's
+ * sequence -- so a session's codes do not depend on its batch or on how its frames are split into calls. */
+int s2s_qwen3tts_set_sampling(s2s_qwen3tts* m, int32_t slot, const s2s_sampling* talker, const s2s_sampling* predictor);
 /* Generate n_frames frames for the B (<= s2s_qwen3tts_max_batch) sessions slots_h[B] in lock step: 3 persistent
  * launches per frame serve all of them.  codes_out_d [B][n_frames][n_groups] i32.  A session whose first code is
  * codec_eos has finished: the caller drops that frame and everything after it (frames_done is not advanced past it).
@@ -283,6 +295,12 @@ int s2s_qwen3tts_prefill(s2s_qwen3tts* m, int32_t slot, const int32_t* text_ids_
  * still the models' own decisions, the given codes are what is fed forward and kept.  Asynchronous on `stream`. */
 int s2s_qwen3tts_decode_frames(s2s_qwen3tts* m, const int32_t* slots_h, int32_t B, int32_t n_frames,
                                int32_t* codes_out_d, const int32_t* forced_codes_d, void* stream);
+/* Test hook: s2s_qwen3tts_decode_frames plus the logits rows each code was chosen from (optional, NULL = not stored):
+ * talker_logits_out_d [n_frames][B][vocab] (suppressed ids -inf) and pred_logits_out_d [n_frames][n_groups][B][cp_vocab]
+ * (step 0 predicts nothing and is left unwritten). */
+int s2s_qwen3tts_decode_frames_logits(s2s_qwen3tts* m, const int32_t* slots_h, int32_t B, int32_t n_frames,
+                                      int32_t* codes_out_d, const int32_t* forced_codes_d, float* talker_logits_out_d,
+                                      float* pred_logits_out_d, void* stream);
 /* Waveform of the newest `n_new` frames of `slot` (codes kept by the library since prefill), decoded behind up to
  * `left_context` frames of history (Qwen3OmniMoeCode2Wav.chunked_decode); wav_out_d f32 [n_new * 1920 (max)]. */
 int s2s_qwen3tts_decode_audio(s2s_qwen3tts* m, int32_t slot, int32_t n_new, int32_t left_context, float* wav_out_d,

@@ -24,7 +24,8 @@ EXPORTED = [
     "s2s_codec_create", "s2s_codec_destroy", "s2s_codec_bind_tensor", "s2s_codec_init_random", "s2s_codec_finalize",
     "s2s_codec_decode", "s2s_codec_samples", "s2s_codec_total_upsample",
     "s2s_qwen3tts_create", "s2s_qwen3tts_destroy", "s2s_qwen3tts_bind_tensor", "s2s_qwen3tts_init_random",
-    "s2s_qwen3tts_finalize", "s2s_qwen3tts_prefill", "s2s_qwen3tts_decode_frames", "s2s_qwen3tts_decode_audio", "s2s_qwen3tts_decode_audio_batch",
+    "s2s_qwen3tts_finalize", "s2s_qwen3tts_prefill", "s2s_qwen3tts_set_sampling", "s2s_qwen3tts_decode_frames",
+    "s2s_qwen3tts_decode_frames_logits", "s2s_qwen3tts_decode_audio", "s2s_qwen3tts_decode_audio_batch",
     "s2s_qwen3tts_set_frames", "s2s_qwen3tts_frames", "s2s_qwen3tts_max_batch", "s2s_qwen3tts_codec", "s2s_qwen3tts_set_trace",
 ]
 
@@ -152,7 +153,9 @@ def load() -> C.CDLL:
     lib.s2s_qwen3tts_init_random.argtypes = [vp, C.c_uint64]
     lib.s2s_qwen3tts_finalize.argtypes = [vp]
     lib.s2s_qwen3tts_prefill.argtypes = [vp, i32, C.POINTER(i32), i32, i32, vp]
+    lib.s2s_qwen3tts_set_sampling.argtypes = [vp, i32, C.POINTER(Sampling), C.POINTER(Sampling)]
     lib.s2s_qwen3tts_decode_frames.argtypes = [vp, C.POINTER(i32), i32, i32, vp, vp, vp]
+    lib.s2s_qwen3tts_decode_frames_logits.argtypes = [vp, C.POINTER(i32), i32, i32, vp, vp, vp, vp, vp]
     lib.s2s_qwen3tts_decode_audio.argtypes = [vp, i32, i32, i32, vp, C.POINTER(i32), vp]
     lib.s2s_qwen3tts_decode_audio_batch.argtypes = [vp, C.POINTER(i32), i32, i32, i32, vp, i64, C.POINTER(i32), vp]
     lib.s2s_qwen3tts_set_frames.argtypes = [vp, i32, i32]

@@ -301,6 +301,29 @@ void llama_fill_dec_params(s2s_llama* m, LlamaDecParams& p) {
   p.samp_rows = m->samp_rows; p.seen = m->seen; p.seen_words = m->seen_words;
 }
 
+int samp_from_abi(const s2s_sampling* s, int vocab, const char* who, SampSlot* out) {
+  SampSlot t = samp_greedy();
+  if (s) {
+    S2S_REQUIRE(!s->do_sample || s->temperature > 0.f, "%s: do_sample needs temperature > 0 (got %g)", who, (double)s->temperature);
+    S2S_REQUIRE(s->top_p > 0.f && s->top_p <= 1.f, "%s: top_p %g outside (0, 1]", who, (double)s->top_p);
+    S2S_REQUIRE(s->top_k >= 0, "%s: top_k %d < 0", who, s->top_k);
+    S2S_REQUIRE(s->repetition_penalty > 0.f, "%s: repetition_penalty %g <= 0", who, (double)s->repetition_penalty);
+    S2S_REQUIRE(s->min_new_tokens >= 0, "%s: min_new_tokens %d < 0", who, s->min_new_tokens);
+    S2S_REQUIRE(s->n_eos >= 0 && s->n_eos <= 8, "%s: %d EOS ids (at most 8)", who, s->n_eos);
+    for (int e = 0; e < s->n_eos; ++e)
+      S2S_REQUIRE(s->eos_ids[e] >= 0 && s->eos_ids[e] < vocab, "%s: EOS id %d outside the vocabulary", who, s->eos_ids[e]);
+    t.do_sample = s->do_sample ? 1 : 0;
+    t.temperature = s->do_sample ? s->temperature : 1.f;
+    t.top_k = s->top_k; t.top_p = s->top_p; t.penalty = s->repetition_penalty;
+    t.min_new = s->min_new_tokens; t.n_eos = s->n_eos;
+    for (int e = 0; e < s->n_eos; ++e) t.eos[e] = s->eos_ids[e];
+    t.seed = s->seed;
+    t.active = t.do_sample || t.penalty != 1.f || (t.min_new > 0 && t.n_eos > 0);
+  }
+  *out = t;
+  return S2S_OK;
+}
+
 // The seen set of a slot that was reset is emptied on the stream of the slot's next launch (session_reset takes no stream).
 static int seen_clear_if_reset(s2s_llama* m, int slot, cudaStream_t st) {
   if (!m->seen_stale[slot]) return S2S_OK;
@@ -621,24 +644,8 @@ int s2s_llama_session_reset(s2s_llama* m, int32_t slot) {
 
 int s2s_llama_set_sampling(s2s_llama* m, int32_t slot, const s2s_sampling* s) {
   S2S_REQUIRE(m && slot >= 0 && slot < m->cfg.max_sessions, "llama set_sampling: bad slot %d", slot);
-  SampSlot t = samp_greedy();
-  if (s) {
-    S2S_REQUIRE(!s->do_sample || s->temperature > 0.f, "llama set_sampling: do_sample needs temperature > 0 (got %g)", (double)s->temperature);
-    S2S_REQUIRE(s->top_p > 0.f && s->top_p <= 1.f, "llama set_sampling: top_p %g outside (0, 1]", (double)s->top_p);
-    S2S_REQUIRE(s->top_k >= 0, "llama set_sampling: top_k %d < 0", s->top_k);
-    S2S_REQUIRE(s->repetition_penalty > 0.f, "llama set_sampling: repetition_penalty %g <= 0", (double)s->repetition_penalty);
-    S2S_REQUIRE(s->min_new_tokens >= 0, "llama set_sampling: min_new_tokens %d < 0", s->min_new_tokens);
-    S2S_REQUIRE(s->n_eos >= 0 && s->n_eos <= 8, "llama set_sampling: %d EOS ids (at most 8)", s->n_eos);
-    for (int e = 0; e < s->n_eos; ++e)
-      S2S_REQUIRE(s->eos_ids[e] >= 0 && s->eos_ids[e] < m->cfg.vocab, "llama set_sampling: EOS id %d outside the vocabulary", s->eos_ids[e]);
-    t.do_sample = s->do_sample ? 1 : 0;
-    t.temperature = s->do_sample ? s->temperature : 1.f;
-    t.top_k = s->top_k; t.top_p = s->top_p; t.penalty = s->repetition_penalty;
-    t.min_new = s->min_new_tokens; t.n_eos = s->n_eos;
-    for (int e = 0; e < s->n_eos; ++e) t.eos[e] = s->eos_ids[e];
-    t.seed = s->seed;
-    t.active = t.do_sample || t.penalty != 1.f || (t.min_new > 0 && t.n_eos > 0);
-  }
+  SampSlot t;
+  S2S_CHECK(samp_from_abi(s, m->cfg.vocab, "llama set_sampling", &t));
   t.base = m->samp[slot].base;
   m->samp[slot] = t;
   return S2S_OK;

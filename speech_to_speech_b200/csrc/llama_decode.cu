@@ -187,7 +187,7 @@ __device__ __noinline__ void ld_select(const LlamaDecParams& p, int step, float*
         }
         if (p.forced && step == p.n_steps - 1) p.out_len[b] = p.n_steps;
         *s_feed = p.forced ? p.forced[b * p.n_steps + step] : tok;
-        if (sc && sc->penalty != 1.f) {
+        if (sc && sc->penalty != 1.f && !p.seen_fixed) {
           const int f = *s_feed;
           atomicOr(p.seen + (long long)p.slot[b] * p.seen_words + (f >> 5), 1u << (f & 31));
         }
@@ -402,7 +402,7 @@ __global__ void llama_decode_init_kernel(const LlamaDecParams p) {
     for (int h = 0; h < p.heads; ++h) p.attn_cnt[b * p.heads + h] = 0u;
     // the first fed id is in the sequence now: it joins the seen set of a session with a repetition penalty (the select
     // phase adds the ids fed after it)
-    if (p.samp && p.samp[b].active && p.samp[b].penalty != 1.f) {
+    if (p.samp && p.samp[b].active && p.samp[b].penalty != 1.f && !p.seen_fixed) {
       const int f = p.first_ids[b];
       atomicOr(p.seen + (long long)p.slot[b] * p.seen_words + (f >> 5), 1u << (f & 31));
     }

@@ -67,6 +67,7 @@ struct LlamaDecParams {
   float* samp_rows;             // [B][vocab] fp32 logits rows of the step (used when logits_out is null)
   unsigned int* seen;           // [slots][seen_words] ids seen by each slot (repetition penalty)
   int seen_words;
+  int seen_fixed;               // 1: the caller maintains the seen sets (Qwen3-TTS talker); the launch adds no fed id
 };
 
 int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int debug_phases, cudaStream_t stream);

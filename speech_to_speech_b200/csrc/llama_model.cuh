@@ -79,3 +79,5 @@ int llama_prefill_rows(s2s_llama* m, int slot, int n, float* logits_out_d, int32
 // Everything of LlamaDecParams that does not depend on the call (geometry, weights, workspace).
 void llama_fill_dec_params(s2s_llama* m, LlamaDecParams& p);
 int llama_max_decode_batch_of(const s2s_llama* m);
+// s2s_sampling -> SampSlot with the range checks of s2s_llama_set_sampling (NULL = greedy); errors are prefixed by `who`
+int samp_from_abi(const s2s_sampling* s, int vocab, const char* who, SampSlot* out);

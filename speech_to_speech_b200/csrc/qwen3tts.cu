@@ -3,7 +3,8 @@
 // Reference path: Qwen3TTSHandler._process_custom_voice -> model.generate_custom_voice_streaming(text, speaker, ...,
 // chunk_size, max_new_tokens) (S/TTS/qwen3_tts_handler.py:946-978).  The arithmetic lives in the absent
 // faster-qwen3-tts; it is pinned to the published cousin (transformers Qwen3-Omni talker, modeling_qwen3_omni_moe.py)
-// through oracle/qwen3tts_ref.py -- dense talker MLP, greedy selection -- and UNPINNED against the real upstream.
+// through oracle/qwen3tts_ref.py -- dense talker MLP, greedy selection by default, the cousin's sampling on request
+// (s2s_qwen3tts_set_sampling) -- and UNPINNED against the real upstream.
 //
 // Both models are Qwen3-style decoders, i.e. the Llama-family engine of llama.cu with qk_norm:
 //   talker    : s2s_llama over the codec vocabulary, driven by EMBEDDINGS: the prompt rows are prefilled through the
@@ -12,6 +13,10 @@
 //   predictor : s2s_llama with one embedding table / output head per residual codebook (multi-table mode): one persistent
 //               launch of n_groups steps per frame: [talker hidden, embed(code0)] then one step per residual codebook.
 // A frame for up to 16 sessions is 3 persistent launches + 3 small glue kernels; nothing synchronises with the host.
+// Sampling (sampling.cuh): the talker's draws use Philox stream 0 at the talker position, the predictor's stream 1 + the
+// frame's index since prefill at the predictor position, so a session's codes depend only on (seed, prompt, settings),
+// not on its batch or on how its frames are split into calls.  The talker's repetition penalty acts on the first codes of
+// the frames kept since prefill: frame_finish_kernel adds each kept code0, the decode launch adds nothing (seen_fixed).
 #include <math.h>
 #include <string.h>
 
@@ -89,7 +94,8 @@ __global__ void frame_prepare_kernel(TtsBatch tb, int f, const float* __restrict
 __global__ void frame_mid_kernel(const float* __restrict__ hidden, const float* __restrict__ norm_w, float eps, int d,
                                  float* __restrict__ x_in_p, int* __restrict__ pslot_d, int* __restrict__ ppos_d,
                                  const int* __restrict__ code0, const int* __restrict__ forced /*[B][n_frames][G] or null*/, int f,
-                                 int n_frames, int G, int* __restrict__ code0_feed, int* __restrict__ forced_frame /*[B][G]*/) {
+                                 int n_frames, int G, int* __restrict__ code0_feed, int* __restrict__ forced_frame /*[B][G]*/,
+                                 SampSlot* __restrict__ psamp /*[B] or null*/, TtsBatch tb) {
   __shared__ float red[32];
   const int b = blockIdx.x;
   const float* h = hidden + (long long)b * d;
@@ -103,6 +109,9 @@ __global__ void frame_mid_kernel(const float* __restrict__ hidden, const float* 
   const float r = 1.0f / sqrtf(tot / (float)d + eps);
   for (int i = threadIdx.x; i < d; i += blockDim.x) x_in_p[(long long)b * d + i] = norm_w[i] * (h[i] * r);
   if (threadIdx.x == 0) { pslot_d[b] = b; ppos_d[b] = 0; }
+  // the predictor's positions restart every frame: its draws take the frame's own Philox stream
+  // (frames since prefill = talker positions since prefill: set_frames after codec_eos does not move it)
+  if (threadIdx.x == 0 && psamp) psamp[b].stream = 1ull + (unsigned long long)(tb.pos0[b] - (PROMPT_ROWS - 1) + f);
   // teacher forcing (parity tests): the code predictor is fed the given codes of this frame, its own argmax is still reported
   if (threadIdx.x < G) {
     if (forced) forced_frame[b * G + threadIdx.x] = forced[((long long)b * n_frames + f) * G + threadIdx.x];
@@ -118,7 +127,8 @@ __global__ void frame_finish_kernel(TtsBatch tb, int f, int n_frames, int G, con
                                     const T* __restrict__ talker_embed, const T* __restrict__ pred_embed, long long pred_stride,
                                     int d, const float* __restrict__ trailing_all, long long trailing_stride,
                                     const float* __restrict__ pad_all, float* __restrict__ xnext_all,
-                                    int* __restrict__ codes_out, int* __restrict__ history, long long history_stride) {
+                                    int* __restrict__ codes_out, int* __restrict__ history, long long history_stride,
+                                    unsigned int* __restrict__ tseen, int seen_words) {
   const int b = blockIdx.x, slot = tb.slot[b], fa = tb.frames0[b] + f;
   // reported: the models' own decisions (talker argmax, predictor argmaxes); fed forward / kept: the forced codes if given
   const int* pc = forced_frame ? forced_frame + b * G : pcodes + b * G;
@@ -126,6 +136,8 @@ __global__ void frame_finish_kernel(TtsBatch tb, int f, int n_frames, int G, con
     codes_out[((long long)b * n_frames + f) * G + threadIdx.x] = threadIdx.x == 0 ? code0[b] : pcodes[b * G + threadIdx.x];
     history[(long long)slot * history_stride + (long long)fa * G + threadIdx.x] = pc[threadIdx.x];
   }
+  // the kept first code joins the slot's talker seen set (repetition penalty over the generated code0s only)
+  if (threadIdx.x == 0) atomicOr(tseen + (long long)slot * seen_words + (pc[0] >> 5), 1u << (pc[0] & 31));
   const float* extra = fa < tb.n_trailing[b] ? trailing_all + (long long)slot * trailing_stride + (long long)fa * d
                                               : pad_all + (long long)slot * d;
   for (int i = threadIdx.x; i < d; i += blockDim.x) {
@@ -176,6 +188,9 @@ struct s2s_qwen3tts {
   int *tslot_d = nullptr, *tpos_d = nullptr, *pslot_d = nullptr, *ppos_d = nullptr, *code0 = nullptr, *pcodes = nullptr,
       *tlen = nullptr, *plen = nullptr, *code0_feed = nullptr, *forced_frame = nullptr;
   unsigned char* suppress = nullptr;
+  // token choice per slot (s2s_qwen3tts_set_sampling); reset to greedy by every prefill
+  std::vector<SampSlot> tsamp, psamp;   // [max_sessions] talker, code predictor
+  SampSlot* samp_d = nullptr;           // [2][TTS_MAX_B] the call's packed talker | predictor parameters
 };
 
 namespace {
@@ -268,6 +283,9 @@ int s2s_qwen3tts_create(s2s_ctx* ctx, const s2s_qwen3tts_config* cfg, s2s_qwen3t
     S2S_CHECK(talloc(m, &m->code0_feed, TTS_MAX_B * 4));
     S2S_CHECK(talloc(m, &m->forced_frame, (size_t)TTS_MAX_B * c.n_groups * 4));
     S2S_CHECK(talloc(m, &m->suppress, (size_t)c.vocab));
+    m->tsamp.assign(c.max_sessions, samp_greedy());
+    m->psamp.assign(c.max_sessions, samp_greedy());
+    S2S_CHECK(talloc(m, &m->samp_d, 2 * TTS_MAX_B * sizeof(SampSlot)));
     // transformers generate(): the last 1024 ids of the codec vocabulary except codec_eos are never predicted (TF:3954-3962)
     std::vector<unsigned char> mask((size_t)c.vocab, 0);
     for (int i = c.vocab - 1024; i < c.vocab; ++i) if (i != c.codec_eos) mask[(size_t)i] = 1;
@@ -411,14 +429,40 @@ int s2s_qwen3tts_prefill(s2s_qwen3tts* m, int32_t slot, const int32_t* text_ids_
   S2S_CHECK_CUDA(cudaMemcpyAsync(m->pad_embed + (long long)slot * d, m->proj_out + (long long)(n_text + 5) * d, (size_t)d * 4,
                                  cudaMemcpyDeviceToDevice, st));
   m->talker->len[slot] = 0;
+  // a new utterance: greedy until s2s_qwen3tts_set_sampling, and no first code seen yet (the prompt's codec ids are not
+  // penalised: the cousin's talker.generate gets no input_ids)
+  m->tsamp[slot] = samp_greedy();
+  m->psamp[slot] = samp_greedy();
+  S2S_CHECK_CUDA(cudaMemsetAsync(m->talker->seen + (long long)slot * m->talker->seen_words, 0, (size_t)m->talker->seen_words * 4, st));
   S2S_CHECK(llama_prefill_rows(m->talker, slot, PROMPT_ROWS - 1, nullptr, nullptr, nullptr, st));
   auto& s = m->sess[slot];
   s.n_trailing = n_text; s.frames = 0; s.pos = PROMPT_ROWS - 1; s.active = true;
   return S2S_OK;
 }
 
+int s2s_qwen3tts_set_sampling(s2s_qwen3tts* m, int32_t slot, const s2s_sampling* talker, const s2s_sampling* predictor) {
+  S2S_REQUIRE(m && slot >= 0 && slot < m->cfg.max_sessions, "qwen3tts set_sampling: bad slot %d", slot);
+  for (const s2s_sampling* s : {talker, predictor})
+    S2S_REQUIRE(!s || s->min_new_tokens == 0, "qwen3tts set_sampling: min_new_tokens must be 0 (codec_eos is the only stop)");
+  S2S_REQUIRE(!predictor || predictor->repetition_penalty == 1.f,
+              "qwen3tts set_sampling: the code predictor has no repetition penalty (got %g)", (double)predictor->repetition_penalty);
+  SampSlot t, p;
+  S2S_CHECK(samp_from_abi(talker, m->cfg.vocab, "qwen3tts set_sampling (talker)", &t));
+  S2S_CHECK(samp_from_abi(predictor, m->cfg.cp_vocab, "qwen3tts set_sampling (predictor)", &p));
+  t.n_eos = 0; p.n_eos = 0;
+  m->tsamp[slot] = t;
+  m->psamp[slot] = p;
+  return S2S_OK;
+}
+
 int s2s_qwen3tts_decode_frames(s2s_qwen3tts* m, const int32_t* slots_h, int32_t B, int32_t n_frames, int32_t* codes_out_d,
                                const int32_t* forced_codes_d, void* stream) {
+  return s2s_qwen3tts_decode_frames_logits(m, slots_h, B, n_frames, codes_out_d, forced_codes_d, nullptr, nullptr, stream);
+}
+
+int s2s_qwen3tts_decode_frames_logits(s2s_qwen3tts* m, const int32_t* slots_h, int32_t B, int32_t n_frames, int32_t* codes_out_d,
+                                      const int32_t* forced_codes_d, float* talker_logits_out_d, float* pred_logits_out_d,
+                                      void* stream) {
   S2S_REQUIRE(m && m->finalized && slots_h && codes_out_d, "qwen3tts decode_frames: null argument / not finalized");
   const auto& c = m->cfg;
   const int max_b = tts_max_batch(m);
@@ -438,6 +482,19 @@ int s2s_qwen3tts_decode_frames(s2s_qwen3tts* m, const int32_t* slots_h, int32_t 
   }
   const int d = c.d_model, G = c.n_groups;
   const bool bf = c.compute_dtype == S2S_BF16;
+  // the batch's token-choice tables, one H2D copy per call and only when a session is not greedy (the copy is staged from
+  // this pageable buffer before cudaMemcpyAsync returns)
+  SampSlot samp_h[2 * TTS_MAX_B];
+  bool t_any = false, p_any = false;
+  for (int b = 0; b < B; ++b) {
+    samp_h[b] = m->tsamp[slots_h[b]];
+    samp_h[TTS_MAX_B + b] = m->psamp[slots_h[b]];
+    t_any |= samp_h[b].active != 0;
+    p_any |= samp_h[TTS_MAX_B + b].active != 0;
+  }
+  if (t_any || p_any) S2S_CHECK_CUDA(cudaMemcpyAsync(m->samp_d, samp_h, sizeof(samp_h), cudaMemcpyHostToDevice, st));
+  SampSlot* tsamp_d = t_any ? m->samp_d : nullptr;
+  SampSlot* psamp_d = p_any ? m->samp_d + TTS_MAX_B : nullptr;
   for (int f = 0; f < n_frames; ++f) {
     frame_prepare_kernel<<<B, 256, 0, st>>>(tb, f, m->xnext, d, m->x_in_t, m->tslot_d, m->tpos_d);
     S2S_LAUNCH_CHECK();
@@ -447,10 +504,12 @@ int s2s_qwen3tts_decode_frames(s2s_qwen3tts* m, const int32_t* slots_h, int32_t 
       p.B = B; p.slot = m->tslot_d; p.pos = m->tpos_d; p.max_len = max_pos + f + 1;
       p.x_in = m->x_in_t; p.first_ids = m->code0; p.n_steps = 1; p.eos = -1; p.out_ids = m->code0; p.out_len = m->tlen;
       p.hidden_out = m->hidden; p.suppress = m->suppress;
+      p.samp = tsamp_d; p.seen_fixed = 1;
+      p.logits_out = talker_logits_out_d ? talker_logits_out_d + (long long)f * B * c.vocab : nullptr;
       S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->talker->debug_phases, st));
     }
     frame_mid_kernel<<<B, 256, 0, st>>>(m->hidden, m->talker->norm_f, c.rms_eps, d, m->x_in_p, m->pslot_d, m->ppos_d, m->code0,
-                                        forced_codes_d, f, n_frames, G, m->code0_feed, m->forced_frame);
+                                        forced_codes_d, f, n_frames, G, m->code0_feed, m->forced_frame, psamp_d, tb);
     S2S_LAUNCH_CHECK();
     {   // code predictor: [hidden, embed(code0)] then one step per residual codebook, each with its own table / head
       LlamaDecParams p{};
@@ -459,15 +518,17 @@ int s2s_qwen3tts_decode_frames(s2s_qwen3tts* m, const int32_t* slots_h, int32_t 
       p.x_in = m->x_in_p; p.first_ids = m->code0_feed; p.n_steps = G; p.eos = -1; p.out_ids = m->pcodes; p.out_len = m->plen;
       p.forced = forced_codes_d ? m->forced_frame : nullptr;
       p.embed0 = m->talker->embed; p.embed_stride = (long long)m->pred->embed_table_elems; p.head_stride = (long long)m->pred->head_t_table_elems;
+      p.samp = psamp_d;
+      p.logits_out = pred_logits_out_d ? pred_logits_out_d + (long long)f * G * B * c.cp_vocab : nullptr;
       S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->pred->debug_phases, st));
     }
     const int* ff = forced_codes_d ? m->forced_frame : nullptr;
     if (bf) frame_finish_kernel<__nv_bfloat16><<<B, 256, 0, st>>>(tb, f, n_frames, G, m->pcodes, m->code0, ff, (const __nv_bfloat16*)m->talker->embed,
           (const __nv_bfloat16*)m->pred->embed, (long long)m->pred->embed_table_elems, d, m->trailing, m->trailing_stride, m->pad_embed,
-          m->xnext, codes_out_d, m->history, m->history_stride);
+          m->xnext, codes_out_d, m->history, m->history_stride, m->talker->seen, m->talker->seen_words);
     else frame_finish_kernel<__half><<<B, 256, 0, st>>>(tb, f, n_frames, G, m->pcodes, m->code0, ff, (const __half*)m->talker->embed,
           (const __half*)m->pred->embed, (long long)m->pred->embed_table_elems, d, m->trailing, m->trailing_stride, m->pad_embed,
-          m->xnext, codes_out_d, m->history, m->history_stride);
+          m->xnext, codes_out_d, m->history, m->history_stride, m->talker->seen, m->talker->seen_words);
     S2S_LAUNCH_CHECK();
   }
   for (int b = 0; b < B; ++b) {

@@ -6,8 +6,10 @@
 //   3. z / temperature, top-k (ties with the k-th value kept; 0 or >= vocab = off), top-p (ascending sort, inclusive
 //      cumulative softmax, remove cum <= 1 - top_p, keep >= 1)
 //   4. Gumbel-max over the survivors: argmax_i(z_i - log(-log u_i)), ties -> lowest id, u_i from Philox4x64-10 keyed by the
-//      slot's seed with counter (token id + 1, predicted position, 0, 0) -- the first block numpy.random.Philox(key=seed,
-//      counter=[id, position, 0, 0]) produces -- so a token depends only on (seed, position, logits).
+//      slot's seed with counter (token id + 1, predicted position, stream, 0) -- the first block
+//      numpy.random.Philox(key=seed, counter=[id, position, stream, 0]) produces -- so a token depends only on (seed,
+//      position, stream, logits).  The LLM and the Qwen3-TTS talker draw from stream 0; the Qwen3-TTS code predictor,
+//      whose positions repeat every frame, from stream 1 + the frame's index since the utterance's prefill.
 // Top-k and top-p are exact radix selects over the order-preserving bits of the processed value (8 bits per level, 256-bin
 // shared histograms; top-p's histogram sums probability mass in 2^-40 fixed point, so the sums are deterministic), so
 // the vocabulary is never sorted.  Every pass recomputes the processed value from the row (L2-resident) instead of storing it.
@@ -22,6 +24,7 @@ struct SampSlot {               // per-session parameters of a launch (host-pack
   float temperature, top_p, penalty;
   int eos[8];
   unsigned long long seed;
+  unsigned long long stream;    // Philox counter word 2
 };
 // the parameters of a greedy session
 inline SampSlot samp_greedy() {
@@ -40,8 +43,8 @@ struct SampShared {             // shared scratch of sample_row
 };
 
 __host__ __device__ __forceinline__ unsigned long long samp_philox(unsigned long long seed, unsigned long long c0,
-                                                                   unsigned long long c1) {
-  unsigned long long x0 = c0, x1 = c1, x2 = 0, x3 = 0, k0 = seed, k1 = 0;
+                                                                   unsigned long long c1, unsigned long long c2) {
+  unsigned long long x0 = c0, x1 = c1, x2 = c2, x3 = 0, k0 = seed, k1 = 0;
 #pragma unroll
   for (int r = 0; r < 10; ++r) {
     if (r) { k0 += 0x9E3779B97F4A7C15ull; k1 += 0xBB67AE8584CAA73Bull; }
@@ -224,7 +227,7 @@ static __device__ __noinline__ int sample_row(const float* row, int V, const Sam
   bv = -INFINITY; bi = 0x7fffffff;
   samp_for_each(row, sn, s, mask_eos, V, [&](int i, float z) {
     if (samp_key(z) < thr) return;
-    const unsigned long long r = samp_philox(s.seed, (unsigned long long)i + 1ull, (unsigned long long)pred_pos);
+    const unsigned long long r = samp_philox(s.seed, (unsigned long long)i + 1ull, (unsigned long long)pred_pos, s.stream);
     const double u = (double)(r >> 11) * (1.0 / 9007199254740992.0);
     const double g = (double)z - log(-log(u));
     if (g > bv || (g == bv && i < bi)) { bv = g; bi = i; }

@@ -5,7 +5,7 @@ from __future__ import annotations
 import ctypes as C
 import threading
 from dataclasses import dataclass
-from typing import Mapping, Optional, Sequence
+from typing import Any, Mapping, Optional, Sequence
 
 import numpy as np
 import torch
@@ -531,17 +531,43 @@ class Qwen3TTSEngine:
         arr, n = _lib.i32_array(text_ids)
         check(self.lib.s2s_qwen3tts_prefill(self.handle, slot, arr, n, int(speaker_id), _stream_ptr(self.device)), "s2s_qwen3tts_prefill")
 
-    def decode_frames(self, slots: Sequence[int], n_frames: int, forced: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def set_sampling(self, slot: int, *, talker: Optional[Mapping[str, Any]] = None, predictor: Optional[Mapping[str, Any]] = None,
+                     seed: int = 0) -> None:
+        """Token choice of the utterance just prefilled in `slot` (prefill resets it to greedy): `talker` / `predictor` take
+        the keywords of LlamaEngine.set_sampling (do_sample, temperature, top_k, top_p, repetition_penalty), None = greedy.
+        One seed serves both models (include/s2s_b200.h s2s_qwen3tts_set_sampling)."""
+        def conv(d):
+            if d is None:
+                return None
+            d = dict(d)
+            unknown = set(d) - {"do_sample", "temperature", "top_k", "top_p", "repetition_penalty", "min_new_tokens"}
+            if unknown:
+                raise ValueError(f"unknown sampling options {sorted(unknown)}")
+            return C.byref(_lib.Sampling(int(bool(d.get("do_sample", False))), float(d.get("temperature", 1.0)), int(d.get("top_k", 0)),
+                                         float(d.get("top_p", 1.0)), float(d.get("repetition_penalty", 1.0)),
+                                         int(d.get("min_new_tokens", 0)), 0, (C.c_int32 * 8)(), int(seed) & 0xFFFFFFFFFFFFFFFF))
+        check(self.lib.s2s_qwen3tts_set_sampling(self.handle, slot, conv(talker), conv(predictor)), "s2s_qwen3tts_set_sampling")
+
+    def decode_frames(self, slots: Sequence[int], n_frames: int, forced: Optional[torch.Tensor] = None, return_logits: bool = False):
         """-> codes int32 cuda [B, n_frames, n_groups] (asynchronous).  forced (int32 cuda, same shape): teacher-forced
-        feedback for parity tests; the returned codes are still the models' own decisions."""
+        feedback for parity tests; the returned codes are still the models' own decisions.  return_logits: also the rows
+        the codes were chosen from, (codes, talker f32 [n_frames, B, vocab], predictor f32 [n_frames, n_groups, B, cp_vocab]
+        whose step 0 is unused)."""
         sl, B = _lib.i32_array(slots)
-        codes = torch.empty((B, n_frames, self.n_groups), dtype=torch.int32, device=f"cuda:{self.device}")
+        dev = f"cuda:{self.device}"
+        codes = torch.empty((B, n_frames, self.n_groups), dtype=torch.int32, device=dev)
         if forced is not None:
             forced = forced.to(torch.int32).contiguous()
             assert tuple(forced.shape) == (B, n_frames, self.n_groups)
-        check(self.lib.s2s_qwen3tts_decode_frames(self.handle, sl, B, n_frames, _ptr(codes), _ptr(forced), _stream_ptr(self.device)),
-              "s2s_qwen3tts_decode_frames")
-        return codes
+        if not return_logits:
+            check(self.lib.s2s_qwen3tts_decode_frames(self.handle, sl, B, n_frames, _ptr(codes), _ptr(forced), _stream_ptr(self.device)),
+                  "s2s_qwen3tts_decode_frames")
+            return codes
+        tl = torch.empty((n_frames, B, self.cfg.vocab), dtype=torch.float32, device=dev)
+        pl = torch.full((n_frames, self.n_groups, B, self.cfg.cp_vocab), float("nan"), dtype=torch.float32, device=dev)
+        check(self.lib.s2s_qwen3tts_decode_frames_logits(self.handle, sl, B, n_frames, _ptr(codes), _ptr(forced), _ptr(tl), _ptr(pl),
+                                                         _stream_ptr(self.device)), "s2s_qwen3tts_decode_frames_logits")
+        return codes, tl, pl
 
     def frames(self, slot: int) -> int:
         return int(self.lib.s2s_qwen3tts_frames(self.handle, slot))

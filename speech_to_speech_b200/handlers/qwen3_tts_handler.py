@@ -17,16 +17,24 @@ session-voice logic unchanged; on a machine without the reference it subclasses 
 
 `gen_kwargs["max_sessions"] = N` (or setup kwarg `max_sessions`) shares ONE engine between the N pipeline units of the
 process and merges the chunk requests of concurrently speaking sessions into one launch sequence (tts_model.py).
+
+Sampling: the qwen-tts generation keywords in gen_kwargs (`do_sample, temperature, top_k, top_p, repetition_penalty,
+subtalker_dosample, subtalker_temperature, subtalker_top_k, subtalker_top_p`, tts_model.SAMPLING_KEYWORDS) and
+`sampling_seed` are taken out of gen_kwargs before the base class sees them and validated at setup.  The engine is shared,
+so they travel with every call: `self.model` is then a per-handler view of the shared model that adds them, and a fresh
+64-bit seed from this handler's generator, to generate_custom_voice_streaming.  Without them the handler decodes greedily.
 Arithmetic parity: pinned to the transformers cousin, UNPINNED vs faster-qwen3-tts (absent) -- DESIGN.md."""
 from __future__ import annotations
 
 import logging
+import os
+import random
 from typing import Any, Optional
 
 import numpy as np
 
 from ..batcher import acquire_shared, assign_lane, release_shared
-from ..tts_model import B200Qwen3TTS, DeviceAudio
+from ..tts_model import _UNSUPPORTED_SAMPLING, SAMPLING_KEYWORDS, B200Qwen3TTS, DeviceAudio, resolve_sampling
 
 logger = logging.getLogger(__name__)
 
@@ -41,6 +49,23 @@ def _base_class() -> Any:
 
 
 _Base = _base_class()
+
+
+class HandlerModelView:
+    """One handler's view of the shared B200Qwen3TTS: every attribute is the model's, and generate_custom_voice_streaming
+    receives the handler's generation options and a fresh seed from the handler's generator (call keywords win)."""
+
+    def __init__(self, model: Any, options: dict, sampling_seed: Optional[int]):
+        self.wrapped = model
+        self.options = dict(options)
+        self._rng = random.Random(int(sampling_seed) if sampling_seed is not None else int.from_bytes(os.urandom(8), "little"))
+
+    def __getattr__(self, name: str) -> Any:
+        return getattr(self.wrapped, name)
+
+    def generate_custom_voice_streaming(self, *args: Any, **kwargs: Any):
+        kw = {**self.options, "sampling_seed": self._rng.getrandbits(64), **kwargs}
+        return self.wrapped.generate_custom_voice_streaming(*args, **kw)
 
 
 class B200Qwen3TTSHandler(_Base):  # type: ignore[misc, valid-type]
@@ -58,6 +83,11 @@ class B200Qwen3TTSHandler(_Base):  # type: ignore[misc, valid-type]
             lane = assign_lane(("qwen3tts", str(kwargs.get("model_name", "")), str(kwargs.get("device", "cuda"))), self._b200_lanes)
         self._b200_lane = int(lane) % self._b200_lanes
         self._b200_seed = int(gk.pop("seed", 0))
+        # sampling options: out of gen_kwargs (the reference's MLX path forwards gen_kwargs), checked now so a bad one fails at load
+        opts = {k: gk.pop(k) for k in list(gk) if k in SAMPLING_KEYWORDS or k in _UNSUPPORTED_SAMPLING}
+        resolve_sampling(None, **opts)
+        self._b200_sampling = {k: v for k, v in opts.items() if v is not None}
+        self._b200_sampling_seed = gk.pop("sampling_seed", None)
         kwargs["gen_kwargs"] = gk
         if "backend" in kwargs and kwargs["backend"] == "ggml":
             kwargs["backend"] = "torch"     # the ggml options of the reference slot do not apply; accept its default silently
@@ -89,6 +119,8 @@ class B200Qwen3TTSHandler(_Base):  # type: ignore[misc, valid-type]
                                                 backend=backend, max_sessions=n, codec_precision=prec, lane=lane, lanes=lanes)
 
         self.model = acquire_shared(key, build, lambda m: m.close())
+        if getattr(self, "_b200_sampling", None) or getattr(self, "_b200_sampling_seed", None) is not None:
+            self.model = HandlerModelView(self.model, self._b200_sampling, self._b200_sampling_seed)
         self._b200_shared_key = key
         self._b200_device = dev
         logger.info("Qwen3-TTS model loaded (libs2s_b200, %s, %d session slot%s)", dt, n, "" if n == 1 else "s")
@@ -96,6 +128,7 @@ class B200Qwen3TTSHandler(_Base):  # type: ignore[misc, valid-type]
     # ---- every GPU call of this handler's thread goes to its lane's stream ----------------------------------------------
     def _b200_lane_context(self):
         m = getattr(self, "model", None)
+        m = m.wrapped if isinstance(m, HandlerModelView) else m
         if isinstance(m, B200Qwen3TTS):
             return m.lane_context()
         import contextlib

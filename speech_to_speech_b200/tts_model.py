@@ -9,9 +9,11 @@ contract the reference's tests pin with fakes (T/test_qwen3_tts_handler_backend.
 
 The arithmetic (talker, code predictor, codec decoder: csrc/qwen3tts.cu, csrc/codec_decode.cu) follows the published
 cousin of Qwen3-TTS in transformers (Qwen3-Omni talker + Code2Wav) and is UNPINNED against faster-qwen3-tts, which is
-absent everywhere (DESIGN.md).  Deliberate differences, all stated there: greedy code selection (upstream samples),
-`language` / `instruct` are accepted and ignored (the cousin's prompt has no slot for them), voice cloning and voice
-design need the upstream speaker encoder and raise.  No CPU fallback.
+absent everywhere (DESIGN.md).  Deliberate differences, all stated there: code selection is greedy unless asked otherwise
+(upstream samples by default; `sampling=COUSIN_SAMPLING` or the per-call qwen-tts keywords `do_sample, temperature, top_k,
+top_p, repetition_penalty, subtalker_dosample, subtalker_temperature, subtalker_top_k, subtalker_top_p` switch the
+device sampler on), `language` / `instruct` are accepted and ignored (the cousin's prompt has no slot for them), voice
+cloning and voice design need the upstream speaker encoder and raise.  No CPU fallback.
 
 Concurrent sessions: one engine per (checkpoint, dtype, device) is shared by all handler instances of the process
 (`max_sessions` slots); the chunk requests of concurrently speaking sessions are merged by the SessionBatcher into ONE
@@ -22,6 +24,7 @@ import contextlib
 import json
 import logging
 import os
+import random
 import threading
 import types
 from time import perf_counter
@@ -60,6 +63,81 @@ CODEC_GEOMETRIES: dict[str, dict] = {
 }
 DEFAULT_SPEAKERS = {"aiden": 2301, "ethan": 2302, "chelsie": 2303}   # codec-vocabulary ids of the preset voices (random-init models)
 
+# The sampling of the published cousin (transformers Qwen3-Omni): talker.generate(do_sample=True, top_k=50, top_p=1.0,
+# temperature=0.9, repetition_penalty=1.05) and, for every frame, code_predictor.generate(do_sample=True, top_k=50,
+# top_p=0.8) at the predictor's default temperature 1.0 (modeling_qwen3_omni_moe.py:3905-3909, 3251-3259).
+COUSIN_SAMPLING = {
+    "talker": dict(do_sample=True, temperature=0.9, top_k=50, top_p=1.0, repetition_penalty=1.05),
+    "predictor": dict(do_sample=True, temperature=1.0, top_k=50, top_p=0.8),
+}
+# qwen-tts / faster-qwen3-tts generation keywords -> (model, Qwen3TTSEngine.set_sampling keyword)
+SAMPLING_KEYWORDS = {
+    "do_sample": ("talker", "do_sample"), "temperature": ("talker", "temperature"), "top_k": ("talker", "top_k"),
+    "top_p": ("talker", "top_p"), "repetition_penalty": ("talker", "repetition_penalty"),
+    "subtalker_dosample": ("predictor", "do_sample"), "subtalker_temperature": ("predictor", "temperature"),
+    "subtalker_top_k": ("predictor", "top_k"), "subtalker_top_p": ("predictor", "top_p"),
+}
+# generation options the device sampler does not implement, with the value at which they do nothing
+_UNSUPPORTED_SAMPLING = {"min_p": 0.0, "typical_p": 1.0, "epsilon_cutoff": 0.0, "eta_cutoff": 0.0, "num_beams": 1,
+                         "no_repeat_ngram_size": 0, "min_new_tokens": 0, "subtalker_min_p": 0.0, "subtalker_typical_p": 1.0,
+                         "subtalker_repetition_penalty": 1.0}
+_NEUTRAL = dict(do_sample=False, temperature=1.0, top_k=0, top_p=1.0, repetition_penalty=1.0)
+
+
+def resolve_sampling(base: Optional[Mapping] = None, **options: Any) -> dict:
+    """The token choice of an utterance: `base` ({"talker": dict | None, "predictor": dict | None}, None = greedy) overlaid
+    by the qwen-tts keywords in `options` (SAMPLING_KEYWORDS; None values are ignored).  A model's unset values come from
+    its base dict, else from the neutral ones (T 1, top_k 0 = off, top_p 1, penalty 1).  -> {"talker": ..., "predictor":
+    ...}, each the keywords of Qwen3TTSEngine.set_sampling or None when that model decodes greedily.  Raises ValueError for
+    keywords the device sampler does not implement and for out-of-range values."""
+    base = dict(base or {})
+    unknown = set(base) - {"talker", "predictor"}
+    if unknown:
+        raise ValueError(f"sampling presets have 'talker' and 'predictor' entries only, got {sorted(unknown)}")
+    over: dict = {"talker": {}, "predictor": {}}
+    for k, v in options.items():
+        if v is None:
+            continue
+        if k in _UNSUPPORTED_SAMPLING:
+            off = _UNSUPPORTED_SAMPLING[k]
+            if v != off and not (k == "num_beams" and int(v) <= 1):
+                raise ValueError(f"`{k}` (={v}) is not supported by the Qwen3-TTS device sampler: it implements do_sample, temperature, "
+                                 f"top_k, top_p, repetition_penalty (talker) and their subtalker_* counterparts (code predictor)")
+            continue
+        if k not in SAMPLING_KEYWORDS:
+            raise ValueError(f"unknown Qwen3-TTS generation option `{k}`")
+        model, key = SAMPLING_KEYWORDS[k]
+        over[model][key] = v
+    out: dict = {}
+    for model in ("talker", "predictor"):
+        b = base.get(model)
+        if b is not None and set(b) - set(_NEUTRAL):
+            raise ValueError(f"unknown {model} sampling options {sorted(set(b) - set(_NEUTRAL))}")
+        if b is None and not over[model]:
+            out[model] = None
+            continue
+        c = {**_NEUTRAL, **(b or {}), **over[model]}
+        c = dict(do_sample=bool(c["do_sample"]), temperature=float(c["temperature"]), top_k=int(c["top_k"]), top_p=float(c["top_p"]),
+                 repetition_penalty=float(c["repetition_penalty"]))
+        if c["do_sample"] and not c["temperature"] > 0.0:
+            raise ValueError(f"{model} `temperature` (={c['temperature']}) has to be a strictly positive float when sampling")
+        if c["do_sample"] and not 0.0 < c["top_p"] <= 1.0:
+            raise ValueError(f"{model} `top_p` has to be a float in (0, 1], but is {c['top_p']}")
+        if c["top_k"] < 0:
+            raise ValueError(f"{model} `top_k` has to be >= 0, but is {c['top_k']}")
+        if not c["repetition_penalty"] > 0.0:
+            raise ValueError(f"{model} `repetition_penalty` has to be a strictly positive float, but is {c['repetition_penalty']}")
+        if model == "predictor" and c["repetition_penalty"] != 1.0:
+            raise ValueError("the code predictor has no repetition penalty")
+        if not c["do_sample"]:
+            c.update(temperature=1.0, top_k=0, top_p=1.0)
+        out[model] = c if (c["do_sample"] or c["repetition_penalty"] != 1.0) else None
+    return out
+
+
+def is_greedy(sampling: Mapping) -> bool:
+    return sampling.get("talker") is None and sampling.get("predictor") is None
+
 
 class DeviceAudio:
     """A chunk of 24 kHz fp32 audio that is still on the GPU.  `np.asarray(chunk)` copies it to the host, so a consumer
@@ -97,7 +175,8 @@ def byte_tokenizer(text_vocab: int, reserved: int = 16) -> Callable[[str], list]
 class B200Qwen3TTS:
     def __init__(self, engine: Any, tokenize: Callable[[str], Sequence[int]], speakers: Mapping[str, int], max_sessions: int = 1,
                  batch_wait_s: float = 0.012, tts_model_type: str = "custom_voice", lane: int = 0, lanes: int = 1,
-                 batch_gap_s: Optional[float] = 0.003, prefetch_chunks: bool = True):
+                 batch_gap_s: Optional[float] = 0.003, prefetch_chunks: bool = True, sampling: Optional[Mapping] = None,
+                 sampling_seed: Optional[int] = None):
         # batch_gap_s: a session needs a few ms of host work between two chunk requests (resample + int16 + D2H of the chunk it
         # just received); the gap must cover it, or the sessions of the launch that just ended miss the next one and two groups
         # alternate in half-full launches (measured: mean batch 7.8 of 16 with a 0.6 ms gap)
@@ -105,6 +184,10 @@ class B200Qwen3TTS:
         self.lane, self.lanes = int(lane), int(lanes)
         self.prefetch_chunks = bool(prefetch_chunks)   # False: request chunk k + 1 only after the consumer took chunk k (A/B, tests)
         self.tokenize = tokenize
+        # default token choice of generate_custom_voice_streaming (None = greedy; COUSIN_SAMPLING = the cousin's) and one
+        # 64-bit Philox seed per sampled utterance, drawn from a generator seeded by sampling_seed (OS entropy when None)
+        self.sampling = resolve_sampling(sampling)
+        self._seed_rng = random.Random(int(sampling_seed) if sampling_seed is not None else int.from_bytes(os.urandom(8), "little"))
         self.speakers = {str(k).lower(): int(v) for k, v in speakers.items()}
         self.sample_rate = SAMPLE_RATE
         self._lock = threading.Lock()           # one thread at a time talks to the engine handle
@@ -144,7 +227,7 @@ class B200Qwen3TTS:
     @classmethod
     def from_pretrained(cls, model_name: str, device: Any = "cuda", dtype: Any = None, attn_implementation: str = "eager",
                         backend: str = "torch", max_sessions: int = 1, codec_precision: int = 1, lane: int = 0, lanes: int = 1,
-                        **_ignored: Any) -> "B200Qwen3TTS":
+                        sampling: Optional[Mapping] = None, sampling_seed: Optional[int] = None, **_ignored: Any) -> "B200Qwen3TTS":
         """Load a checkpoint DIRECTORY in the cousin's layout: `config.json` with {"talker": ..., "code2wav": ..., "speaker_id":
         ...}, `model.safetensors` with the talker state dict (+ "text_embedding.weight", "code2wav.*") and tokenizer files.
         Hub ids cannot be resolved offline, and the real Qwen3-TTS checkpoint layout is unverified (upstream absent): both
@@ -172,7 +255,7 @@ class B200Qwen3TTS:
                             {k[len("code2wav."):]: v for k, v in sd.items() if k.startswith("code2wav.")})
         tok = AutoTokenizer.from_pretrained(model_name)
         return cls(eng, lambda text: tok.encode(text, add_special_tokens=False), cfg.get("speaker_id") or DEFAULT_SPEAKERS,
-                   max_sessions=max_sessions, lane=lane, lanes=lanes)
+                   max_sessions=max_sessions, lane=lane, lanes=lanes, sampling=sampling, sampling_seed=sampling_seed)
 
     # ---- the calls the handler makes ------------------------------------------------------------------------------------
     def get_supported_speakers(self) -> list:
@@ -186,14 +269,17 @@ class B200Qwen3TTS:
 
     def generate_custom_voice_streaming(self, text: str, speaker: str, language: Optional[str] = None, instruct: Optional[str] = None,
                                         chunk_size: int = 8, max_new_tokens: int = 1536, non_streaming_mode: Optional[bool] = True,
-                                        **_unused: Any) -> Iterator[tuple]:
+                                        sampling_seed: Optional[int] = None, **generation: Any) -> Iterator[tuple]:
+        """generation: the qwen-tts sampling keywords (resolve_sampling), overlaid on the model's default `sampling`.
+        sampling_seed: the utterance's 64-bit Philox seed (default: the next one of the model's seed generator)."""
+        sampling = resolve_sampling(self.sampling, **generation)
         sid = self.speakers.get(str(speaker).lower())
         if sid is None:
             raise ValueError(f"unknown Qwen3-TTS speaker {speaker!r}; supported: {self.get_supported_speakers()}")
         if instruct:
             logger.debug("B200Qwen3TTS: `instruct` is accepted but has no slot in the built prompt layout; ignored")
         ids = list(self.tokenize(text or "Hello."))
-        yield from self._generate(ids, sid, chunk_size=chunk_size, max_new_tokens=max_new_tokens)
+        yield from self._generate(ids, sid, chunk_size=chunk_size, max_new_tokens=max_new_tokens, sampling=sampling, seed=sampling_seed)
 
     def generate_voice_clone_streaming(self, *a: Any, **k: Any) -> Iterator[tuple]:
         raise NotImplementedError("voice cloning needs the upstream speaker encoder (faster-qwen3-tts), which is absent; "
@@ -238,7 +324,8 @@ class B200Qwen3TTS:
                     out[i] = (valid, out[i][1], w)
         return out
 
-    def _generate(self, text_ids: Sequence[int], speaker_id: int, chunk_size: int, max_new_tokens: int) -> Iterator[tuple]:
+    def _generate(self, text_ids: Sequence[int], speaker_id: int, chunk_size: int, max_new_tokens: int,
+                  sampling: Optional[Mapping] = None, seed: Optional[int] = None) -> Iterator[tuple]:
         eng = self.engine
         chunk = max(1, int(chunk_size))
         budget = max(1, min(int(max_new_tokens), eng.cfg.max_positions - 16))
@@ -249,6 +336,10 @@ class B200Qwen3TTS:
         try:
             with self._lock:
                 eng.prefill(slot, ids, speaker_id)
+                if sampling is not None and not is_greedy(sampling):   # prefill left the slot greedy
+                    if seed is None:
+                        seed = self._seed_rng.getrandbits(64)
+                    eng.set_sampling(slot, talker=sampling["talker"], predictor=sampling["predictor"], seed=seed)
             done = 0
             if self.batcher is None:
                 while done < budget:
