@@ -190,7 +190,7 @@ int s2s_llama_prefill(s2s_llama* m, int32_t slot, const int32_t* ids_h, int32_t 
 int s2s_llama_prefill_batch(s2s_llama* m, const int32_t* slots_h, int32_t B, const int32_t* ids_h, const int32_t* n_h,
                             int32_t* next_ids_d, void* stream);
 
-/* Decode for B (<= s2s_llama_max_decode_batch: 16, 4 for Llama-3-8B) sessions in one persistent launch, each token chosen as
+/* Decode for B (<= s2s_llama_max_decode_batch: 16, also for Llama-3-8B) sessions in one persistent launch, each token chosen as
  * its slot's s2s_llama_set_sampling says (argmax by default).  slots_h[B]; first_ids_d[B] are the tokens to
  * feed first (the prefill's choice); ids_out_d [B, n_steps] receives the n_steps tokens generated AFTER them; eos stops
  * a row (eos_id < 0 disables); forced_d optional [B, n_steps] teacher-forced feedback; logits_out_d optional
@@ -200,7 +200,8 @@ int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int3
                      const int32_t* forced_d, float* logits_out_d, void* stream);
 /* Profiling aid (see s2s_whisper_set_trace): CTA 0's [phase begin, body end, barrier exit] stamps, trace_d[capacity][3]. */
 int s2s_llama_set_trace(s2s_llama* m, uint64_t* trace_d, int32_t capacity);
-/* Largest B accepted by s2s_llama_decode for this geometry (shared-memory budget of the decode kernel, <= 16). */
+/* Largest B accepted by s2s_llama_decode for this geometry (shared-memory budget of the decode kernel, <= 16); the
+ * environment variable S2S_LLAMA_MAX_DECODE_B lowers the value reported here (A/B measurements). */
 int32_t s2s_llama_max_decode_batch(s2s_llama* m);
 /* End-to-end with HOST buffers: (chunked) prefill + decode with the slot's token choice, synchronous.  ids_out_h[0] is
  * the token chosen from the prompt's last position, n_steps tokens in total (generate() semantics of the reference's pipeline call). */

@@ -61,16 +61,28 @@ struct s2s_ctx {
 // The attribute is per function, not per launch: host threads of different lanes launch the same kernel with different
 // sizes at the same time, and "set the size I need, then launch" races (a smaller size set by the other thread in between
 // makes the launch fail with cudaErrorLaunchOutOfResources).  The maximum is valid for every launch.
+// The largest dynamic shared-memory size a launch of `kern` can use on `device`: the per-block opt-in limit minus the
+// kernel's static shared memory (the budget the decode kernels' shared-memory plans are made against).
 template <typename K>
-inline cudaError_t s2s_opt_in_max_smem(K kern, int device, size_t need, const char** why) {
-  static thread_local const void* last_ok = nullptr;   // fast path: this thread already saw this kernel opted in
+inline cudaError_t s2s_max_dyn_smem(K kern, int device, long long* max_dyn, cudaFuncAttributes* attrs = nullptr) {
   cudaFuncAttributes fa;
   cudaError_t e = cudaFuncGetAttributes(&fa, (const void*)kern);
   if (e != cudaSuccess) return e;
   int optin = 0;
   e = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
   if (e != cudaSuccess) return e;
-  const long long max_dyn = (long long)optin - (long long)fa.sharedSizeBytes;
+  *max_dyn = (long long)optin - (long long)fa.sharedSizeBytes;
+  if (attrs) *attrs = fa;
+  return cudaSuccess;
+}
+
+template <typename K>
+inline cudaError_t s2s_opt_in_max_smem(K kern, int device, size_t need, const char** why) {
+  static thread_local const void* last_ok = nullptr;   // fast path: this thread already saw this kernel opted in
+  cudaFuncAttributes fa;
+  long long max_dyn = 0;
+  cudaError_t e = s2s_max_dyn_smem(kern, device, &max_dyn, &fa);
+  if (e != cudaSuccess) return e;
   if ((long long)need > max_dyn) { if (why) *why = "dynamic shared memory exceeds the device limit"; return cudaErrorInvalidValue; }
   if (last_ok == (const void*)kern && fa.maxDynamicSharedSizeBytes >= max_dyn) return cudaSuccess;
   e = cudaFuncSetAttribute((const void*)kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_dyn);

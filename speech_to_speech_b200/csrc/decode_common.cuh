@@ -129,11 +129,14 @@ struct DecSmem {
   unsigned int si_off, red_s_off, wb_off, redbuf_off, ring_off;
 };
 // rg: rows of the fp32 statistics copy that are resident at a time (stage_rows_norm walks the B rows in groups of rg; rg = B
-// = everything in one memory round trip, the default); kmax: widest activation operand that is staged WHOLE (a wider one is
-// staged in K-chunks of kmax columns, gemv_mma_chunked).
+// = everything in one memory round trip, the default; DEC_NORM_L2 = no copy at all, the rows are read from L2 into
+// registers); kmax: widest activation operand that is staged WHOLE (a wider one is staged in K-chunks of kmax columns,
+// gemv_mma_chunked).
+constexpr int DEC_NORM_L2 = -1;
 __host__ __device__ inline DecSmem dec_smem_layout(int B, int d, int kmax, int wb_floats, int rg = 0) {
   DecSmem L;
-  if (rg <= 0 || rg > B) rg = B;
+  if (rg == DEC_NORM_L2) rg = 0;
+  else if (rg <= 0 || rg > B) rg = B;
   const unsigned int xh_small = (((unsigned)B * (unsigned)(d + GV_XPAD) * 2u) + 15u) & ~15u;
   unsigned int xh_bytes = (unsigned)B * (unsigned)(kmax + GV_XPAD) * 2u;
   const unsigned int with_stats = xh_small + (unsigned)rg * (unsigned)d * 4u;
@@ -148,11 +151,16 @@ __host__ __device__ inline DecSmem dec_smem_layout(int B, int d, int kmax, int w
   L.ring_off = (L.redbuf_off + 2u * DEC_THREADS * 16u + 127u) & ~127u;
   return L;
 }
-// ring slots that fit next to the fixed part (at most 4 per warp)
-inline int dec_ring_slots(const DecSmem& L) {
-  const long long avail = 220LL * 1024 - (long long)L.ring_off - 256;  // static shared memory (parameter tables) takes ~5 KB
-  long long s = avail / ((long long)DEC_WARPS * (GV_SLOT_BYTES + 8));
-  return (int)(s > 4 ? 4 : s);
+// dynamic shared memory of a layout with `slots` weight-ring slots per warp (slots + their mbarriers + alignment slack)
+inline size_t dec_smem_bytes(const DecSmem& L, int slots) {
+  return (size_t)L.ring_off + (size_t)DEC_WARPS * slots * (GV_SLOT_BYTES + 8) + 128;
+}
+// ring slots that fit next to the fixed part (at most 4 per warp) in `max_dyn` bytes of dynamic shared memory: the device's
+// per-block opt-in limit minus the kernel's static shared memory (s2s_max_dyn_smem)
+inline int dec_ring_slots(const DecSmem& L, long long max_dyn) {
+  int s = 0;
+  while (s < 4 && (long long)dec_smem_bytes(L, s + 1) <= max_dyn) ++s;
+  return s;
 }
 
 // 16-byte asynchronous global -> shared copy through L2 (no registers held while in flight)
@@ -234,9 +242,72 @@ static __device__ __forceinline__ void norm_from_smem(const float* xs, int B, in
   __syncthreads();
 }
 
+// The same without the fp32 copy (rg = DEC_NORM_L2: the 16-bit operand of 16 Llama-3-8B sessions leaves no room for it):
+// every warp reads its half of a row from L2 straight into registers, NORM_L2_ROWS rows per pass, and normalises from the
+// registers -- one L2 pass.  The arithmetic is norm_from_smem's with 2 warps per row, i.e. that of a 4-row group: the rows
+// come out bit-identical to those of a launch that stages them in groups of 4 (Llama-3-8B at 8 sessions).
+constexpr int NORM_L2_WPR = 2, NORM_L2_ROWS = DEC_WARPS / NORM_L2_WPR, NORM_L2_MAX_D = 4096;
+template <typename T>
+static __device__ __noinline__ void stage_rows_norm_l2(const float* x, int B, int d, T* xh, int mode, const float* w,
+                                                       const float* bias, float eps, float* s_red, float* wb, int wb_ready) {
+  constexpr int PER = NORM_L2_MAX_D / (NORM_L2_WPR * 64);   // float2 per lane
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int sub = warp % NORM_L2_WPR, rsel = warp / NORM_L2_WPR, grp = rsel * NORM_L2_WPR;
+  const int xstride = d + GV_XPAD;
+  const float inv_d = 1.f / (float)d;
+  if (!wb_ready) stage_norm_weights(w, mode == 1 ? bias : nullptr, d, wb);
+  cp_async_wait_all();
+#pragma unroll 1
+  for (int r0 = 0, it = 0; r0 < B; r0 += NORM_L2_ROWS, ++it) {
+    const int row = r0 + rsel;
+    float2 v[PER];
+    float s1 = 0.f, s2 = 0.f;
+    if (row < B) {
+      const float* xr = x + (long long)row * d;
+#pragma unroll
+      for (int j = 0; j < PER; ++j) {
+        const int i = (sub * 32 + lane) * 2 + j * NORM_L2_WPR * 64;
+        if (i < d) v[j] = __ldcg(reinterpret_cast<const float2*>(xr + i));
+      }
+#pragma unroll
+      for (int j = 0; j < PER; ++j) {
+        if ((sub * 32 + lane) * 2 + j * NORM_L2_WPR * 64 < d) {
+          s1 += v[j].x + v[j].y;
+          s2 = fmaf(v[j].x, v[j].x, s2);
+          s2 = fmaf(v[j].y, v[j].y, s2);
+        }
+      }
+    }
+    s1 = warp_sum(s1);
+    s2 = warp_sum(s2);
+    if (lane == 0) { s_red[it * 2 * DEC_WARPS + warp] = s1; s_red[it * 2 * DEC_WARPS + DEC_WARPS + warp] = s2; }
+    __syncthreads();   // also orders the norm weights (cp.async above) before their readers
+    if (row < B) {
+      float t1 = 0.f, t2 = 0.f;
+      for (int k = 0; k < NORM_L2_WPR; ++k) { t1 += s_red[it * 2 * DEC_WARPS + grp + k]; t2 += s_red[it * 2 * DEC_WARPS + DEC_WARPS + grp + k]; }
+      const float mean = (mode == 1) ? t1 * inv_d : 0.f;
+      const float var = fmaxf(t2 * inv_d - mean * mean, 0.f);
+      const float rstd = rsqrtf(var + eps);
+      T* dst = xh + row * xstride;
+#pragma unroll
+      for (int j = 0; j < PER; ++j) {
+        const int i = (sub * 32 + lane) * 2 + j * NORM_L2_WPR * 64;
+        if (i < d) {
+          const float2 g = *reinterpret_cast<const float2*>(wb + i);
+          float y0 = (v[j].x - mean) * rstd * g.x, y1 = (v[j].y - mean) * rstd * g.y;
+          if (mode == 1) { const float2 bb = *reinterpret_cast<const float2*>(wb + d + i); y0 += bb.x; y1 += bb.y; }
+          *reinterpret_cast<uint32_t*>(dst + i) = DT<T>::pack2(y0, y1);
+        }
+      }
+    }
+  }
+  __syncthreads();
+}
+
 template <typename T>
 static __device__ __noinline__ void stage_rows_norm(const float* x, int B, int d, float* xs, T* xh, int mode, const float* w,
                                                     const float* bias, float eps, float* s_red, float* wb, int wb_ready, int rg = 0) {
+  if (rg == DEC_NORM_L2) { stage_rows_norm_l2<T>(x, B, d, xh, mode, w, bias, eps, s_red, wb, wb_ready); return; }
   if (rg <= 0 || rg > B) rg = B;
   const uint32_t xs_s = smem_u32(xs);
   // rows in groups of rg (all of them at once unless the fp32 copy of B rows does not fit next to the 16-bit operand)

@@ -284,7 +284,8 @@ GemmProblem lgemm(const void* a, int64_t lda, const void* w, int64_t ldw, int64_
 }  // namespace
 
 int llama_max_decode_batch_of(const s2s_llama* m) {
-  return std::min(MAX_DEC_B, llama_decode_max_batch(m->cfg.d_model, m->cfg.ffn, m->cfg.heads * m->cfg.head_dim, dec_grid(m->ctx)));
+  return std::min(MAX_DEC_B, llama_decode_max_batch(m->ctx->device, m->cfg.compute_dtype, m->cfg.d_model, m->cfg.ffn,
+                                                    m->cfg.heads * m->cfg.head_dim, dec_grid(m->ctx)));
 }
 
 void llama_fill_dec_params(s2s_llama* m, LlamaDecParams& p) {
@@ -737,7 +738,14 @@ int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int3
 
 int32_t s2s_llama_max_decode_batch(s2s_llama* m) {
   if (!m) return 0;
-  return llama_max_decode_batch_of(m);
+  int b = llama_max_decode_batch_of(m);
+  // developer knob: a smaller batch per launch than the shared-memory plan allows, so that one build can time both (e.g. 12:
+  // the Llama-3-8B limit before the third plan tier).  Only what the engine reports changes; the TTS slot is unaffected.
+  if (const char* e = getenv("S2S_LLAMA_MAX_DECODE_B")) {
+    const int v = atoi(e);
+    if (v >= 1 && v < b) b = v;
+  }
+  return b;
 }
 
 int s2s_llama_set_trace(s2s_llama* m, uint64_t* trace_d, int32_t capacity) {

@@ -18,7 +18,7 @@
 #include <algorithm>
 
 #include "llama_decode.cuh"
-#include "decode_common.cuh"
+#include "llama_decode_plan.cuh"
 
 namespace {
 
@@ -94,7 +94,8 @@ __device__ __noinline__ void ld_attn(const LlamaDecParams& p, int layer, int ste
   const int kvd = p.kv_heads * HD;
   constexpr int REC = HD + PART_PAD;
   const int n_blocks = (p.max_len + step + ATT_BLK - 1) / ATT_BLK, BH = p.B * H;  // longest session
-  const int plan = attn_plan(BH, n_blocks, p.s_max, (int)gridDim.x);
+  // the split plan of assoc_b sessions (LlamaDecPlan): it fixes the softmax-merge association of every item
+  const int plan = attn_plan(p.assoc_b * H, n_blocks, p.s_max, (int)gridDim.x);
   const int S = plan & 0x7f, bps = (n_blocks + S - 1) / S;
   const bool wl = plan & ATTN_WARP_LEVEL;
   const T* kv = reinterpret_cast<const T*>(p.kv);
@@ -247,8 +248,6 @@ template <typename T>
 struct LdSmem {
   T* xh; float* xs; float* sv; int* si; float* s_red; float* wb; float4* red;
 };
-
-__host__ __device__ inline int ld_kmax(int d, int ffn, int qd) { return (d > ffn ? d : ffn) > qd ? (d > ffn ? d : ffn) : qd; }
 
 template <typename T>
 __device__ __forceinline__ void ld_phase(const LlamaDecParams& p, int step, int ph, const LdSmem<T>& sm, GemvRing& ring,
@@ -412,20 +411,24 @@ __global__ void llama_decode_init_kernel(const LlamaDecParams p) {
 
 template <typename T>
 int launch_t(s2s_ctx* ctx, const LlamaDecParams& p, int debug_phases, cudaStream_t stream) {
-  int kmax = 0, rg = 0, kc = 0, slots = 0;
   int grid = dec_grid(ctx);                          // the context's SM partition (s2s_set_sm_partition)
   if (const char* e = getenv("S2S_DECODE_CTAS")) {   // developer knob: override for experiments (tests/dev/dev_lanes.py)
     const int v = atoi(e);
     if (v >= 8 && v < ctx->num_sms) grid = v;
   }
-  S2S_REQUIRE(llama_decode_plan(p.B, p.d, p.ffn, p.heads * p.hd, grid, &kmax, &rg, &kc, &slots),
+  auto kern = llama_decode_kernel<T>;
+  long long max_dyn = 0;
+  S2S_CHECK_CUDA(s2s_max_dyn_smem(kern, ctx->device, &max_dyn));
+  LlamaDecPlan pl;
+  S2S_REQUIRE(llama_decode_plan(p.B, p.d, p.ffn, p.heads * p.hd, grid, max_dyn, &pl),
               "llama decode: batch %d does not fit shared memory for d %d, ffn %d", p.B, p.d, p.ffn);
-  const DecSmem lay = dec_smem_layout(p.B, p.d, kmax, p.d, rg);
+  const DecSmem lay = dec_smem_layout(p.B, p.d, pl.kmax, p.d, pl.rg);
   LlamaDecParams pr = p;
   pr.sync_relaxed = dec_sync_relaxed_env();
-  pr.ring_slots = slots; pr.norm_rg = rg; pr.down_kc = kc;
-  const size_t smem = (size_t)lay.ring_off + (size_t)DEC_WARPS * pr.ring_slots * (GV_SLOT_BYTES + 8) + 128;
-  auto kern = llama_decode_kernel<T>;
+  pr.ring_slots = pl.slots; pr.norm_rg = pl.rg; pr.down_kc = pl.kc; pr.assoc_b = pl.assoc_b;
+  const size_t smem = dec_smem_bytes(lay, pl.slots);
+  S2S_REQUIRE((long long)smem <= max_dyn, "llama decode: plan of batch %d needs %zu B of shared memory, %lld available", p.B, smem,
+              max_dyn);
   S2S_CHECK_CUDA(s2s_opt_in_max_smem(kern, ctx->device, smem, nullptr));
   llama_decode_init_kernel<T><<<p.B, 256, 0, stream>>>(pr);
   S2S_LAUNCH_CHECK();
@@ -461,30 +464,10 @@ int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int de
   return S2S_ERR_UNSUPPORTED;
 }
 
-// Shared-memory plan of a batch.  Preferred: everything staged whole in one round trip (rg = B, kc = 0).  When that does not
-// leave two ring slots per warp: stage the ffn-wide down-projection operand in K-chunks of max(d, qd) columns and walk the
-// fp32 statistics copy in row groups (largest power of two that fits) -- Llama-3-8B: 4 sessions whole, 8 with chunks.
-bool llama_decode_plan(int B, int d, int ffn, int qd, int grid, int* kmax, int* rg, int* kc, int* ring_slots) {
-  {
-    const int km = ld_kmax(d, ffn, qd);
-    const int s = dec_ring_slots(dec_smem_layout(B, d, km, d, B));
-    if (s >= 2) { *kmax = km; *rg = B; *kc = 0; *ring_slots = s; return true; }
-  }
-  const int lim = ((std::max(d, qd) + 255) / 256) * 256;     // chunk = the widest operand that is staged whole anyway
-  if (ffn <= lim || !gemv_chunk_ok(d, ffn, lim, grid)) return false;
-  const int km = ld_kmax(d, lim, qd);
-  for (int g = B; g >= 2; g >>= 1) {
-    int gg = 1;
-    while (gg * 2 <= g) gg *= 2;
-    const int s = dec_ring_slots(dec_smem_layout(B, d, km, d, gg));
-    if (s >= 2) { *kmax = km; *rg = gg; *kc = lim; *ring_slots = s; return true; }
-  }
-  return false;
-}
-
-int llama_decode_max_batch(int d, int ffn, int qd, int grid) {
-  int kmax, rg, kc, slots;
-  for (int B = DEC_MAX_B; B >= 1; --B)
-    if (llama_decode_plan(B, d, ffn, qd, grid, &kmax, &rg, &kc, &slots)) return B;
-  return 0;
+int llama_decode_max_batch(int device, int dtype, int d, int ffn, int qd, int grid) {
+  long long max_dyn = 0;
+  const cudaError_t e = dtype == S2S_F16 ? s2s_max_dyn_smem(llama_decode_kernel<__half>, device, &max_dyn)
+                                         : s2s_max_dyn_smem(llama_decode_kernel<__nv_bfloat16>, device, &max_dyn);
+  if (e != cudaSuccess) return 0;
+  return llama_decode_plan_max_batch(d, ffn, qd, grid, max_dyn);
 }

@@ -57,8 +57,10 @@ struct LlamaDecParams {
   long long embed_stride, head_stride;
   const void* embed0;           // [vocab0, d] 16-bit
   int ring_slots;               // weight-ring slots per warp (set by the launcher)
-  int norm_rg;                  // rows of the fp32 statistics copy resident at a time (set by the launcher; B = all at once)
+  int norm_rg;                  // rows of the fp32 statistics copy resident at a time (set by the launcher; B = all at once;
+                                // DEC_NORM_L2 = no copy, rows read from L2 into registers)
   int down_kc;                  // > 0: the down-projection operand is staged in K-chunks of this many columns (large batches)
+  int assoc_b;                  // the batch whose plan fixes the attention split plan (set by the launcher, see LlamaDecPlan)
   unsigned long long* trace;    // optional [cap][3] globaltimer stamps of CTA 0 (phase begin, body end, barrier exit)
   int trace_cap;
   int sync_relaxed;             // 1: barrier waits without the acquire fence (A/B measurement aid)
@@ -71,8 +73,5 @@ struct LlamaDecParams {
 };
 
 int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int debug_phases, cudaStream_t stream);
-// largest batch per launch on `grid` CTAs that keeps >= 2 weight-ring slots per warp in shared memory
-int llama_decode_max_batch(int d, int ffn, int qd, int grid);
-// shared-memory plan of a batch: kmax = widest operand staged whole, rg = statistics rows per group, kc = down-projection chunk
-// (0 = unchunked); returns false when the batch does not fit
-bool llama_decode_plan(int B, int d, int ffn, int qd, int grid, int* kmax, int* rg, int* kc, int* ring_slots);
+// largest batch per launch on `grid` CTAs that has a shared-memory plan (llama_decode_plan.cuh) on `device`
+int llama_decode_max_batch(int device, int dtype, int d, int ffn, int qd, int grid);

@@ -23,6 +23,10 @@
 #include "whisper_decode.cuh"
 #include "decode_common.cuh"
 
+// Dynamic shared memory the 8-phase kernel's plans are made against: a fixed 220 KB (below the device limit), so that the
+// batch per launch -- and with it the attention split plans and the ids -- does not depend on the kernel's static size.
+constexpr long long WD_SMEM_BUDGET = 220LL * 1024 - 128;
+
 namespace {
 
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
@@ -798,7 +802,7 @@ int launch_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, cudaStre
   const DecSmem lay = dec_smem_layout(p.B, p.d, std::max(p.d, p.ffn), 2 * p.d);
   WhisperDecParams pr = p;
   pr.sync_relaxed = dec_sync_relaxed_env();
-  pr.ring_slots = dec_ring_slots(lay);
+  pr.ring_slots = dec_ring_slots(lay, WD_SMEM_BUDGET);
   {
     const int BH = p.B * p.heads, grid = dec_grid(ctx);
     pr.cross_plan = attn_plan(BH, (p.n_ctx + ATT_BLK - 1) / ATT_BLK, p.s_max, grid);
@@ -807,7 +811,7 @@ int launch_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, cudaStre
     for (int nb = 1; nb <= nb_max; ++nb) pr.self_plan[nb] = (unsigned char)attn_plan(BH, nb, p.s_max, grid);
   }
   S2S_REQUIRE(pr.ring_slots >= 2, "whisper decode: batch %d leaves no shared memory for the weight ring", p.B);
-  const size_t smem = (size_t)lay.ring_off + (size_t)DEC_WARPS * pr.ring_slots * (GV_SLOT_BYTES + 8) + 128;
+  const size_t smem = dec_smem_bytes(lay, pr.ring_slots);
   auto kern = whisper_decode_kernel<T>;
   S2S_CHECK_CUDA(s2s_opt_in_max_smem(kern, ctx->device, smem, nullptr));
   whisper_decode_init_kernel<T><<<p.B, 256, 0, stream>>>(pr);
@@ -850,6 +854,6 @@ int whisper_decode_launch(s2s_ctx* ctx, const WhisperDecParams& p, int dtype, in
 
 int whisper_decode_max_batch(int d, int ffn) {
   for (int B = DEC_MAX_B; B >= 1; --B)
-    if (dec_ring_slots(dec_smem_layout(B, d, std::max(d, ffn), 2 * d)) >= 2) return B;
+    if (dec_ring_slots(dec_smem_layout(B, d, std::max(d, ffn), 2 * d), WD_SMEM_BUDGET) >= 2) return B;
   return 1;
 }
