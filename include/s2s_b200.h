@@ -198,7 +198,7 @@ int s2s_llama_prefill_batch(s2s_llama* m, const int32_t* slots_h, int32_t B, con
 int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int32_t* first_ids_d,
                      int32_t n_steps, int32_t eos_id, int32_t* ids_out_d, int32_t* len_out_d,
                      const int32_t* forced_d, float* logits_out_d, void* stream);
-/* Profiling aid (see s2s_whisper_set_trace): CTA 0's [phase begin, body end, barrier exit] stamps, trace_d[capacity][3]. */
+/* Profiling aid: the stamps of s2s_whisper_set_trace, trace_d[2][capacity][6] (stamp 1, inputs staged, stays 0). */
 int s2s_llama_set_trace(s2s_llama* m, uint64_t* trace_d, int32_t capacity);
 /* Largest B accepted by s2s_llama_decode for this geometry (shared-memory budget of the decode kernel, <= 16); the
  * environment variable S2S_LLAMA_MAX_DECODE_B lowers the value reported here (A/B measurements). */
@@ -314,7 +314,8 @@ int s2s_qwen3tts_decode_audio_batch(s2s_qwen3tts* m, const int32_t* slots_h, int
 int s2s_qwen3tts_set_frames(s2s_qwen3tts* m, int32_t slot, int32_t n_frames);
 int32_t s2s_qwen3tts_frames(s2s_qwen3tts* m, int32_t slot);
 int32_t s2s_qwen3tts_max_batch(s2s_qwen3tts* m);
-/* Profiling aid (see s2s_llama_set_trace): phase stamps of the talker (which = 0) or code-predictor (1) launches. */
+/* Profiling aid (see s2s_llama_set_trace): phase stamps of the talker (which = 0) or code-predictor (1) launches,
+ * trace_d[2][capacity][6]. */
 int s2s_qwen3tts_set_trace(s2s_qwen3tts* m, int32_t which, uint64_t* trace_d, int32_t capacity);
 s2s_codec* s2s_qwen3tts_codec(s2s_qwen3tts* m);
 

@@ -133,6 +133,15 @@ struct DecSmem {
 // registers); kmax: widest activation operand that is staged WHOLE (a wider one is staged in K-chunks of kmax columns,
 // gemv_mma_chunked).
 constexpr int DEC_NORM_L2 = -1;
+// the part after the activation operand, from aux_off on (shared with the cluster kernel's layout, whisper_decode.cu)
+__host__ __device__ inline void dec_smem_tail(DecSmem& L, unsigned int aux_off, int wb_floats) {
+  L.aux_off = aux_off;
+  L.si_off = L.aux_off + DEC_WARPS * DEC_MAX_B * 4;
+  L.red_s_off = L.si_off + DEC_WARPS * DEC_MAX_B * 4;
+  L.wb_off = L.red_s_off + 2 * DEC_WARPS * DEC_MAX_B * 4;   // s_red: [row iterations <= 16][2][DEC_WARPS]
+  L.redbuf_off = (L.wb_off + (unsigned)wb_floats * 4u + 15u) & ~15u;
+  L.ring_off = (L.redbuf_off + 2u * DEC_THREADS * 16u + 127u) & ~127u;
+}
 __host__ __device__ inline DecSmem dec_smem_layout(int B, int d, int kmax, int wb_floats, int rg = 0) {
   DecSmem L;
   if (rg == DEC_NORM_L2) rg = 0;
@@ -143,12 +152,7 @@ __host__ __device__ inline DecSmem dec_smem_layout(int B, int d, int kmax, int w
   if (with_stats > xh_bytes) xh_bytes = with_stats;
   xh_bytes = (xh_bytes + 127u) & ~127u;
   L.xs_off = xh_small;
-  L.aux_off = xh_bytes;
-  L.si_off = L.aux_off + DEC_WARPS * DEC_MAX_B * 4;
-  L.red_s_off = L.si_off + DEC_WARPS * DEC_MAX_B * 4;
-  L.wb_off = L.red_s_off + 2 * DEC_WARPS * DEC_MAX_B * 4;   // s_red: [row iterations <= 16][2][DEC_WARPS]
-  L.redbuf_off = (L.wb_off + (unsigned)wb_floats * 4u + 15u) & ~15u;
-  L.ring_off = (L.redbuf_off + 2u * DEC_THREADS * 16u + 127u) & ~127u;
+  dec_smem_tail(L, xh_bytes, wb_floats);
   return L;
 }
 // dynamic shared memory of a layout with `slots` weight-ring slots per warp (slots + their mbarriers + alignment slack)
@@ -421,6 +425,14 @@ struct GemvArgs {
   // here kc columns at a time from xsrc (row stride xsrc_ld), so a K wider than shared memory allows serves large batches
   const void* xsrc; int xsrc_ld; int kc;
 };
+// every field to its neutral value: a plain [N, K = d] projection into out (ldo = d), planned on the fly
+__device__ __forceinline__ void gemv_args_reset(GemvArgs& a, int d, float* out) {
+  a.W = nullptr; a.N = 0; a.K = d; a.bias = nullptr; a.mode = EPI_STORE; a.out = out; a.ldo = d; a.out_h = nullptr; a.ldh = 0;
+  a.kv0 = nullptr; a.kv_which = 0; a.kv_batch = 0; a.d = d;
+  a.suppress = nullptr; a.first_step = 0; a.logits_out = nullptr; a.logits_ld = 0;
+  a.pos = nullptr; a.slot = nullptr; a.kv_slot = 0; a.kv_ld = 0; a.rope = nullptr; a.hd = 0; a.q_rows = 0; a.k_rows = 0;
+  a.q_scale = 1.f; a.kraw = nullptr; a.plan_id = -1; a.xsrc = nullptr; a.xsrc_ld = 0; a.kc = 0;
+}
 
 // epilogue of the row pair (row0, row0 + 1), row0 even, for session b.  v already carries the bias.
 // LLAMA selects which modes exist in the instantiation (smaller code per model family).  Kept inline: with ~220 KB of
@@ -516,6 +528,36 @@ struct GemvRing {
   GemvPlan plan;
   const GemvPlan* plans_s;  // shared memory: plans of the kernel's projection shapes, computed once at kernel start
 };
+
+// Shared-memory views of one CTA (see dec_smem_layout)
+template <typename T>
+struct DecViews {
+  T* xh; float* xs; float* sv; int* si; float* s_red; float* wb; float4* red;
+};
+template <typename T>
+__device__ __forceinline__ DecViews<T> dec_views(unsigned char* smem, const DecSmem& L) {
+  return {reinterpret_cast<T*>(smem), reinterpret_cast<float*>(smem + L.xs_off), reinterpret_cast<float*>(smem + L.aux_off),
+          reinterpret_cast<int*>(smem + L.si_off), reinterpret_cast<float*>(smem + L.red_s_off),
+          reinterpret_cast<float*>(smem + L.wb_off), reinterpret_cast<float4*>(smem + L.redbuf_off)};
+}
+// Lane 0 of every warp sets up the warp's ring: `slots` slots at rb + warp * slots * GV_SLOT_BYTES, the mbarriers after
+// all warps' slots.  Ends with a __syncthreads().
+__device__ __forceinline__ void gemv_ring_init(GemvRing& ring, unsigned char* rb, int slots, const GemvPlan* plans_s) {
+  const int warp = threadIdx.x >> 5;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(rb + (size_t)DEC_WARPS * slots * GV_SLOT_BYTES) + warp * slots;
+  if ((threadIdx.x & 31) == 0) {   // lane 0 owns the warp's ring state in shared memory
+    ring.slots = slots;
+    ring.base_s = smem_u32(rb + (size_t)warp * slots * GV_SLOT_BYTES);
+    ring.bars_s = smem_u32(bars);
+    ring.slot = 0;
+    ring.parity = 0;
+    ring.plans_s = plans_s;
+    ring.pre_valid = 0; ring.pre_pj = 0; ring.pre_pu = 0; ring.pre_nvalid = 0; ring.pre_W = nullptr;
+    for (int i = 0; i < slots; ++i) mbar_init(bars + i, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+}
 
 __device__ __forceinline__ void bulk_g2s(uint32_t smem_dst, const void* gsrc, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
@@ -923,6 +965,38 @@ __device__ __forceinline__ void gemv_argmax_candidates(float (&best_v)[2], int (
   }
 }
 
+// ---- token choice of the select phase (one warp per session) ----------------------------------------------------
+// the argmax over the grid's per-CTA candidates of session b (the lowest id on ties), in every lane
+__device__ __forceinline__ int dec_argmax_merge(const float* cand_val, const int* cand_idx, int b) {
+  const int lane = threadIdx.x & 31;
+  float bv = -INFINITY; int bi = 0x7fffffff;
+#pragma unroll 1
+  for (int c = lane; c < (int)gridDim.x; c += 32) {
+    const float v = __ldcg(cand_val + b * gridDim.x + c); const int i = __ldcg(cand_idx + b * gridDim.x + c);
+    if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, bv, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
+  }
+  return bi;
+}
+// One thread: output id i of n of session b (eos once the session is done), the EOS / length bookkeeping, and the id fed
+// to the next step (the forced one under teacher forcing).  was_done = done[b] and forced_tok = forced[b][i] are loaded
+// by the caller before the candidate loads, so that their round trips overlap.
+template <typename P>
+__device__ __forceinline__ int dec_record_token(const P& p, int b, int i, int n, int tok, int was_done, int forced_tok) {
+  if (was_done) tok = p.eos;
+  p.out_ids[b * n + i] = tok;
+  if (!was_done && !p.forced) {
+    if (tok == p.eos) { p.done[b] = 1; p.out_len[b] = i + 1; atomicAdd(p.n_done, 1); }
+    else if (i == n - 1) { p.out_len[b] = n; }
+  }
+  if (p.forced && i == n - 1) p.out_len[b] = n;
+  return p.forced ? forced_tok : tok;
+}
+
 // ---- attention: CTA-level items ------------------------------------------------------------------------------
 // One item = (session, head, key split).  The 8 warps of the CTA stride over the item's 32-key blocks; each warp keeps
 // a running (m, l, o) over its blocks (one memory round trip per block: the 8 K and 8 V vectors of a block are
@@ -1145,4 +1219,146 @@ __device__ __forceinline__ void attn_finish_item(const float* rec_s, int n_rec /
   // last split of this (session, head): merge the records
   attn_merge_records<T, HD>(part_bh, splits, out16);
   if (lane == 0) *cnt = 0u;
+}
+
+// One item (session, head, split s of S over the key blocks [blk0, blk1)) of an attention phase planned by attn_plan:
+// warp-level, this warp alone; CTA-level, the 8 warps stride over the blocks and warp 0 finishes.  rec_s: DEC_WARPS records
+// of shared memory; part_bh, cnt, out16: the (session, head)'s records, split counter and 16-bit output.
+template <typename T, int HD>
+__device__ __forceinline__ void attn_run_item(bool warp_level, const float* q, const T* K, const T* V, long long ld, int n_keys,
+                                              int blk0, int blk1, float* rec_s, float* part_bh, int s, int S, unsigned int* cnt,
+                                              T* out16) {
+  constexpr int REC = HD + PART_PAD;
+  const int warp = threadIdx.x >> 5;
+  if (warp_level) {
+    attend_blocks<T, HD>(q, K, V, ld, ld, n_keys, blk0, blk1, 1, rec_s + warp * REC);
+    attn_finish_item<T, HD>(rec_s + warp * REC, 1, part_bh, s, S, cnt, out16);
+    __syncwarp();
+  } else {
+    attend_blocks<T, HD>(q, K, V, ld, ld, n_keys, blk0 + warp, blk1, DEC_WARPS, rec_s + warp * REC);
+    __syncthreads();
+    if (warp == 0) attn_finish_item<T, HD>(rec_s, DEC_WARPS, part_bh, s, S, cnt, out16);
+    __syncthreads();
+  }
+}
+
+// ---- the token-step loop of the persistent decode kernels --------------------------------------------------------
+__device__ __forceinline__ unsigned long long dec_clock_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
+
+struct DecNorm { const float *w, *b; };   // norm weights (and LayerNorm bias) of a phase's input; w == null: none
+
+// Runs phases [ph_begin, ph_end) of steps [step_begin, step_end) (coop: every phase of every step, with a grid barrier after
+// each).  The kernel's Model supplies, as __forceinline__ members:
+//   n_phases                      phases per token step
+//   skip(step, ph)                nothing to do: no work, no barrier, no trace record
+//   has_gemv(step, ph)            the phase starts with a projection; gemv_args(step, ph, a) builds its arguments
+//   lookahead_target(step, ph)    the phase the look-ahead prepares; norm_of(ph): the norm weights it stages
+//   prefetch_l2(step, ph)         L2 warm-up for the next phase (may be empty)
+//   phase(step, ph, sm, ring, ready, scratch, wb_ready, tr)  the phase body; ready: its prepared arguments or null
+//   stamps_barrier                the loop records trace stamps 2 and 3 (else the phase body may use them)
+// Between a phase's grid_arrive and grid_wait the CTA prepares the next target phase up to 3 phases ahead, when the ring
+// holds nothing yet: its arguments and first weight units (not for a K-chunked projection, which starts its own stream) and
+// its norm weights (once per target phase).  Argument structs and ring state live in shared memory, written by one thread.
+// s_args[0] holds the prepared arguments, s_args + 1 is the phase's scratch.
+// Trace (p.trace != null): CTA 0 and the last CTA record, per phase that runs, trace[2][trace_cap][6] globaltimer stamps:
+// phase begin, inputs staged (0 where the phase does not record it), arrived, next phase prepared, body end, barrier exit.
+template <typename T, typename P, typename Model>
+__device__ __forceinline__ void dec_run(const P& p, const Model& m, const DecViews<T>& sm, GemvRing& ring, GemvArgs* s_args,
+                                        int step_begin, int step_end, int ph_begin, int ph_end, int coop) {
+  const int n_ph = m.n_phases;
+  unsigned int epoch = 0;
+  int trace_i = 0;
+  GemvArgs& pre_args = s_args[0];
+  if (threadIdx.x == 0) pre_args.K = p.d;   // gemv_drain reads it
+  int pre_tag = -1, wb_tag = -1;  // (step, phase) the prepared arguments / staged norm weights belong to
+  for (int step = step_begin; step < step_end; ++step) {
+    const int pb = coop ? 0 : ph_begin, pe = coop ? n_ph : ph_end;
+    for (int ph = pb; ph < pe; ++ph) {
+      const bool skip = m.skip(step, ph);
+      const bool tracing = p.trace && trace_i < p.trace_cap && threadIdx.x == 0 &&
+                           (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1);
+      unsigned long long* tr = tracing ? p.trace + ((blockIdx.x == 0 ? 0 : 1) * (long long)p.trace_cap + trace_i) * 6 : nullptr;
+      if (tracing) tr[0] = dec_clock_ns();
+      const int tag = step * n_ph + ph;
+      if (!skip) m.phase(step, ph, sm, ring, pre_tag == tag ? &pre_args : nullptr, s_args + 1, wb_tag == tag, tr);
+      if (tracing) tr[4] = dec_clock_ns();
+      if (coop && !skip) {
+        grid_arrive(p.sync_counter, epoch);
+        if (tracing && Model::stamps_barrier) tr[2] = dec_clock_ns();  // arrived (results published)
+        // ---- between arrive and wait: everything for the next phases that does not depend on other CTAs ----
+        int nph = ph + 1, nstep = step;
+        if (nph == n_ph) { nph = 0; nstep = step + 1; }
+        if (nstep < step_end) m.prefetch_l2(nstep, nph);
+        if (!ring.pre_valid) {
+#pragma unroll 1
+          for (int look = 0; look < 3 && nstep < step_end; ++look) {
+            if (m.lookahead_target(nstep, nph)) {
+              const int ntag = nstep * n_ph + nph;
+              if (m.has_gemv(nstep, nph)) {
+                if (threadIdx.x == 0) m.gemv_args(nstep, nph, pre_args);  // one thread writes the shared struct
+                __syncthreads();
+                if (pre_args.kc == 0) gemv_prefetch<T>(pre_args, ring);   // plan + first weight units -> shared memory
+                pre_tag = ntag;
+              }
+              const DecNorm nw = m.norm_of(nph);   // wb is idle until that phase stages its input
+              if (nw.w && wb_tag != ntag) { stage_norm_weights(nw.w, nw.b, p.d, sm.wb); wb_tag = ntag; }
+              break;
+            }
+            if (++nph == n_ph) { nph = 0; ++nstep; }
+          }
+        }
+        if (tracing && Model::stamps_barrier) tr[3] = dec_clock_ns();  // next phase prepared
+        grid_wait(p.sync_counter, epoch, p.sync_relaxed);
+      }
+      if (tracing) tr[5] = dec_clock_ns();
+      if (!skip) ++trace_i;
+    }
+    if (coop && !p.forced && *reinterpret_cast<volatile int*>(p.n_done) >= p.B) break;
+  }
+  gemv_drain(pre_args.K, ring);  // early exit: never leave a bulk copy in flight
+}
+
+// init kernels, one CTA per session b: its bookkeeping (done, out_len, attention split counters; CTA 0 also the finished
+// count and the grid barrier) and its n output ids (eos)
+template <typename P>
+__device__ __forceinline__ void dec_init_session(const P& p, int b, int n) {
+  if (threadIdx.x == 0) {
+    p.done[b] = 0;
+    p.out_len[b] = 0;
+    if (b == 0) { *p.n_done = 0; *p.sync_counter = 0; }
+    for (int h = 0; h < p.heads; ++h) p.attn_cnt[b * p.heads + h] = 0u;
+  }
+  for (int i = threadIdx.x; i < n; i += blockDim.x) p.out_ids[b * n + i] = p.eos;
+}
+
+// Host: one cooperative launch of a persistent decode kernel over n_steps steps of n_ph phases, or (debug_phases) one
+// ordinary launch per (step, phase), where kernel boundaries replace the grid barrier.  cluster > 0: clusters of that size.
+template <typename P>
+inline int dec_launch(void (*kern)(P, int, int, int, int, int), const P& p, int grid, int cluster, size_t smem, int n_steps,
+                      int n_ph, int debug_phases, cudaStream_t stream) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(grid); cfg.blockDim = dim3(DEC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
+  cudaLaunchAttribute at[2];
+  int n_at = 0;
+  if (cluster > 0) {
+    at[n_at].id = cudaLaunchAttributeClusterDimension;
+    at[n_at].val.clusterDim.x = cluster; at[n_at].val.clusterDim.y = 1; at[n_at].val.clusterDim.z = 1;
+    ++n_at;
+  }
+  cfg.attrs = at;
+  if (!debug_phases) {
+    at[n_at].id = cudaLaunchAttributeCooperative; at[n_at].val.cooperative = 1;
+    cfg.numAttrs = n_at + 1;
+    S2S_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, p, 0, n_steps, 0, n_ph, 1));
+    s2s_count_launch();
+    return S2S_OK;
+  }
+  cfg.numAttrs = n_at;
+  for (int s = 0; s < n_steps; ++s)
+    for (int ph = 0; ph < n_ph; ++ph) S2S_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, p, s, s + 1, ph, ph + 1, 0));
+  return S2S_OK;
 }

@@ -22,12 +22,6 @@
 
 namespace {
 
-__device__ __forceinline__ unsigned long long gtimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-
 // Qwen3: RMSNorm over head_dim of a raw q / k row (fp32 statistics, Qwen3RMSNorm), then RoPE.  One warp; rows are stored
 // pair-adjacent (2j, 2j+1) = rotate_half partners (j, j + hd/2), and so are the norm weights.  y: this lane's PER elements.
 template <int HD>
@@ -114,16 +108,7 @@ __device__ __noinline__ void ld_attn(const LlamaDecParams& p, int layer, int ste
       if (wl || warp == 0) ld_qk_prepare<T, HD>(p, layer, b, h, pos, blk1 == nb);
       if (wl) __syncwarp(); else __syncthreads();
     }
-    if (wl) {
-      attend_blocks<T, HD>(q, Kb, Kb + p.kv_which_stride, kvd, kvd, len, blk0, blk1, 1, rec_s + warp * REC);
-      attn_finish_item<T, HD>(rec_s + warp * REC, 1, part_bh, s, S, p.attn_cnt + bh, out16);
-      __syncwarp();
-    } else {
-      attend_blocks<T, HD>(q, Kb, Kb + p.kv_which_stride, kvd, kvd, len, blk0 + warp, blk1, DEC_WARPS, rec_s + warp * REC);
-      __syncthreads();
-      if (warp == 0) attn_finish_item<T, HD>(rec_s, DEC_WARPS, part_bh, s, S, p.attn_cnt + bh, out16);
-      __syncthreads();
-    }
+    attn_run_item<T, HD>(wl, q, Kb, Kb + p.kv_which_stride, kvd, len, blk0, blk1, rec_s, part_bh, s, S, p.attn_cnt + bh, out16);
   }
 }
 
@@ -160,38 +145,17 @@ __device__ __noinline__ void ld_select(const LlamaDecParams& p, int step, float*
       stok = sample_row(row, p.vocab, *sc, p.seen + (long long)p.slot[b] * p.seen_words, p.pos[b] + 1, s_samp);
     }
     if (warp == 0) {
-      float bv = -INFINITY; int bi = 0x7fffffff;
-      if (sampled) {
-        bi = stok;
-      } else if (ld_has_head(p, step)) {
-#pragma unroll 1
-        for (int c = lane; c < (int)gridDim.x; c += 32) {
-          const float v = __ldcg(p.cand_val + b * gridDim.x + c); const int i = __ldcg(p.cand_idx + b * gridDim.x + c);
-          if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float ov = __shfl_xor_sync(0xffffffffu, bv, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-          if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-        }
-      } else {
-        bi = p.first_ids[b];  // multi-table mode, step 0: nothing predicted, the known first id is fed
-      }
+      // bookkeeping operands first: their round trips overlap the candidate loads
+      const int was_done = p.done[b];
+      const int forced_tok = p.forced ? p.forced[b * p.n_steps + step] : 0;
+      int tok;
+      if (sampled) tok = stok;
+      else if (ld_has_head(p, step)) tok = dec_argmax_merge(p.cand_val, p.cand_idx, b);
+      else tok = p.first_ids[b];  // multi-table mode, step 0: nothing predicted, the known first id is fed
       if (lane == 0) {
-        int tok = bi;
-        const bool was_done = p.done[b] != 0;
-        if (was_done) tok = p.eos;
-        p.out_ids[b * p.n_steps + step] = tok;
-        if (!was_done && !p.forced) {
-          if (tok == p.eos) { p.done[b] = 1; p.out_len[b] = step + 1; atomicAdd(p.n_done, 1); }
-          else if (step == p.n_steps - 1) { p.out_len[b] = p.n_steps; }
-        }
-        if (p.forced && step == p.n_steps - 1) p.out_len[b] = p.n_steps;
-        *s_feed = p.forced ? p.forced[b * p.n_steps + step] : tok;
-        if (sc && sc->penalty != 1.f && !p.seen_fixed) {
-          const int f = *s_feed;
-          atomicOr(p.seen + (long long)p.slot[b] * p.seen_words + (f >> 5), 1u << (f & 31));
-        }
+        const int f = dec_record_token(p, b, step, p.n_steps, tok, was_done, forced_tok);
+        *s_feed = f;
+        if (sc && sc->penalty != 1.f && !p.seen_fixed) atomicOr(p.seen + (long long)p.slot[b] * p.seen_words + (f >> 5), 1u << (f & 31));
         p.pos[b] = p.pos[b] + 1;  // the fed token sits at the next position
       }
     }
@@ -205,92 +169,101 @@ __device__ __noinline__ void ld_select(const LlamaDecParams& p, int step, float*
   }
 }
 
+// The kernel's phases for dec_run (decode_common.cuh).  Holds a reference to the kernel's shared copy of the parameters.
 template <typename T>
-__device__ __forceinline__ bool ld_gemv_args(const LlamaDecParams& p, int step, int ph, GemvArgs& a) {
-  const int d = p.d, B = p.B, qd = p.heads * p.hd, kvd = p.kv_heads * p.hd;
-  a.K = d; a.mode = EPI_STORE; a.out = p.q; a.ldo = qd; a.out_h = nullptr; a.ldh = 0; a.d = d; a.kv0 = nullptr; a.kv_which = 0; a.kv_batch = 0;
-  a.suppress = nullptr; a.first_step = 0; a.logits_out = nullptr; a.logits_ld = 0; a.bias = nullptr; a.W = nullptr; a.N = 0;
-  a.pos = p.pos; a.slot = p.slot; a.kv_slot = p.kv_slot_stride; a.kv_ld = kvd; a.rope = p.rope; a.hd = p.hd;
-  a.q_rows = qd; a.k_rows = kvd; a.q_scale = rsqrtf((float)p.hd); a.kraw = nullptr; a.plan_id = -1;
-  a.xsrc = nullptr; a.xsrc_ld = 0; a.kc = 0;
-  const int kind = ld_kind(p, ph);
-  if (kind < 6) {
-    const int layer = ph / ld_nsub(p);
-    const LlamaDecLayer& w = p.lw[layer];
-    switch (kind) {
-      case 0:
-        a.W = w.w_qkv; a.N = qd + 2 * kvd; a.mode = EPI_QKV_ROPE; a.out = p.q; a.ldo = qd; a.plan_id = 0;
-        a.kv0 = reinterpret_cast<T*>(p.kv) + (long long)layer * p.kv_layer_stride; a.kv_which = p.kv_which_stride;
-        a.kraw = p.qk_norm ? p.kraw : nullptr;
-        return true;
-      case 2: a.W = w.w_o; a.N = d; a.K = qd; a.mode = EPI_RESID; a.out = p.x; a.ldo = d; a.plan_id = 1; return true;
-      case 3: a.W = w.w_gu; a.N = 2 * p.ffn; a.mode = EPI_SWIGLU; a.out_h = p.h; a.ldh = p.ffn; a.plan_id = 2; return true;
-      case 4:
-        a.W = w.w_down; a.N = d; a.K = p.ffn; a.mode = EPI_RESID; a.out = p.x; a.ldo = d; a.plan_id = 3;
-        if (p.down_kc > 0) { a.xsrc = p.h; a.xsrc_ld = p.ffn; a.kc = p.down_kc; a.plan_id = -1; }
-        return true;
-      default: return false;
+struct LdModel {
+  static constexpr bool stamps_barrier = true;
+  const LlamaDecParams& p;
+  int n_phases;
+
+  __device__ __forceinline__ bool skip(int step, int ph) const {   // nothing to predict: no work, no barrier
+    return ld_kind(p, ph) == 6 && !ld_has_head(p, step);
+  }
+  __device__ __forceinline__ bool has_gemv(int step, int ph) const { return ld_has_gemv(p, step, ph); }
+  __device__ __forceinline__ bool lookahead_target(int step, int ph) const { return ld_has_gemv(p, step, ph); }
+  __device__ __forceinline__ void prefetch_l2(int, int) const {}
+  __device__ __forceinline__ DecNorm norm_of(int ph) const {
+    const int k = ld_kind(p, ph);
+    if (k == 0) return {p.lw[ph / ld_nsub(p)].norm1, nullptr};
+    if (k == 3) return {p.lw[ph / ld_nsub(p)].norm2, nullptr};
+    return {k == 6 ? p.norm_f : nullptr, nullptr};
+  }
+
+  __device__ __forceinline__ void gemv_args(int step, int ph, GemvArgs& a) const {
+    const int d = p.d, B = p.B, qd = p.heads * p.hd, kvd = p.kv_heads * p.hd;
+    gemv_args_reset(a, d, p.q);
+    a.pos = p.pos; a.slot = p.slot; a.kv_slot = p.kv_slot_stride; a.kv_ld = kvd; a.rope = p.rope; a.hd = p.hd;
+    a.q_rows = qd; a.k_rows = kvd; a.q_scale = rsqrtf((float)p.hd);
+    const int kind = ld_kind(p, ph);
+    if (kind < 6) {
+      const int layer = ph / ld_nsub(p);
+      const LlamaDecLayer& w = p.lw[layer];
+      switch (kind) {
+        case 0:
+          a.W = w.w_qkv; a.N = qd + 2 * kvd; a.mode = EPI_QKV_ROPE; a.out = p.q; a.ldo = qd; a.plan_id = 0;
+          a.kv0 = reinterpret_cast<T*>(p.kv) + (long long)layer * p.kv_layer_stride; a.kv_which = p.kv_which_stride;
+          a.kraw = p.qk_norm ? p.kraw : nullptr;
+          return;
+        case 2: a.W = w.w_o; a.N = d; a.K = qd; a.mode = EPI_RESID; a.out = p.x; a.ldo = d; a.plan_id = 1; return;
+        case 3: a.W = w.w_gu; a.N = 2 * p.ffn; a.mode = EPI_SWIGLU; a.out_h = p.h; a.ldh = p.ffn; a.plan_id = 2; return;
+        case 4:
+          a.W = w.w_down; a.N = d; a.K = p.ffn; a.mode = EPI_RESID; a.out = p.x; a.ldo = d; a.plan_id = 3;
+          if (p.down_kc > 0) { a.xsrc = p.h; a.xsrc_ld = p.ffn; a.kc = p.down_kc; a.plan_id = -1; }
+          return;
+        default: return;
+      }
+    }
+    if (kind == 6 && ld_has_head(p, step)) {
+      a.W = ld_multi(p) ? reinterpret_cast<const T*>(p.lm_head) + (long long)(step - 1) * p.head_stride : p.lm_head;
+      a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 4; a.suppress = p.suppress;
+      // sessions that sample read their row back in the select phase: from logits_out when the caller asked for it, else from
+      // the row scratch (every row of such a launch is stored, a few MB against the step's weight stream)
+      a.logits_out = p.logits_out ? p.logits_out + (long long)step * B * p.vocab : p.samp ? p.samp_rows : nullptr;
+      a.logits_ld = p.vocab;
     }
   }
-  if (kind == 6 && ld_has_head(p, step)) {
-    a.W = ld_multi(p) ? reinterpret_cast<const T*>(p.lm_head) + (long long)(step - 1) * p.head_stride : p.lm_head;
-    a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 4; a.suppress = p.suppress;
-    // sessions that sample read their row back in the select phase: from logits_out when the caller asked for it, else from
-    // the row scratch (every row of such a launch is stored, a few MB against the step's weight stream)
-    a.logits_out = p.logits_out ? p.logits_out + (long long)step * B * p.vocab : p.samp ? p.samp_rows : nullptr;
-    a.logits_ld = p.vocab;
-    return true;
-  }
-  return false;
-}
 
-template <typename T>
-struct LdSmem {
-  T* xh; float* xs; float* sv; int* si; float* s_red; float* wb; float4* red;
+  __device__ __forceinline__ void phase(int step, int ph, const DecViews<T>& sm, GemvRing& ring, GemvArgs* ready,
+                                        GemvArgs* scratch, int wb_ready, unsigned long long*) const {
+    const int d = p.d, B = p.B;
+    float best_v[2] = {-INFINITY, -INFINITY};
+    int best_i[2] = {0x7fffffff, 0x7fffffff};
+    const int kind = ld_kind(p, ph);
+    if (!ready && ld_has_gemv(p, step, ph)) {
+      if (threadIdx.x == 0) gemv_args(step, ph, *scratch);  // one thread writes the shared struct
+      __syncthreads();
+    }
+    GemvArgs& a = ready ? *ready : *scratch;
+    if (kind < 6) {
+      const int layer = ph / ld_nsub(p);
+      const LlamaDecLayer& w = p.lw[layer];
+      switch (kind) {
+        case 0: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 2, w.norm1, nullptr, p.eps, sm.s_red, sm.wb, wb_ready, p.norm_rg); break;
+        case 1:
+          if (p.hd == 128) ld_attn<T, 128>(p, layer, step, reinterpret_cast<float*>(sm.red));
+          else ld_attn<T, 64>(p, layer, step, reinterpret_cast<float*>(sm.red));
+          return;
+        case 2: stage_rows_copy<T>(reinterpret_cast<const T*>(p.attn16), B, p.heads * p.hd, sm.xh); break;
+        case 3: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 2, w.norm2, nullptr, p.eps, sm.s_red, sm.wb, wb_ready, p.norm_rg); break;
+        default:
+          if (a.kc > 0) { gemv_mma_chunked<T, true>(a, sm.xh, B, best_v, best_i, ring, sm.red); return; }
+          stage_rows_copy<T>(reinterpret_cast<const T*>(p.h), B, p.ffn, sm.xh); break;
+      }
+      gemv_mma<T, true>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
+      return;
+    }
+    if (kind == 6) {
+      if (p.hidden_out && blockIdx.x == 0)  // the residual stream before the final norm (Qwen3-TTS: input of the code predictor)
+        for (int i = threadIdx.x; i < B * d; i += DEC_THREADS) p.hidden_out[(long long)step * B * d + i] = __ldcg(p.x + i);
+      stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 2, p.norm_f, nullptr, p.eps, sm.s_red, sm.wb, wb_ready, p.norm_rg);
+      gemv_mma<T, true>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
+      gemv_argmax_candidates(best_v, best_i, B, sm.sv, sm.si, p.cand_val, p.cand_idx);
+    } else {
+      static_assert(sizeof(SampShared) <= 2 * DEC_THREADS * 16, "sampling scratch must fit the tail-round buffer");
+      ld_select<T>(p, step, sm.sv, *reinterpret_cast<SampShared*>(sm.red));
+    }
+  }
 };
-
-template <typename T>
-__device__ __forceinline__ void ld_phase(const LlamaDecParams& p, int step, int ph, const LdSmem<T>& sm, GemvRing& ring,
-                                         GemvArgs* ready, GemvArgs& a_scratch, int wb_ready) {
-  const int d = p.d, B = p.B;
-  float best_v[2] = {-INFINITY, -INFINITY};
-  int best_i[2] = {0x7fffffff, 0x7fffffff};
-  // argument struct and ring state live in shared memory (all threads write identical values), not on the stack
-  const int kind = ld_kind(p, ph);
-  if (!ready && ld_has_gemv(p, step, ph)) {
-    if (threadIdx.x == 0) ld_gemv_args<T>(p, step, ph, a_scratch);  // one thread writes the shared struct
-    __syncthreads();
-  }
-  GemvArgs& a = ready ? *ready : a_scratch;
-  if (kind < 6) {
-    const int layer = ph / ld_nsub(p);
-    const LlamaDecLayer& w = p.lw[layer];
-    switch (kind) {
-      case 0: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 2, w.norm1, nullptr, p.eps, sm.s_red, sm.wb, wb_ready, p.norm_rg); break;
-      case 1:
-        if (p.hd == 128) ld_attn<T, 128>(p, layer, step, reinterpret_cast<float*>(sm.red));
-        else ld_attn<T, 64>(p, layer, step, reinterpret_cast<float*>(sm.red));
-        return;
-      case 2: stage_rows_copy<T>(reinterpret_cast<const T*>(p.attn16), B, p.heads * p.hd, sm.xh); break;
-      case 3: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 2, w.norm2, nullptr, p.eps, sm.s_red, sm.wb, wb_ready, p.norm_rg); break;
-      default:
-        if (a.kc > 0) { gemv_mma_chunked<T, true>(a, sm.xh, B, best_v, best_i, ring, sm.red); return; }
-        stage_rows_copy<T>(reinterpret_cast<const T*>(p.h), B, p.ffn, sm.xh); break;
-    }
-    gemv_mma<T, true>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-    return;
-  }
-  if (kind == 6) {
-    if (p.hidden_out && blockIdx.x == 0)  // the residual stream before the final norm (Qwen3-TTS: input of the code predictor)
-      for (int i = threadIdx.x; i < B * d; i += DEC_THREADS) p.hidden_out[(long long)step * B * d + i] = __ldcg(p.x + i);
-    stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 2, p.norm_f, nullptr, p.eps, sm.s_red, sm.wb, wb_ready, p.norm_rg);
-    gemv_mma<T, true>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-    gemv_argmax_candidates(best_v, best_i, B, sm.sv, sm.si, p.cand_val, p.cand_idx);
-  } else {
-    static_assert(sizeof(SampShared) <= 2 * DEC_THREADS * 16, "sampling scratch must fit the tail-round buffer");
-    ld_select<T>(p, step, sm.sv, *reinterpret_cast<SampShared*>(sm.red));
-  }
-}
 
 template <typename T>
 __global__ void __launch_bounds__(DEC_THREADS, 1)
@@ -310,78 +283,10 @@ llama_decode_kernel(const LlamaDecParams p, int step_begin, int step_end, int ph
   __syncthreads();
   const int kmax_whole = p.down_kc > 0 ? ld_kmax(p.d, p.down_kc, p.heads * p.hd) : ld_kmax(p.d, p.ffn, p.heads * p.hd);
   const DecSmem lay = dec_smem_layout(p.B, p.d, kmax_whole, p.d, p.norm_rg);
-  LdSmem<T> sm;
-  sm.xh = reinterpret_cast<T*>(smem_raw);
-  sm.xs = reinterpret_cast<float*>(smem_raw + lay.xs_off);
-  sm.sv = reinterpret_cast<float*>(smem_raw + lay.aux_off);
-  sm.si = reinterpret_cast<int*>(smem_raw + lay.si_off);
-  sm.s_red = reinterpret_cast<float*>(smem_raw + lay.red_s_off);
-  sm.wb = reinterpret_cast<float*>(smem_raw + lay.wb_off);
-  sm.red = reinterpret_cast<float4*>(smem_raw + lay.redbuf_off);
   GemvRing& ring = s_rings[threadIdx.x >> 5];
-  {
-    unsigned char* rb = smem_raw + lay.ring_off;
-    const int warp = threadIdx.x >> 5;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(rb + (size_t)DEC_WARPS * p.ring_slots * GV_SLOT_BYTES) + warp * p.ring_slots;
-    if ((threadIdx.x & 31) == 0) {   // lane 0 owns the warp's ring state in shared memory
-      ring.slots = p.ring_slots;
-      ring.base_s = smem_u32(rb + (size_t)warp * p.ring_slots * GV_SLOT_BYTES);
-      ring.bars_s = smem_u32(bars);
-      ring.slot = 0;
-      ring.parity = 0;
-      ring.plans_s = s_plans;
-      ring.pre_valid = 0; ring.pre_pj = 0; ring.pre_pu = 0; ring.pre_nvalid = 0; ring.pre_W = nullptr;
-      for (int i = 0; i < p.ring_slots; ++i) mbar_init(bars + i, 1);
-      fence_barrier_init();
-    }
-    __syncthreads();
-  }
-  unsigned int epoch = 0;
-  int trace_i = 0;
-  GemvArgs& pre_args = s_args[0];
-  if (threadIdx.x == 0) pre_args.K = p.d;
-  int pre_tag = -1, wb_tag = -1;
-  const int n_ph = ld_nsub(p) * p.layers + 2;
-  for (int step = step_begin; step < step_end; ++step) {
-    const int pb = coop ? 0 : ph_begin, pe = coop ? n_ph : ph_end;
-    for (int ph = pb; ph < pe; ++ph) {
-      const bool tracing = sp.trace && trace_i < sp.trace_cap && threadIdx.x == 0 && blockIdx.x == 0;
-      unsigned long long* tr = tracing ? sp.trace + (long long)trace_i * 3 : nullptr;
-      if (tracing) tr[0] = gtimer_ns();
-      const bool skip = ld_kind(sp, ph) == 6 && !ld_has_head(sp, step);  // nothing to predict: no work, no barrier
-      if (!skip) ld_phase<T>(sp, step, ph, sm, ring, (pre_tag == step * n_ph + ph) ? &pre_args : nullptr, s_args[1], wb_tag == step * n_ph + ph);
-      if (tracing) tr[1] = gtimer_ns();
-      if (coop && !skip) {
-        grid_arrive(p.sync_counter, epoch);
-        // ---- between arrive and wait: prepare the next projection (arguments, first weight units, norm weights) ----
-        if (!ring.pre_valid) {
-          int nph = ph + 1, nstep = step;
-          if (nph == n_ph) { nph = 0; nstep = step + 1; }
-#pragma unroll 1
-          for (int look = 0; look < 3 && nstep < step_end; ++look) {
-            if (ld_has_gemv(sp, nstep, nph)) {
-              if (threadIdx.x == 0) ld_gemv_args<T>(sp, nstep, nph, pre_args);  // one thread writes the shared struct
-              __syncthreads();
-              if (pre_args.kc == 0) gemv_prefetch<T>(pre_args, ring);   // a K-chunked projection starts its own stream
-              pre_tag = nstep * n_ph + nph;
-              const float* nw = nullptr;
-              const int nk = ld_kind(sp, nph);
-              if (nk == 0) nw = sp.lw[nph / ld_nsub(sp)].norm1; else if (nk == 3) nw = sp.lw[nph / ld_nsub(sp)].norm2;
-              else if (nk == 6) nw = sp.norm_f;
-              if (nw && wb_tag != pre_tag) { stage_norm_weights(nw, nullptr, sp.d, sm.wb); wb_tag = pre_tag; }
-              break;
-            }
-            if (++nph == n_ph) { nph = 0; ++nstep; }
-          }
-        }
-        grid_wait(p.sync_counter, epoch, p.sync_relaxed);
-      }
-      if (tracing) tr[2] = gtimer_ns();
-      ++trace_i;
-    }
-    if (coop && !p.forced && *reinterpret_cast<volatile int*>(p.n_done) >= p.B) break;
-  }
-  gemv_drain(pre_args.K, ring);
+  gemv_ring_init(ring, smem_raw + lay.ring_off, p.ring_slots, s_plans);
+  const LdModel<T> model{sp, ld_nsub(p) * p.layers + 2};
+  dec_run<T>(p, model, dec_views<T>(smem_raw, lay), ring, s_args, step_begin, step_end, ph_begin, ph_end, coop);
 }
 
 template <typename T>
@@ -394,19 +299,13 @@ __global__ void llama_decode_init_kernel(const LlamaDecParams p) {
     const T* e = reinterpret_cast<const T*>(p.embed) + (long long)tok * p.d;
     for (int i = threadIdx.x; i < p.d; i += blockDim.x) p.x[(long long)b * p.d + i] = DT<T>::to_f(e[i]);
   }
-  if (threadIdx.x == 0) {
-    p.done[b] = 0;
-    p.out_len[b] = 0;
-    if (b == 0) { *p.n_done = 0; *p.sync_counter = 0; }
-    for (int h = 0; h < p.heads; ++h) p.attn_cnt[b * p.heads + h] = 0u;
-    // the first fed id is in the sequence now: it joins the seen set of a session with a repetition penalty (the select
-    // phase adds the ids fed after it)
-    if (p.samp && p.samp[b].active && p.samp[b].penalty != 1.f && !p.seen_fixed) {
-      const int f = p.first_ids[b];
-      atomicOr(p.seen + (long long)p.slot[b] * p.seen_words + (f >> 5), 1u << (f & 31));
-    }
+  // the first fed id is in the sequence now: it joins the seen set of a session with a repetition penalty (the select
+  // phase adds the ids fed after it)
+  if (threadIdx.x == 0 && p.samp && p.samp[b].active && p.samp[b].penalty != 1.f && !p.seen_fixed) {
+    const int f = p.first_ids[b];
+    atomicOr(p.seen + (long long)p.slot[b] * p.seen_words + (f >> 5), 1u << (f & 31));
   }
-  for (int i = threadIdx.x; i < p.n_steps; i += blockDim.x) p.out_ids[b * p.n_steps + i] = p.eos;
+  dec_init_session(p, b, p.n_steps);
 }
 
 template <typename T>
@@ -432,22 +331,7 @@ int launch_t(s2s_ctx* ctx, const LlamaDecParams& p, int debug_phases, cudaStream
   S2S_CHECK_CUDA(s2s_opt_in_max_smem(kern, ctx->device, smem, nullptr));
   llama_decode_init_kernel<T><<<p.B, 256, 0, stream>>>(pr);
   S2S_LAUNCH_CHECK();
-  const int n_ph = ld_nsub(p) * p.layers + 2;
-  if (!debug_phases) {
-    int sb = 0, se = p.n_steps, pb = 0, pe = n_ph, coop = 1;
-    LlamaDecParams pp = pr;
-    void* args[] = {&pp, &sb, &se, &pb, &pe, &coop};
-    S2S_CHECK_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(DEC_THREADS), args, smem, stream));
-    s2s_count_launch();
-  } else {
-    for (int s = 0; s < p.n_steps; ++s)
-      for (int ph = 0; ph < n_ph; ++ph) {
-        if (ph == n_ph - 2 && pr.head_stride != 0 && s == 0) continue;  // multi-table mode: step 0 predicts nothing
-        kern<<<grid, DEC_THREADS, smem, stream>>>(pr, s, s + 1, ph, ph + 1, 0);
-        S2S_LAUNCH_CHECK();
-      }
-  }
-  return S2S_OK;
+  return dec_launch(kern, pr, grid, 0, smem, p.n_steps, ld_nsub(p) * p.layers + 2, debug_phases, stream);
 }
 
 }  // namespace

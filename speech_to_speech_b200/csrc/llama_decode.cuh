@@ -61,7 +61,7 @@ struct LlamaDecParams {
                                 // DEC_NORM_L2 = no copy, rows read from L2 into registers)
   int down_kc;                  // > 0: the down-projection operand is staged in K-chunks of this many columns (large batches)
   int assoc_b;                  // the batch whose plan fixes the attention split plan (set by the launcher, see LlamaDecPlan)
-  unsigned long long* trace;    // optional [cap][3] globaltimer stamps of CTA 0 (phase begin, body end, barrier exit)
+  unsigned long long* trace;    // optional [2][cap][6] globaltimer stamps (profiling aid, dec_run)
   int trace_cap;
   int sync_relaxed;             // 1: barrier waits without the acquire fence (A/B measurement aid)
   // ---- per-session token choice (sampling.cuh); samp == null: every session takes the argmax-candidate path ----

@@ -29,13 +29,6 @@ constexpr long long WD_SMEM_BUDGET = 220LL * 1024 - 128;
 
 namespace {
 
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
-
-
 constexpr int HD = 64;
 static_assert(ATT_CHUNK == ATT_CHUNK_KEYS, "chunk size mismatch");
 
@@ -69,34 +62,17 @@ __device__ __noinline__ void wd_prefetch(const WhisperDecParams& p, int step, in
 template <typename T>
 __device__ __forceinline__ void wd_attn_items(const WhisperDecParams& p, int plan, int n_keys, const T* kv0, long long b_stride,
                                               long long h_stride, long long v_off, long long ld, float* rec_s) {
-  const int d = p.d, H = p.heads, warp = threadIdx.x >> 5;
+  const int d = p.d, H = p.heads;
   constexpr int REC = HD + PART_PAD;
   const int n_blocks = (n_keys + ATT_BLK - 1) / ATT_BLK, BH = p.B * H;
   const int S = plan & 0x7f, bps = (n_blocks + S - 1) / S;
-  if (plan & ATTN_WARP_LEVEL) {
+  const bool wl = plan & ATTN_WARP_LEVEL;
 #pragma unroll 1
-    for (int it = dec_first_item(); it < BH * S; it += dec_item_stride()) {
-      const int s = it % S, bh = it / S, h = bh % H, b = bh / H;
-      const T* Kb = kv0 + b * b_stride + h * h_stride;
-      attend_blocks<T, HD>(p.q + b * d + h * HD, Kb, Kb + v_off, ld, ld, n_keys, s * bps, min((s + 1) * bps, n_blocks), 1,
-                           rec_s + warp * REC);
-      attn_finish_item<T, HD>(rec_s + warp * REC, 1, p.part + (long long)bh * p.s_max * REC, s, S, p.attn_cnt + bh,
-                              reinterpret_cast<T*>(p.attn16) + (long long)b * d + h * HD);
-      __syncwarp();
-    }
-    return;
-  }
-#pragma unroll 1
-  for (int it = blockIdx.x; it < BH * S; it += gridDim.x) {
+  for (int it = wl ? dec_first_item() : (int)blockIdx.x; it < BH * S; it += wl ? dec_item_stride() : (int)gridDim.x) {
     const int s = it % S, bh = it / S, h = bh % H, b = bh / H;
     const T* Kb = kv0 + b * b_stride + h * h_stride;
-    attend_blocks<T, HD>(p.q + b * d + h * HD, Kb, Kb + v_off, ld, ld, n_keys, s * bps + warp, min((s + 1) * bps, n_blocks),
-                         DEC_WARPS, rec_s + warp * REC);
-    __syncthreads();
-    if (warp == 0)
-      attn_finish_item<T, HD>(rec_s, DEC_WARPS, p.part + (long long)bh * p.s_max * REC, s, S, p.attn_cnt + bh,
-                              reinterpret_cast<T*>(p.attn16) + (long long)b * d + h * HD);
-    __syncthreads();
+    attn_run_item<T, HD>(wl, p.q + b * d + h * HD, Kb, Kb + v_off, ld, n_keys, s * bps, min((s + 1) * bps, n_blocks), rec_s,
+                         p.part + (long long)bh * p.s_max * REC, s, S, p.attn_cnt + bh, reinterpret_cast<T*>(p.attn16) + (long long)b * d + h * HD);
   }
 }
 
@@ -129,30 +105,11 @@ __device__ __noinline__ void wd_select(const WhisperDecParams& p, int g, int pos
     if (warp == 0) {
       if (g >= 0) {
         // bookkeeping operands first: their round trips overlap the candidate loads
-        const int was_done_i = p.done[b];
+        const int was_done = p.done[b];
         const int forced_tok = p.forced ? p.forced[b * p.max_new + g] : 0;
-        float bv = -INFINITY; int bi = 0x7fffffff;
-#pragma unroll 1
-        for (int c = lane; c < (int)gridDim.x; c += 32) {
-          const float v = __ldcg(p.cand_val + b * gridDim.x + c); const int i = __ldcg(p.cand_idx + b * gridDim.x + c);
-          if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
-        }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-          const float ov = __shfl_xor_sync(0xffffffffu, bv, o); const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
-          if (ov > bv || (ov == bv && oi < bi)) { bv = ov; bi = oi; }
-        }
+        const int tok = dec_argmax_merge(p.cand_val, p.cand_idx, b);
         if (lane == 0) {
-          int tok = bi;
-          const bool was_done = was_done_i != 0;
-          if (was_done) tok = p.eos;
-          p.out_ids[b * p.max_new + g] = tok;
-          if (!was_done && !p.forced) {
-            if (tok == p.eos) { p.done[b] = 1; p.out_len[b] = g + 1; atomicAdd(p.n_done, 1); }
-            else if (g == p.max_new - 1) { p.out_len[b] = p.max_new; }
-          }
-          if (p.forced && g == p.max_new - 1) p.out_len[b] = p.max_new;
-          const int feed = p.forced ? forced_tok : tok;
+          const int feed = dec_record_token(p, b, g, p.max_new, tok, was_done, forced_tok);
           if (pos + 1 < p.max_pos) p.tokens[b * p.max_pos + pos + 1] = feed;
           *s_feed = feed;
         }
@@ -171,100 +128,103 @@ __device__ __noinline__ void wd_select(const WhisperDecParams& p, int g, int pos
   }
 }
 
-// does phase `ph` of token step `step` start with a projection?  (pure predicate: the argument struct lives in shared
-// memory and is written by ONE warp, so nobody may call wd_gemv_args just to find out)
-__device__ __forceinline__ bool wd_has_gemv(const WhisperDecParams& p, int step, int ph) {
-  if (ph < 8 * p.layers) return (ph & 7) != 1 && (ph & 7) != 4;
-  return ph == 8 * p.layers && step >= p.n_prefix - 1;
-}
-
-// Arguments of the projection GEMV of phase `ph` (false: the phase has none).  Shared by the phase itself and by
-// the cross-barrier weight prefetch of the NEXT projection.
+// The 8-phase kernel's phases for dec_run (decode_common.cuh).  Holds a reference to the kernel's shared copy of the parameters.
 template <typename T>
-__device__ __forceinline__ bool wd_gemv_args(const WhisperDecParams& p, int step, int ph, GemvArgs& a) {
-  const int L = p.layers, pos = step, d = p.d, B = p.B;
-  a.K = d; a.mode = EPI_STORE; a.out = p.q; a.ldo = d; a.out_h = nullptr; a.ldh = 0; a.d = d; a.kv0 = nullptr; a.kv_which = 0; a.kv_batch = 0;
-  a.suppress = nullptr; a.first_step = 0; a.logits_out = nullptr; a.logits_ld = 0; a.bias = nullptr; a.W = nullptr; a.N = 0;
-  a.pos = nullptr; a.slot = nullptr; a.kv_slot = 0; a.kv_ld = 0; a.rope = nullptr; a.hd = HD; a.q_rows = 0; a.k_rows = 0; a.q_scale = 1.f; a.kraw = nullptr; a.xsrc = nullptr; a.xsrc_ld = 0; a.kc = 0; a.plan_id = 1;
-  if (ph < 8 * L) {
-    const int layer = ph >> 3;
-    const WhisperDecLayer& w = p.lw[layer];
-    switch (ph & 7) {
-      case 0: {
-        const long long kvs = (long long)p.max_pos * d;
-        a.W = w.w_qkv; a.N = 3 * d; a.bias = w.b_qkv; a.mode = EPI_QKV; a.out = p.q; a.plan_id = 0;
-        a.kv0 = reinterpret_cast<T*>(p.self_kv) + ((long long)layer * 2) * kvs + (long long)pos * d;
-        a.kv_which = kvs; a.kv_batch = (long long)L * 2 * kvs;
-      } return true;
-      case 2: a.W = w.w_o; a.N = d; a.bias = w.b_o; a.mode = EPI_RESID; a.out = p.x; return true;
-      case 3: a.W = w.w_cq; a.N = d; a.bias = w.b_cq; a.mode = EPI_STORE; a.out = p.q; return true;
-      case 5: a.W = w.w_co; a.N = d; a.bias = w.b_co; a.mode = EPI_RESID; a.out = p.x; return true;
-      case 6: a.W = w.w_fc1; a.N = p.ffn; a.bias = w.b_fc1; a.mode = EPI_GELU; a.out_h = p.h; a.ldh = p.ffn; a.plan_id = 2; return true;
-      case 7: a.W = w.w_fc2; a.N = d; a.K = p.ffn; a.bias = w.b_fc2; a.mode = EPI_RESID; a.out = p.x; a.plan_id = 3; return true;
-      default: return false;
+struct WdModel {
+  static constexpr bool stamps_barrier = true;
+  const WhisperDecParams& p;
+  int n_phases;
+
+  // the logits phase is skipped while the forced prompt is still being fed
+  __device__ __forceinline__ bool skip(int step, int ph) const { return ph == 8 * p.layers && step < p.n_prefix - 1; }
+  // pure predicate: the argument struct lives in shared memory and is written by ONE thread, so nobody may call gemv_args
+  // just to find out
+  __device__ __forceinline__ bool has_gemv(int step, int ph) const {
+    if (ph < 8 * p.layers) return (ph & 7) != 1 && (ph & 7) != 4;
+    return ph == 8 * p.layers && step >= p.n_prefix - 1;
+  }
+  __device__ __forceinline__ bool lookahead_target(int step, int ph) const { return has_gemv(step, ph); }
+  __device__ __forceinline__ void prefetch_l2(int step, int ph) const { wd_prefetch<T>(p, step, ph); }
+  __device__ __forceinline__ DecNorm norm_of(int ph) const {
+    if (ph >= 8 * p.layers) return {p.lnf_w, p.lnf_b};
+    const WhisperDecLayer& w = p.lw[ph >> 3];
+    const int sub = ph & 7;
+    if (sub == 0) return {w.ln1_w, w.ln1_b};
+    if (sub == 3) return {w.ln2_w, w.ln2_b};
+    if (sub == 6) return {w.ln3_w, w.ln3_b};
+    return {nullptr, nullptr};
+  }
+
+  // arguments of the projection GEMV of phase `ph` (has_gemv): shared by the phase itself and by the look-ahead
+  __device__ __forceinline__ void gemv_args(int step, int ph, GemvArgs& a) const {
+    const int L = p.layers, pos = step, d = p.d, B = p.B;
+    gemv_args_reset(a, d, p.q);
+    a.plan_id = 1;
+    if (ph < 8 * L) {
+      const int layer = ph >> 3;
+      const WhisperDecLayer& w = p.lw[layer];
+      switch (ph & 7) {
+        case 0: {
+          const long long kvs = (long long)p.max_pos * d;
+          a.W = w.w_qkv; a.N = 3 * d; a.bias = w.b_qkv; a.mode = EPI_QKV; a.out = p.q; a.plan_id = 0;
+          a.kv0 = reinterpret_cast<T*>(p.self_kv) + ((long long)layer * 2) * kvs + (long long)pos * d;
+          a.kv_which = kvs; a.kv_batch = (long long)L * 2 * kvs;
+        } return;
+        case 2: a.W = w.w_o; a.N = d; a.bias = w.b_o; a.mode = EPI_RESID; a.out = p.x; return;
+        case 3: a.W = w.w_cq; a.N = d; a.bias = w.b_cq; a.mode = EPI_STORE; a.out = p.q; return;
+        case 5: a.W = w.w_co; a.N = d; a.bias = w.b_co; a.mode = EPI_RESID; a.out = p.x; return;
+        case 6: a.W = w.w_fc1; a.N = p.ffn; a.bias = w.b_fc1; a.mode = EPI_GELU; a.out_h = p.h; a.ldh = p.ffn; a.plan_id = 2; return;
+        case 7: a.W = w.w_fc2; a.N = d; a.K = p.ffn; a.bias = w.b_fc2; a.mode = EPI_RESID; a.out = p.x; a.plan_id = 3; return;
+        default: return;
+      }
+    }
+    const int g = step - (p.n_prefix - 1);
+    if (ph == 8 * L && g >= 0) {
+      a.W = p.embed_t; a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 4; a.suppress = p.suppress; a.first_step = (g == 0);
+      a.logits_out = p.logits_out ? p.logits_out + (long long)g * B * p.vocab : nullptr; a.logits_ld = p.vocab;
     }
   }
-  const int g = step - (p.n_prefix - 1);
-  if (ph == 8 * L && g >= 0) {
-    a.W = p.embed_t; a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 4; a.suppress = p.suppress; a.first_step = (g == 0);
-    a.logits_out = p.logits_out ? p.logits_out + (long long)g * B * p.vocab : nullptr; a.logits_ld = p.vocab;
-    return true;
-  }
-  return false;
-}
 
-// Shared-memory views of one CTA (see dec_smem_layout)
-template <typename T>
-struct WdSmem {
-  T* xh; float* xs; float* sv; int* si; float* s_red; float* wb; float4* red;
-};
-
-// One phase = (stage inputs into shared memory) + (one shared routine).  Thin: only argument setup is inlined.
-template <typename T>
-__device__ __forceinline__ void wd_phase(const WhisperDecParams& p, int step, int ph, const WdSmem<T>& sm, GemvRing& ring,
-                                         GemvArgs* ready, GemvArgs& a_scratch, int wb_ready, unsigned long long* tr) {
-  const int L = p.layers, pos = step, d = p.d, B = p.B;
-  float best_v[2] = {-INFINITY, -INFINITY};
-  int best_i[2] = {0x7fffffff, 0x7fffffff};
-  // argument struct and ring state live in SHARED memory (every thread writes identical values): per-thread copies
-  // on the stack (256 x ~300 B) do not fit the small L1 left next to the weight rings and turned into L2 traffic
-  bool has_gemv = true;
-  if (!ready) {
-    has_gemv = wd_has_gemv(p, step, ph);
-    if (has_gemv) {
-      if (threadIdx.x == 0) wd_gemv_args<T>(p, step, ph, a_scratch);  // one thread writes, everybody reads after the barrier
+  // One phase = (stage inputs into shared memory) + (one shared routine).  Thin: only argument setup is inlined.
+  __device__ __forceinline__ void phase(int step, int ph, const DecViews<T>& sm, GemvRing& ring, GemvArgs* ready,
+                                        GemvArgs* scratch, int wb_ready, unsigned long long* tr) const {
+    const int L = p.layers, pos = step, d = p.d, B = p.B;
+    float best_v[2] = {-INFINITY, -INFINITY};
+    int best_i[2] = {0x7fffffff, 0x7fffffff};
+    // argument struct and ring state live in SHARED memory (one thread writes): per-thread copies on the stack
+    // (256 x ~300 B) do not fit the small L1 left next to the weight rings and turned into L2 traffic
+    if (!ready && has_gemv(step, ph)) {
+      if (threadIdx.x == 0) gemv_args(step, ph, *scratch);  // one thread writes, everybody reads after the barrier
       __syncthreads();
     }
-  }
-  GemvArgs& a = ready ? *ready : a_scratch;
-  if (ph < 8 * L) {
-    const int layer = ph >> 3;
-    const WhisperDecLayer& w = p.lw[layer];
-    switch (ph & 7) {
-      case 0: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, w.ln1_w, w.ln1_b, 1e-5f, sm.s_red, sm.wb, wb_ready); break;
-      case 1: wd_self_attn<T>(p, layer, pos, reinterpret_cast<float*>(sm.red)); return;
-      case 2: stage_rows_copy<T>(reinterpret_cast<const T*>(p.attn16), B, d, sm.xh); break;
-      case 3: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, w.ln2_w, w.ln2_b, 1e-5f, sm.s_red, sm.wb, wb_ready); break;
-      case 4: wd_cross_attn<T>(p, layer, reinterpret_cast<float*>(sm.red)); return;
-      case 5: stage_rows_copy<T>(reinterpret_cast<const T*>(p.attn16), B, d, sm.xh); break;
-      case 6: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, w.ln3_w, w.ln3_b, 1e-5f, sm.s_red, sm.wb, wb_ready); break;
-      default: stage_rows_copy<T>(reinterpret_cast<const T*>(p.h), B, p.ffn, sm.xh); break;
+    GemvArgs& a = ready ? *ready : *scratch;
+    if (ph < 8 * L) {
+      const int layer = ph >> 3;
+      const WhisperDecLayer& w = p.lw[layer];
+      switch (ph & 7) {
+        case 0: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, w.ln1_w, w.ln1_b, 1e-5f, sm.s_red, sm.wb, wb_ready); break;
+        case 1: wd_self_attn<T>(p, layer, pos, reinterpret_cast<float*>(sm.red)); return;
+        case 2: stage_rows_copy<T>(reinterpret_cast<const T*>(p.attn16), B, d, sm.xh); break;
+        case 3: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, w.ln2_w, w.ln2_b, 1e-5f, sm.s_red, sm.wb, wb_ready); break;
+        case 4: wd_cross_attn<T>(p, layer, reinterpret_cast<float*>(sm.red)); return;
+        case 5: stage_rows_copy<T>(reinterpret_cast<const T*>(p.attn16), B, d, sm.xh); break;
+        case 6: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, w.ln3_w, w.ln3_b, 1e-5f, sm.s_red, sm.wb, wb_ready); break;
+        default: stage_rows_copy<T>(reinterpret_cast<const T*>(p.h), B, p.ffn, sm.xh); break;
+      }
+      if (tr) tr[1] = dec_clock_ns();  // inputs staged
+      gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
+      return;
     }
-    if (tr) tr[1] = globaltimer_ns();  // inputs staged
-    gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-    return;
+    if (ph == 8 * L) {
+      // final LayerNorm + tied output projection + suppress masks + per-CTA argmax candidates
+      stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, p.lnf_w, p.lnf_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
+      gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
+      gemv_argmax_candidates(best_v, best_i, B, sm.sv, sm.si, p.cand_val, p.cand_idx);
+    } else {
+      wd_select<T>(p, step - (p.n_prefix - 1), pos, sm.sv);
+    }
   }
-  const int g = step - (p.n_prefix - 1);  // index of the token generated at this step
-  if (ph == 8 * L) {
-    if (!has_gemv) return;
-    // final LayerNorm + tied output projection + suppress masks + per-CTA argmax candidates
-    stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, p.lnf_w, p.lnf_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
-    gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-    gemv_argmax_candidates(best_v, best_i, B, sm.sv, sm.si, p.cand_val, p.cand_idx);
-  } else {
-    wd_select<T>(p, g, pos, sm.sv);
-  }
-}
+};
 
 template <typename T>
 __global__ void __launch_bounds__(DEC_THREADS, 1)
@@ -274,7 +234,7 @@ whisper_decode_kernel(const WhisperDecParams p, int step_begin, int step_end, in
   __shared__ WhisperDecLayer s_layers[32];  // per-layer pointer tables: no global pointer chase inside a phase
   __shared__ GemvPlan s_plans[5];           // qkv [3d,d] | [d,d] | fc1 [ffn,d] | fc2 [d,ffn] | logits [vocab,d]
   __shared__ GemvArgs s_args[2];            // [0] prepared for the next projection, [1] built in-phase
-  __shared__ GemvRing s_rings[DEC_WARPS];   // per-warp ring state (all lanes write identical values)
+  __shared__ GemvRing s_rings[DEC_WARPS];   // per-warp ring state
   if (threadIdx.x < 5) {
     const int i = threadIdx.x;
     gemv_make_plan(i == 0 ? 3 * p.d : i == 2 ? p.ffn : i == 4 ? p.vocab : p.d, i == 3 ? p.ffn : p.d, s_plans[i]);
@@ -283,88 +243,11 @@ whisper_decode_kernel(const WhisperDecParams p, int step_begin, int step_end, in
   for (int i = threadIdx.x; i < p.layers; i += DEC_THREADS) s_layers[i] = p.lw[i];
   __syncthreads();
   const DecSmem lay = dec_smem_layout(p.B, p.d, max(p.d, p.ffn), 2 * p.d);
-  WdSmem<T> sm;
-  sm.xh = reinterpret_cast<T*>(smem_raw);
-  sm.xs = reinterpret_cast<float*>(smem_raw + lay.xs_off);
-  sm.sv = reinterpret_cast<float*>(smem_raw + lay.aux_off);
-  sm.si = reinterpret_cast<int*>(smem_raw + lay.si_off);
-  sm.s_red = reinterpret_cast<float*>(smem_raw + lay.red_s_off);
-  sm.wb = reinterpret_cast<float*>(smem_raw + lay.wb_off);
-  sm.red = reinterpret_cast<float4*>(smem_raw + lay.redbuf_off);
   GemvRing& ring = s_rings[threadIdx.x >> 5];
-  {
-    unsigned char* rb = smem_raw + lay.ring_off;
-    const int warp = threadIdx.x >> 5;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(rb + (size_t)DEC_WARPS * p.ring_slots * GV_SLOT_BYTES) + warp * p.ring_slots;
-    if ((threadIdx.x & 31) == 0) {   // lane 0 owns the warp's ring state in shared memory
-      ring.slots = p.ring_slots;
-      ring.base_s = smem_u32(rb + (size_t)warp * p.ring_slots * GV_SLOT_BYTES);
-      ring.bars_s = smem_u32(bars);
-      ring.slot = 0;
-      ring.parity = 0;
-      ring.plans_s = s_plans;
-      ring.pre_valid = 0; ring.pre_pj = 0; ring.pre_pu = 0; ring.pre_nvalid = 0; ring.pre_W = nullptr;
-      for (int i = 0; i < p.ring_slots; ++i) mbar_init(bars + i, 1);
-      fence_barrier_init();
-    }
-    __syncthreads();
-  }
-  unsigned int epoch = 0;
-  int trace_i = 0;
-  GemvArgs& pre_args = s_args[0];
-  if (threadIdx.x == 0) pre_args.K = p.d;
-  int pre_tag = -1, wb_tag = -1;  // (step, phase) the prepared arguments / staged norm weights belong to
-  const int n_ph = 8 * p.layers + 2;
-  for (int step = step_begin; step < step_end; ++step) {
-    const int pb = coop ? 0 : ph_begin, pe = coop ? n_ph : ph_end;
-    for (int ph = pb; ph < pe; ++ph) {
-      // the logits phase is skipped while the forced prompt is still being fed
-      const bool skip = (ph == 8 * p.layers) && (step < p.n_prefix - 1);
-      const bool tracing = sp.trace && trace_i < sp.trace_cap && threadIdx.x == 0 &&
-                           (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1);
-      unsigned long long* tr = tracing ? sp.trace + ((blockIdx.x == 0 ? 0 : 1) * (long long)sp.trace_cap + trace_i) * 6 : nullptr;
-      if (tracing) tr[0] = globaltimer_ns();
-      if (!skip) wd_phase<T>(sp, step, ph, sm, ring, (pre_tag == step * n_ph + ph) ? &pre_args : nullptr, s_args[1],
-                             wb_tag == step * n_ph + ph, tr);
-      if (tracing) tr[4] = globaltimer_ns();
-      if (coop && !skip) {
-        grid_arrive(p.sync_counter, epoch);
-        if (tracing) tr[2] = globaltimer_ns();  // arrived (results published)
-        // ---- between arrive and wait: everything for the NEXT phases that does not depend on other CTAs ----
-        int nph = ph + 1, nstep = step;
-        if (nph == n_ph) { nph = 0; nstep = step + 1; }
-        if (nstep < step_end) wd_prefetch<T>(sp, nstep, nph);  // cross-attention K/V chunk -> L2
-        if (!ring.pre_valid) {
-#pragma unroll 1
-          for (int look = 0; look < 3 && nstep < step_end; ++look) {
-            if (wd_has_gemv(sp, nstep, nph)) {
-              if (threadIdx.x == 0) wd_gemv_args<T>(sp, nstep, nph, pre_args);  // one thread writes the shared struct
-              __syncthreads();
-              gemv_prefetch<T>(pre_args, ring);  // plan + first weight units of the next projection -> shared memory
-              pre_tag = nstep * n_ph + nph;
-              // its LayerNorm weights -> shared memory (wb is idle until that phase stages its input)
-              const float *nw = nullptr, *nb = nullptr;
-              if (nph < 8 * p.layers) {
-                const WhisperDecLayer& w = sp.lw[nph >> 3];
-                const int sub = nph & 7;
-                if (sub == 0) { nw = w.ln1_w; nb = w.ln1_b; } else if (sub == 3) { nw = w.ln2_w; nb = w.ln2_b; }
-                else if (sub == 6) { nw = w.ln3_w; nb = w.ln3_b; }
-              } else { nw = sp.lnf_w; nb = sp.lnf_b; }
-              if (nw && wb_tag != pre_tag) { stage_norm_weights(nw, nb, sp.d, sm.wb); wb_tag = pre_tag; }
-              break;
-            }
-            if (++nph == n_ph) { nph = 0; ++nstep; }
-          }
-        }
-        if (tracing) tr[3] = globaltimer_ns();  // next phase prepared
-        grid_wait(p.sync_counter, epoch, p.sync_relaxed);
-      }
-      if (tracing) tr[5] = globaltimer_ns();
-      if (!skip) ++trace_i;
-    }
-    if (coop && !p.forced && *reinterpret_cast<volatile int*>(p.n_done) >= p.B) break;
-  }
-  gemv_drain(pre_args.K, ring);  // early exit: never leave a bulk copy in flight
+  gemv_ring_init(ring, smem_raw + lay.ring_off, p.ring_slots, s_plans);
+  const WdModel<T> model{sp, 8 * p.layers + 2};
+  // the loop reads the shared copy here (the kernel parameter costs this kernel ~20 registers; the other two prefer it)
+  dec_run<T>(sp, model, dec_views<T>(smem_raw, lay), ring, s_args, step_begin, step_end, ph_begin, ph_end, coop);
 }
 
 // =====================================================================================================================
@@ -414,45 +297,6 @@ __device__ __forceinline__ void cluster_barrier(int relaxed) {
 
 struct WdcCtx { int cid, rank, cs; };
 
-__device__ __forceinline__ bool wdc_has_gemv(const WhisperDecParams& p, int cid, int step, int ph) {
-  if (ph < 4 * p.layers) return (ph & 3) >= 2 || cid < p.heads;
-  return ph == 4 * p.layers && step >= p.n_prefix - 1;
-}
-
-// first projection of phase `ph` (4 per layer + logits); false: none (select, or a cluster without a head)
-template <typename T>
-__device__ __forceinline__ bool wdc_gemv_args(const WhisperDecParams& p, const WdcCtx& cx, int step, int ph, GemvArgs& a) {
-  const int L = p.layers, pos = step, d = p.d, B = p.B;
-  a.K = d; a.mode = EPI_STORE; a.out = p.q; a.ldo = d; a.out_h = nullptr; a.ldh = 0; a.d = d; a.kv0 = nullptr; a.kv_which = 0; a.kv_batch = 0;
-  a.suppress = nullptr; a.first_step = 0; a.logits_out = nullptr; a.logits_ld = 0; a.bias = nullptr; a.W = nullptr; a.N = 0;
-  a.pos = nullptr; a.slot = nullptr; a.kv_slot = 0; a.kv_ld = 0; a.rope = nullptr; a.hd = HD; a.q_rows = 0; a.k_rows = 0; a.q_scale = 1.f; a.kraw = nullptr; a.xsrc = nullptr; a.xsrc_ld = 0; a.kc = 0; a.plan_id = -1;
-  if (ph < 4 * L) {
-    const int layer = ph >> 2;
-    const WhisperDecLayer& w = p.lw[layer];
-    switch (ph & 3) {
-      case 0: {
-        if (cx.cid >= p.heads) return false;
-        const long long kvs = (long long)p.max_pos * d;
-        a.W = w.w_qkv; a.N = 3 * d; a.bias = w.b_qkv; a.mode = EPI_QKV; a.out = p.q; a.plan_id = 0;
-        a.kv0 = reinterpret_cast<T*>(p.self_kv) + ((long long)layer * 2) * kvs + (long long)pos * d;
-        a.kv_which = kvs; a.kv_batch = (long long)L * 2 * kvs;
-      } return true;
-      case 1:
-        if (cx.cid >= p.heads) return false;
-        a.W = w.w_cq; a.N = d; a.bias = w.b_cq; a.mode = EPI_STORE; a.out = p.q; a.plan_id = 1; return true;
-      case 2: a.W = w.w_fc1; a.N = p.ffn; a.bias = w.b_fc1; a.mode = EPI_GELU; a.out_h = p.h; a.ldh = p.ffn; a.plan_id = 3; return true;
-      default: a.W = w.w_fc2; a.N = d; a.K = p.ffn; a.bias = w.b_fc2; a.mode = EPI_RESID; a.out = p.x; a.plan_id = 4; return true;
-    }
-  }
-  const int g = step - (p.n_prefix - 1);
-  if (ph == 4 * L && g >= 0) {
-    a.W = p.embed_t; a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 5; a.suppress = p.suppress; a.first_step = (g == 0);
-    a.logits_out = p.logits_out ? p.logits_out + (long long)g * B * p.vocab : nullptr; a.logits_ld = p.vocab;
-    return true;
-  }
-  return false;
-}
-
 // the head's 64-column slice of an out-projection: partial[h][b][row] = sum_{k < 64} W[row][64 h + k] * o_h[b][k]
 __device__ __forceinline__ void wdc_out_args(const WhisperDecParams& p, const WdcCtx& cx, int layer, bool cross, GemvArgs& a) {
   const WhisperDecLayer& w = p.lw[layer];
@@ -460,133 +304,173 @@ __device__ __forceinline__ void wdc_out_args(const WhisperDecParams& p, const Wd
   a.out = (cross ? p.part_x1 : p.part_x0) + (long long)cx.cid * p.B * p.d; a.ldo = p.d; a.plan_id = 2;
 }
 
-// self / cross attention block of one layer (see the header comment).  scratch: (heads + 1) * B * d floats.
+// The cluster kernel's phases for dec_run (decode_common.cuh): the kernel's shared copy of the parameters and the cluster
+// identity.  Stamps 2 and 3 of the trace are the block's intra-phase milestones (S2S_TRACE_MODE selects which).
 template <typename T>
-__device__ __forceinline__ void wdc_block(const WhisperDecParams& p, const WdcCtx& cx, int step, int layer, bool cross,
-                                          const WdSmem<T>& sm, GemvRing& ring, GemvArgs* ready, GemvArgs* scratch /*[2]*/,
-                                          int wb_ready, unsigned long long* tr) {
-  const WhisperDecLayer& w = p.lw[layer];
-  const int d = p.d, B = p.B, H = p.heads, warp = threadIdx.x >> 5;
-  constexpr int REC = HD + PART_PAD;
-  float best_v[2] = {-INFINITY, -INFINITY};
-  int best_i[2] = {0x7fffffff, 0x7fffffff};
-  // A. input of the block
-  if (!cross) {
-    stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, w.ln1_w, w.ln1_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
-  } else {
-    stage_rows_norm_sum<T>(p.x, p.part_x0, H, (long long)B * d, w.b_o, blockIdx.x == 0 ? p.x_alt : nullptr, B, d, sm.xs, sm.xh, 1,
-                           w.ln2_w, w.ln2_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
+struct WdcModel {
+  static constexpr bool stamps_barrier = false;
+  const WhisperDecParams& p;
+  WdcCtx cx;
+  int n_phases;
+
+  __device__ __forceinline__ bool skip(int step, int ph) const { return ph == 4 * p.layers && step < p.n_prefix - 1; }
+  // false: select, or a cluster without a head
+  __device__ __forceinline__ bool has_gemv(int step, int ph) const {
+    if (ph < 4 * p.layers) return (ph & 3) >= 2 || cx.cid < p.heads;
+    return ph == 4 * p.layers && step >= p.n_prefix - 1;
   }
-  if (tr) tr[1] = globaltimer_ns();
-  if (cx.cid >= H) return;  // no head for this cluster (nothing was prefetched for it: wdc_has_gemv)
-  const int h = cx.cid;
-  // B. the head's q (k, v) rows
-  GemvArgs& a = ready ? *ready : scratch[0];
-  GemvArgs& ao = scratch[1];
-  if (threadIdx.x == 0) {  // ONE thread writes the shared argument structs; the barrier publishes them
-    if (!ready) wdc_gemv_args<T>(p, cx, step, layer * 4 + (cross ? 1 : 0), scratch[0]);
-    ao = a;
-    wdc_out_args(p, cx, layer, cross, ao);
+  // every CTA stages its input, also clusters without a head: the look-ahead stages their norm weights
+  __device__ __forceinline__ bool lookahead_target(int step, int ph) const { return !skip(step, ph) && ph != 4 * p.layers + 1; }
+  __device__ __forceinline__ void prefetch_l2(int, int) const {}
+  __device__ __forceinline__ DecNorm norm_of(int ph) const {
+    if (ph >= 4 * p.layers) return {p.lnf_w, p.lnf_b};
+    const WhisperDecLayer& w = p.lw[ph >> 2];
+    const int sub = ph & 3;
+    if (sub == 0) return {w.ln1_w, w.ln1_b};
+    if (sub == 1) return {w.ln2_w, w.ln2_b};
+    if (sub == 2) return {w.ln3_w, w.ln3_b};
+    return {nullptr, nullptr};
   }
-  __syncthreads();
-  gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-  if (tr && p.trace_mode == 0) tr[2] = globaltimer_ns();
-  // C. start streaming the head's out-projection slice
-  gemv_prefetch<T>(ao, ring);
-  // D. q (and the new k, v cache rows) of the head are visible to the whole cluster
-  cluster_barrier(p.sync_relaxed);
-  if (tr && p.trace_mode == 0) tr[3] = globaltimer_ns();
-  // E. attention: 32-key blocks over (CTA rank, warp); one record per CTA
-  float* rec_s = reinterpret_cast<float*>(sm.red);
-  {
-    const int n_keys = cross ? p.n_ctx : step + 1;
-    const int n_blocks = (n_keys + ATT_BLK - 1) / ATT_BLK;
-    const long long kvs = (long long)p.max_pos * d, head_elems = (long long)p.n_ctx * HD;
-#pragma unroll 1
-    for (int b = 0; b < B; ++b) {
-      const T* Kb; long long v_off, ld;
-      if (cross) {
-        Kb = reinterpret_cast<const T*>(p.cross_kv) + (((long long)b * p.layers + layer) * 2 * H + h) * head_elems;
-        v_off = H * head_elems; ld = HD;
-      } else {
-        Kb = reinterpret_cast<const T*>(p.self_kv) + ((long long)b * p.layers + layer) * 2 * kvs + h * HD;
-        v_off = kvs; ld = d;
+
+  // first projection of phase `ph` (4 per layer + logits; has_gemv)
+  __device__ __forceinline__ void gemv_args(int step, int ph, GemvArgs& a) const {
+    const int L = p.layers, pos = step, d = p.d, B = p.B;
+    gemv_args_reset(a, d, p.q);
+    if (ph < 4 * L) {
+      const int layer = ph >> 2;
+      const WhisperDecLayer& w = p.lw[layer];
+      switch (ph & 3) {
+        case 0: {
+          const long long kvs = (long long)p.max_pos * d;
+          a.W = w.w_qkv; a.N = 3 * d; a.bias = w.b_qkv; a.mode = EPI_QKV; a.out = p.q; a.plan_id = 0;
+          a.kv0 = reinterpret_cast<T*>(p.self_kv) + ((long long)layer * 2) * kvs + (long long)pos * d;
+          a.kv_which = kvs; a.kv_batch = (long long)L * 2 * kvs;
+        } return;
+        case 1: a.W = w.w_cq; a.N = d; a.bias = w.b_cq; a.mode = EPI_STORE; a.out = p.q; a.plan_id = 1; return;
+        case 2: a.W = w.w_fc1; a.N = p.ffn; a.bias = w.b_fc1; a.mode = EPI_GELU; a.out_h = p.h; a.ldh = p.ffn; a.plan_id = 3; return;
+        default: a.W = w.w_fc2; a.N = d; a.K = p.ffn; a.bias = w.b_fc2; a.mode = EPI_RESID; a.out = p.x; a.plan_id = 4; return;
       }
-      attend_blocks<T, HD>(p.q + b * d + h * HD, Kb, Kb + v_off, ld, ld, n_keys, cx.rank + cx.cs * warp, n_blocks,
-                           cx.cs * DEC_WARPS, rec_s + warp * REC);
-      __syncthreads();
-      if (warp == 0)
-        // always the record path (splits >= 2): with a 1-CTA cluster (a profiler that drops the cluster shape) the single
-        // record is merged below like any other, instead of attn_finish_item's splits == 1 shortcut writing a head output
-        attn_finish_item<T, HD>(rec_s, DEC_WARPS, p.part + (long long)(b * H + h) * p.s_max * REC, cx.rank, max(cx.cs, 2), nullptr,
-                                static_cast<T*>(nullptr));
-      __syncthreads();
     }
+    const int g = step - (p.n_prefix - 1);
+    a.W = p.embed_t; a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 5; a.suppress = p.suppress; a.first_step = (g == 0);
+    a.logits_out = p.logits_out ? p.logits_out + (long long)g * B * p.vocab : nullptr; a.logits_ld = p.vocab;
   }
-  // F. every CTA's record of the head is visible to the cluster
-  cluster_barrier(p.sync_relaxed);
-  if (tr && p.trace_mode == 1) tr[2] = globaltimer_ns();
-  // G. merge the CS records (redundantly in every CTA: one L2 round trip, no further hand-off) -> o_h as x operand
-  if (warp < B) attn_merge_records<T, HD>(p.part + (long long)(warp * H + h) * p.s_max * REC, cx.cs, sm.xh + warp * (HD + GV_XPAD));
-  __syncthreads();
-  if (tr && p.trace_mode == 1) tr[3] = globaltimer_ns();
-  // H. the head's slice of the out-projection -> partial residual update
-  gemv_mma<T, false>(ao, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-}
 
-template <typename T>
-__device__ __forceinline__ void wdc_phase(const WhisperDecParams& p, const WdcCtx& cx, int step, int ph, const WdSmem<T>& sm,
-                                          GemvRing& ring, GemvArgs* ready, GemvArgs* scratch /*[2]*/, int wb_ready,
-                                          unsigned long long* tr) {
-  const int L = p.layers, d = p.d, B = p.B;
-  float best_v[2] = {-INFINITY, -INFINITY};
-  int best_i[2] = {0x7fffffff, 0x7fffffff};
-  if (ph < 4 * L) {
-    const int layer = ph >> 2, sub = ph & 3;
-    if (sub < 2) { wdc_block<T>(p, cx, step, layer, sub == 1, sm, ring, ready, scratch, wb_ready, tr); return; }
+  // self / cross attention block of one layer (see the comment above).  scratch: (heads + 1) * B * d floats.
+  __device__ __forceinline__ void block(int step, int layer, bool cross, const DecViews<T>& sm, GemvRing& ring, GemvArgs* ready,
+                                        GemvArgs* scratch /*[2]*/, int wb_ready, unsigned long long* tr) const {
     const WhisperDecLayer& w = p.lw[layer];
-    if (!ready) {
-      if (threadIdx.x == 0) wdc_gemv_args<T>(p, cx, step, ph, scratch[0]);
-      __syncthreads();
+    const int d = p.d, B = p.B, H = p.heads, warp = threadIdx.x >> 5;
+    constexpr int REC = HD + PART_PAD;
+    float best_v[2] = {-INFINITY, -INFINITY};
+    int best_i[2] = {0x7fffffff, 0x7fffffff};
+    // A. input of the block
+    if (!cross) {
+      stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, w.ln1_w, w.ln1_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
+    } else {
+      stage_rows_norm_sum<T>(p.x, p.part_x0, H, (long long)B * d, w.b_o, blockIdx.x == 0 ? p.x_alt : nullptr, B, d, sm.xs, sm.xh, 1,
+                             w.ln2_w, w.ln2_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
     }
+    if (tr) tr[1] = dec_clock_ns();
+    if (cx.cid >= H) return;  // no head for this cluster (nothing was prefetched for it: has_gemv)
+    const int h = cx.cid;
+    // B. the head's q (k, v) rows
     GemvArgs& a = ready ? *ready : scratch[0];
-    if (sub == 2)
-      stage_rows_norm_sum<T>(p.x_alt, p.part_x1, p.heads, (long long)B * d, w.b_co, blockIdx.x == 0 ? p.x : nullptr, B, d, sm.xs,
-                             sm.xh, 1, w.ln3_w, w.ln3_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
-    else
-      stage_rows_copy<T>(reinterpret_cast<const T*>(p.h), B, p.ffn, sm.xh);
-    if (tr) tr[1] = globaltimer_ns();
-    gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-    return;
-  }
-  const int g = step - (p.n_prefix - 1);
-  if (ph == 4 * L) {
-    if (!ready) {
-      if (!wdc_has_gemv(p, cx.cid, step, ph)) return;
-      if (threadIdx.x == 0) wdc_gemv_args<T>(p, cx, step, ph, scratch[0]);
-      __syncthreads();
+    GemvArgs& ao = scratch[1];
+    if (threadIdx.x == 0) {  // ONE thread writes the shared argument structs; the barrier publishes them
+      if (!ready) gemv_args(step, layer * 4 + (cross ? 1 : 0), scratch[0]);
+      ao = a;
+      wdc_out_args(p, cx, layer, cross, ao);
     }
-    GemvArgs& a = ready ? *ready : scratch[0];
-    stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, p.lnf_w, p.lnf_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
+    __syncthreads();
     gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-    gemv_argmax_candidates(best_v, best_i, B, sm.sv, sm.si, p.cand_val, p.cand_idx);
-  } else {
-    wd_select<T>(p, g, step, sm.sv);
+    if (tr && p.trace_mode == 0) tr[2] = dec_clock_ns();
+    // C. start streaming the head's out-projection slice
+    gemv_prefetch<T>(ao, ring);
+    // D. q (and the new k, v cache rows) of the head are visible to the whole cluster
+    cluster_barrier(p.sync_relaxed);
+    if (tr && p.trace_mode == 0) tr[3] = dec_clock_ns();
+    // E. attention: 32-key blocks over (CTA rank, warp); one record per CTA
+    float* rec_s = reinterpret_cast<float*>(sm.red);
+    {
+      const int n_keys = cross ? p.n_ctx : step + 1;
+      const int n_blocks = (n_keys + ATT_BLK - 1) / ATT_BLK;
+      const long long kvs = (long long)p.max_pos * d, head_elems = (long long)p.n_ctx * HD;
+#pragma unroll 1
+      for (int b = 0; b < B; ++b) {
+        const T* Kb; long long v_off, ld;
+        if (cross) {
+          Kb = reinterpret_cast<const T*>(p.cross_kv) + (((long long)b * p.layers + layer) * 2 * H + h) * head_elems;
+          v_off = H * head_elems; ld = HD;
+        } else {
+          Kb = reinterpret_cast<const T*>(p.self_kv) + ((long long)b * p.layers + layer) * 2 * kvs + h * HD;
+          v_off = kvs; ld = d;
+        }
+        attend_blocks<T, HD>(p.q + b * d + h * HD, Kb, Kb + v_off, ld, ld, n_keys, cx.rank + cx.cs * warp, n_blocks,
+                             cx.cs * DEC_WARPS, rec_s + warp * REC);
+        __syncthreads();
+        if (warp == 0)
+          // always the record path (splits >= 2): with a 1-CTA cluster (a profiler that drops the cluster shape) the single
+          // record is merged below like any other, instead of attn_finish_item's splits == 1 shortcut writing a head output
+          attn_finish_item<T, HD>(rec_s, DEC_WARPS, p.part + (long long)(b * H + h) * p.s_max * REC, cx.rank, max(cx.cs, 2), nullptr,
+                                  static_cast<T*>(nullptr));
+        __syncthreads();
+      }
+    }
+    // F. every CTA's record of the head is visible to the cluster
+    cluster_barrier(p.sync_relaxed);
+    if (tr && p.trace_mode == 1) tr[2] = dec_clock_ns();
+    // G. merge the CS records (redundantly in every CTA: one L2 round trip, no further hand-off) -> o_h as x operand
+    if (warp < B) attn_merge_records<T, HD>(p.part + (long long)(warp * H + h) * p.s_max * REC, cx.cs, sm.xh + warp * (HD + GV_XPAD));
+    __syncthreads();
+    if (tr && p.trace_mode == 1) tr[3] = dec_clock_ns();
+    // H. the head's slice of the out-projection -> partial residual update
+    gemv_mma<T, false>(ao, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
   }
-}
 
-// shared-memory layout of the cluster kernel: [xh | scratch (heads + 1) * B * d fp32 | aux | ring]
-struct WdcSmem { unsigned int xs_off, aux_off, si_off, red_s_off, wb_off, redbuf_off, ring_off; };
-__host__ __device__ inline WdcSmem wdc_smem_layout(int B, int d, int kmax, int heads) {
-  WdcSmem L;
-  const unsigned int xh_bytes = (((unsigned)B * (unsigned)(kmax + GV_XPAD) * 2u) + 127u) & ~127u;
-  L.xs_off = xh_bytes;
-  L.aux_off = (L.xs_off + (unsigned)(heads + 1) * (unsigned)B * (unsigned)d * 4u + 127u) & ~127u;
-  L.si_off = L.aux_off + DEC_WARPS * DEC_MAX_B * 4;
-  L.red_s_off = L.si_off + DEC_WARPS * DEC_MAX_B * 4;
-  L.wb_off = L.red_s_off + 2 * DEC_WARPS * DEC_MAX_B * 4;
-  L.redbuf_off = (L.wb_off + 2u * (unsigned)d * 4u + 15u) & ~15u;
-  L.ring_off = (L.redbuf_off + 2u * DEC_THREADS * 16u + 127u) & ~127u;
+  __device__ __forceinline__ void phase(int step, int ph, const DecViews<T>& sm, GemvRing& ring, GemvArgs* ready,
+                                        GemvArgs* scratch /*[2]*/, int wb_ready, unsigned long long* tr) const {
+    const int L = p.layers, d = p.d, B = p.B;
+    float best_v[2] = {-INFINITY, -INFINITY};
+    int best_i[2] = {0x7fffffff, 0x7fffffff};
+    if (ph < 4 * L) {
+      const int layer = ph >> 2, sub = ph & 3;
+      if (sub < 2) { block(step, layer, sub == 1, sm, ring, ready, scratch, wb_ready, tr); return; }
+      const WhisperDecLayer& w = p.lw[layer];
+      if (!ready) {
+        if (threadIdx.x == 0) gemv_args(step, ph, scratch[0]);
+        __syncthreads();
+      }
+      GemvArgs& a = ready ? *ready : scratch[0];
+      if (sub == 2)
+        stage_rows_norm_sum<T>(p.x_alt, p.part_x1, p.heads, (long long)B * d, w.b_co, blockIdx.x == 0 ? p.x : nullptr, B, d, sm.xs,
+                               sm.xh, 1, w.ln3_w, w.ln3_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
+      else
+        stage_rows_copy<T>(reinterpret_cast<const T*>(p.h), B, p.ffn, sm.xh);
+      if (tr) tr[1] = dec_clock_ns();
+      gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
+      return;
+    }
+    if (ph == 4 * L) {
+      if (!ready) {
+        if (threadIdx.x == 0) gemv_args(step, ph, scratch[0]);
+        __syncthreads();
+      }
+      GemvArgs& a = ready ? *ready : scratch[0];
+      stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 1, p.lnf_w, p.lnf_b, 1e-5f, sm.s_red, sm.wb, wb_ready);
+      gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
+      gemv_argmax_candidates(best_v, best_i, B, sm.sv, sm.si, p.cand_val, p.cand_idx);
+    } else {
+      wd_select<T>(p, step - (p.n_prefix - 1), step, sm.sv);
+    }
+  }
+};
+
+// shared-memory layout of the cluster kernel: [xh | scratch (heads + 1) * B * d fp32 | the tail of dec_smem_layout]
+__host__ __device__ inline DecSmem wdc_smem_layout(int B, int d, int kmax, int heads) {
+  DecSmem L;
+  L.xs_off = (((unsigned)B * (unsigned)(kmax + GV_XPAD) * 2u) + 127u) & ~127u;
+  dec_smem_tail(L, (L.xs_off + (unsigned)(heads + 1) * (unsigned)B * (unsigned)d * 4u + 127u) & ~127u, 2 * d);
   return L;
 }
 
@@ -626,88 +510,11 @@ whisper_decode_cluster_kernel(const WhisperDecParams p, int step_begin, int step
   if (threadIdx.x == 0) { sp = p; sp.lw = s_layers; }
   for (int i = threadIdx.x; i < p.layers; i += DEC_THREADS) s_layers[i] = p.lw[i];
   __syncthreads();
-  const WdcSmem lay = wdc_smem_layout(p.B, p.d, max(p.d, p.ffn), p.heads);
-  WdSmem<T> sm;
-  sm.xh = reinterpret_cast<T*>(smem_raw);
-  sm.xs = reinterpret_cast<float*>(smem_raw + lay.xs_off);
-  sm.sv = reinterpret_cast<float*>(smem_raw + lay.aux_off);
-  sm.si = reinterpret_cast<int*>(smem_raw + lay.si_off);
-  sm.s_red = reinterpret_cast<float*>(smem_raw + lay.red_s_off);
-  sm.wb = reinterpret_cast<float*>(smem_raw + lay.wb_off);
-  sm.red = reinterpret_cast<float4*>(smem_raw + lay.redbuf_off);
+  const DecSmem lay = wdc_smem_layout(p.B, p.d, max(p.d, p.ffn), p.heads);
   GemvRing& ring = s_rings[threadIdx.x >> 5];
-  {
-    unsigned char* rb = smem_raw + lay.ring_off;
-    const int warp = threadIdx.x >> 5;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(rb + (size_t)DEC_WARPS * p.ring_slots * GV_SLOT_BYTES) + warp * p.ring_slots;
-    if ((threadIdx.x & 31) == 0) {   // lane 0 owns the warp's ring state in shared memory
-      ring.slots = p.ring_slots;
-      ring.base_s = smem_u32(rb + (size_t)warp * p.ring_slots * GV_SLOT_BYTES);
-      ring.bars_s = smem_u32(bars);
-      ring.slot = 0;
-      ring.parity = 0;
-      ring.plans_s = s_plans;
-      ring.pre_valid = 0; ring.pre_pj = 0; ring.pre_pu = 0; ring.pre_nvalid = 0; ring.pre_W = nullptr;
-      for (int i = 0; i < p.ring_slots; ++i) mbar_init(bars + i, 1);
-      fence_barrier_init();
-    }
-    __syncthreads();
-  }
-  unsigned int epoch = 0;
-  int trace_i = 0;
-  GemvArgs& pre_args = s_args[0];
-  if (threadIdx.x == 0) pre_args.K = p.d;
-  int pre_tag = -1, wb_tag = -1;
-  const int n_ph = 4 * p.layers + 2;
-  for (int step = step_begin; step < step_end; ++step) {
-    const int pb = coop ? 0 : ph_begin, pe = coop ? n_ph : ph_end;
-    for (int ph = pb; ph < pe; ++ph) {
-      const bool skip = (ph == 4 * p.layers) && (step < p.n_prefix - 1);
-      const bool tracing = sp.trace && trace_i < sp.trace_cap && threadIdx.x == 0 &&
-                           (blockIdx.x == 0 || blockIdx.x == gridDim.x - 1);
-      unsigned long long* tr = tracing ? sp.trace + ((blockIdx.x == 0 ? 0 : 1) * (long long)sp.trace_cap + trace_i) * 6 : nullptr;
-      if (tracing) tr[0] = globaltimer_ns();
-      if (!skip) wdc_phase<T>(sp, cx, step, ph, sm, ring, (pre_tag == step * n_ph + ph) ? &pre_args : nullptr, s_args + 1,
-                              wb_tag == step * n_ph + ph, tr);
-      if (tracing) tr[4] = globaltimer_ns();
-      if (coop && !skip) {
-        grid_arrive(p.sync_counter, epoch);
-        int nph = ph + 1, nstep = step;
-        if (nph == n_ph) { nph = 0; nstep = step + 1; }
-        if (!ring.pre_valid) {
-#pragma unroll 1
-          for (int look = 0; look < 3 && nstep < step_end; ++look) {
-            const bool skip_n = (nph == 4 * p.layers) && (nstep < p.n_prefix - 1);
-            const bool is_select = nph == 4 * p.layers + 1;
-            if (!skip_n && !is_select) {
-              // norm weights of the phase (every CTA stages its input, also clusters without a head)
-              const float *nw = nullptr, *nb = nullptr;
-              if (nph < 4 * p.layers) {
-                const WhisperDecLayer& w = sp.lw[nph >> 2];
-                const int sub = nph & 3;
-                if (sub == 0) { nw = w.ln1_w; nb = w.ln1_b; } else if (sub == 1) { nw = w.ln2_w; nb = w.ln2_b; }
-                else if (sub == 2) { nw = w.ln3_w; nb = w.ln3_b; }
-              } else { nw = sp.lnf_w; nb = sp.lnf_b; }
-              if (nw && wb_tag != nstep * n_ph + nph) { stage_norm_weights(nw, nb, sp.d, sm.wb); wb_tag = nstep * n_ph + nph; }   // once per target phase
-              if (wdc_has_gemv(sp, cx.cid, nstep, nph)) {
-                if (threadIdx.x == 0) wdc_gemv_args<T>(sp, cx, nstep, nph, pre_args);
-                __syncthreads();
-                gemv_prefetch<T>(pre_args, ring);
-                pre_tag = nstep * n_ph + nph;
-              }
-              break;
-            }
-            if (++nph == n_ph) { nph = 0; ++nstep; }
-          }
-        }
-        grid_wait(p.sync_counter, epoch, p.sync_relaxed);
-      }
-      if (tracing) tr[5] = globaltimer_ns();
-      if (!skip) ++trace_i;
-    }
-    if (coop && !p.forced && *reinterpret_cast<volatile int*>(p.n_done) >= p.B) break;
-  }
-  gemv_drain(pre_args.K, ring);
+  gemv_ring_init(ring, smem_raw + lay.ring_off, p.ring_slots, s_plans);
+  const WdcModel<T> model{sp, cx, 4 * p.layers + 2};
+  dec_run<T>(p, model, dec_views<T>(smem_raw, lay), ring, s_args, step_begin, step_end, ph_begin, ph_end, coop);
 }
 
 template <typename T>
@@ -717,13 +524,7 @@ __global__ void whisper_decode_init_kernel(const WhisperDecParams p) {
   const int tok = p.tokens[b * p.max_pos];
   const T* e = reinterpret_cast<const T*>(p.embed) + (long long)tok * p.d;
   for (int i = threadIdx.x; i < p.d; i += blockDim.x) p.x[b * p.d + i] = DT<T>::to_f(e[i]) + p.pos[i];
-  if (threadIdx.x == 0) {
-    p.done[b] = 0;
-    p.out_len[b] = 0;
-    if (b == 0) { *p.n_done = 0; *p.sync_counter = 0; }
-    for (int h = 0; h < p.heads; ++h) p.attn_cnt[b * p.heads + h] = 0u;
-  }
-  for (int i = threadIdx.x; i < p.max_new; i += blockDim.x) p.out_ids[b * p.max_new + i] = p.eos;
+  dec_init_session(p, b, p.max_new);
 }
 
 // ---- cluster kernel launcher: returns S2S_OK and sets *used = 1 when the launch configuration exists on this device
@@ -732,11 +533,10 @@ int launch_cluster_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, 
   *used = 0;
   auto kern = whisper_decode_cluster_kernel<T>;
   const int kmax = std::max(p.d, p.ffn);
-  const WdcSmem lay = wdc_smem_layout(p.B, p.d, kmax, p.heads);
-  const long long avail = 220LL * 1024 - (long long)lay.ring_off - 256;
-  int slots = (int)std::min<long long>(4, avail / ((long long)DEC_WARPS * (GV_SLOT_BYTES + 8)));
+  const DecSmem lay = wdc_smem_layout(p.B, p.d, kmax, p.heads);
+  const int slots = dec_ring_slots(lay, WD_SMEM_BUDGET);
   if (slots < 2) return S2S_OK;
-  const size_t smem = (size_t)lay.ring_off + (size_t)DEC_WARPS * slots * (GV_SLOT_BYTES + 8) + 128;
+  const size_t smem = dec_smem_bytes(lay, slots);
   S2S_CHECK_CUDA(s2s_opt_in_max_smem(kern, ctx->device, smem, nullptr));
   // every head needs its own co-resident 8-CTA cluster (queried once per configuration)
   static thread_local size_t cached_smem = 0;
@@ -766,26 +566,7 @@ int launch_cluster_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, 
   pr.cluster_size = cs;
   whisper_decode_init_kernel<T><<<p.B, 256, 0, stream>>>(pr);
   S2S_LAUNCH_CHECK();
-  const int total_steps = p.n_prefix - 1 + p.max_new;
-  const int n_ph = 4 * p.layers + 2;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(n_clusters * cs); cfg.blockDim = dim3(DEC_THREADS); cfg.dynamicSmemBytes = smem; cfg.stream = stream;
-  cudaLaunchAttribute at[2];
-  at[0].id = cudaLaunchAttributeClusterDimension; at[0].val.clusterDim.x = cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-  at[1].id = cudaLaunchAttributeCooperative; at[1].val.cooperative = 1;
-  cfg.attrs = at;
-  if (!debug_phases) {
-    cfg.numAttrs = 2;
-    S2S_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, pr, 0, total_steps, 0, n_ph, 1));
-    s2s_count_launch();
-  } else {
-    cfg.numAttrs = 1;  // one launch per phase: kernel boundaries replace the grid barrier
-    for (int s = 0; s < total_steps; ++s)
-      for (int ph = 0; ph < n_ph; ++ph) {
-        if (ph == 4 * p.layers && s < p.n_prefix - 1) continue;
-        S2S_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, pr, s, s + 1, ph, ph + 1, 0));
-      }
-  }
+  S2S_CHECK(dec_launch(kern, pr, n_clusters * cs, cs, smem, p.n_prefix - 1 + p.max_new, 4 * p.layers + 2, debug_phases, stream));
   *used = 1;
   return S2S_OK;
 }
@@ -816,25 +597,7 @@ int launch_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, cudaStre
   S2S_CHECK_CUDA(s2s_opt_in_max_smem(kern, ctx->device, smem, nullptr));
   whisper_decode_init_kernel<T><<<p.B, 256, 0, stream>>>(pr);
   S2S_LAUNCH_CHECK();
-  const int total_steps = p.n_prefix - 1 + p.max_new;
-  const int n_ph = 8 * p.layers + 2;
-  const int grid = dec_grid(ctx);
-  if (!debug_phases) {
-    int sb = 0, se = total_steps, pb = 0, pe = n_ph, coop = 1;
-    WhisperDecParams pp = pr;
-    void* args[] = {&pp, &sb, &se, &pb, &pe, &coop};
-    S2S_CHECK_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(DEC_THREADS), args, smem, stream));
-    s2s_count_launch();
-  } else {
-    // debug: one ordinary launch per phase (kernel boundaries replace the grid barrier)
-    for (int s = 0; s < total_steps; ++s)
-      for (int ph = 0; ph < n_ph; ++ph) {
-        if (ph == 8 * p.layers && s < p.n_prefix - 1) continue;
-        kern<<<grid, DEC_THREADS, smem, stream>>>(pr, s, s + 1, ph, ph + 1, 0);
-        S2S_LAUNCH_CHECK();
-      }
-  }
-  return S2S_OK;
+  return dec_launch(kern, pr, dec_grid(ctx), 0, smem, p.n_prefix - 1 + p.max_new, 8 * p.layers + 2, debug_phases, stream);
 }
 
 }  // namespace

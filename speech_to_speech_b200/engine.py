@@ -373,7 +373,8 @@ class LlamaEngine:
         return int(self.lib.s2s_llama_max_decode_batch(self.handle))
 
     def set_trace(self, trace: Optional[torch.Tensor]) -> None:
-        cap = 0 if trace is None else trace.shape[0]
+        """trace: cuda int64 [2, capacity, 6] or None (profiling aid, see include/s2s_b200.h)."""
+        cap = 0 if trace is None else trace.shape[1]
         check(self.lib.s2s_llama_set_trace(self.handle, _ptr(trace), cap), "s2s_llama_set_trace")
 
     def generate(self, prompt: Sequence[int], max_new_tokens: int, eos_id: int = -1, slot: int = 0) -> list[int]:

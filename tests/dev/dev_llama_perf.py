@@ -22,9 +22,9 @@ for it in range(3):
 t = time.perf_counter(); out = eng.generate(prompt, 128); print("generate e2e ms", (time.perf_counter() - t) * 1e3, len(out))
 
 # phase timeline (CTA 0), second token step
-tr = torch.zeros((2000, 3), dtype=torch.int64, device="cuda")
+tr = torch.zeros((2, 2000, 6), dtype=torch.int64, device="cuda")
 eng.reset(0); nxt, _ = eng.prefill(0, prompt); eng.set_trace(tr); eng.decode([0], nxt, 4); torch.cuda.synchronize(); eng.set_trace(None)
-t = tr.cpu().numpy(); nph = 5 * g.layers + 2
+t = tr[0].cpu().numpy()[:, [0, 4, 5]]; nph = 5 * g.layers + 2   # phase begin, body end, barrier exit
 names = ["qkv+rope", "attn", "o_proj", "gate_up", "down"]
 for k in range(5):
     sel = [nph + l * 5 + k for l in range(g.layers)]

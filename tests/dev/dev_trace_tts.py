@@ -14,17 +14,19 @@ for s in range(B):
 eng.decode_frames(list(range(B)), 8); torch.cuda.synchronize()
 for which, name, L in ((0, "talker", eng.cfg.layers), (1, "predictor", eng.cfg.cp_layers)):
     cap = 4096
-    tr = torch.zeros((cap, 3), dtype=torch.int64, device="cuda")
+    tr = torch.zeros((2, cap, 6), dtype=torch.int64, device="cuda")
     lib.s2s_qwen3tts_set_trace(eng.handle, which, tr.data_ptr(), cap)
     eng.decode_frames(list(range(B)), 1); torch.cuda.synchronize()
     lib.s2s_qwen3tts_set_trace(eng.handle, which, None, 0)
-    t = tr.cpu().numpy()
+    t = tr[0].cpu().numpy()[:, [0, 4, 5]]   # CTA 0: phase begin, body end, barrier exit
     t = t[t[:, 0] > 0]
     kinds = ["qkv", "attn", "o_proj", "gate_up", "down"]   # Qwen3 q/k norm runs inside the attention items
     body, wait = {}, {}
     n_ph = 5 * L + 2
+    # only phases that run are recorded: the predictor's step 0 predicts nothing and has no logits phase
+    seq = [ph for ph in range(n_ph) if not (which == 1 and ph == 5 * L)] + list(range(n_ph)) * (len(t) // n_ph + 1)
     for i, row in enumerate(t):
-        ph = i % n_ph     # the predictor's step 0 still records its (empty) logits phase: n_ph records per step for both
+        ph = seq[i]
         k = kinds[ph % 5] if ph < 5 * L else ("logits" if ph == 5 * L else "select")
         body.setdefault(k, []).append((row[1] - row[0]) / 1e3)
         wait.setdefault(k, []).append((row[2] - row[1]) / 1e3)
