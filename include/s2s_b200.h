@@ -37,6 +37,8 @@ extern "C" {
 #define S2S_F32 0
 #define S2S_F16 1
 #define S2S_BF16 2
+/* weight storage format only (s2s_llama_set_weight_format); never a bind_tensor source or a compute type */
+#define S2S_FP8_E4M3 3
 
 typedef struct s2s_ctx s2s_ctx;
 typedef struct s2s_whisper s2s_whisper;
@@ -154,6 +156,15 @@ int s2s_llama_destroy(s2s_llama* m);
 int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, const int64_t* shape,
                           int32_t ndim, int32_t dtype);
 int s2s_llama_init_random(s2s_llama* m, uint64_t seed);
+/* Storage format of the matrices the decode launch streams (q/k/v, o, gate/up, down projections of every layer and
+ * lm_head).  `format` = the model's compute_dtype (the default) or S2S_FP8_E4M3: weight-only FP8 with one power-of-two scale
+ * per weight row, quantised from the bound 16-bit tensors at finalize.  The row-major matrices the prefill GEMMs read are
+ * replaced by the dequantised values, so prefill and decode run ONE model: bit for bit the 16-bit engine bound to those
+ * dequantised weights, and a different model from the checkpoint's.  Halves the weight bytes a decode step streams and
+ * the decode copy of the weights.  Call after create and before finalize (S2S_ERR_INVALID afterwards); FP8 needs bf16
+ * compute and a single-table model (S2S_ERR_UNSUPPORTED otherwise). */
+int s2s_llama_set_weight_format(s2s_llama* m, int32_t format);
+int32_t s2s_llama_weight_format(s2s_llama* m);
 int s2s_llama_finalize(s2s_llama* m);
 /* Reset a KV-cache slot (new response).  Also empties the slot's seen-id set (repetition penalty), on the stream of the
  * slot's next prefill or decode. */

@@ -9,6 +9,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("S2S_LIB_PATH") or os.path.join(_HERE, "libs2s_b200.so")
 
 S2S_F32, S2S_F16, S2S_BF16 = 0, 1, 2
+S2S_FP8_E4M3 = 3  # weight storage only (s2s_llama_set_weight_format)
+WEIGHT_FORMAT_CODES = {"float8_e4m3": S2S_FP8_E4M3}
 DTYPE_CODES = {"float32": S2S_F32, "float16": S2S_F16, "bfloat16": S2S_BF16}
 
 # every symbol include/s2s_b200.h declares (checked by tests/test_abi.py)
@@ -20,6 +22,7 @@ EXPORTED = [
     "s2s_gemm", "s2s_attention",
     "s2s_llama_create", "s2s_llama_destroy", "s2s_llama_bind_tensor", "s2s_llama_init_random",
     "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_set_sampling", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
+    "s2s_llama_set_weight_format", "s2s_llama_weight_format",
     "s2s_tts_postproc",
     "s2s_codec_create", "s2s_codec_destroy", "s2s_codec_bind_tensor", "s2s_codec_init_random", "s2s_codec_finalize",
     "s2s_codec_decode", "s2s_codec_samples", "s2s_codec_total_upsample",
@@ -127,6 +130,9 @@ def load() -> C.CDLL:
     lib.s2s_llama_bind_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]
     lib.s2s_llama_init_random.argtypes = [vp, C.c_uint64]
     lib.s2s_llama_finalize.argtypes = [vp]
+    lib.s2s_llama_set_weight_format.argtypes = [vp, i32]
+    lib.s2s_llama_weight_format.argtypes = [vp]
+    lib.s2s_llama_weight_format.restype = i32
     lib.s2s_llama_session_reset.argtypes = [vp, i32]
     lib.s2s_llama_set_sampling.argtypes = [vp, i32, C.POINTER(Sampling)]
     lib.s2s_llama_prefill.argtypes = [vp, i32, C.POINTER(i32), i32, vp, vp, vp]

@@ -12,6 +12,8 @@
 // ring bookkeeping) lives in shared memory, not on the stack: the L1 left next to ~150-220 KB of shared memory is
 // too small for 256 private copies.
 #pragma once
+#include <type_traits>
+
 #include "common.cuh"
 
 constexpr int DEC_THREADS = 256;
@@ -118,6 +120,21 @@ constexpr int GV_UK = 256;           // k elements per ring unit (8 windows of 3
 constexpr int GV_WIN_BYTES = GV_ROWS * 32 * 2;           // one 32-element k window of a tile: 512 B, fragment-major
 constexpr int GV_SLOT_BYTES = GV_ROWS * GV_UK * 2;       // 4096
 constexpr int GV_LAT_ELEMS = 352;    // cost model: one dependent round ~ streaming 352 k-elements of a tile
+// Weight format of the streamed operand (compile-time, F8 = false unless stated): 16-bit elements of the compute type, or
+// FP8 E4M3 codes with one power-of-two fp32 scale per weight row (weight_tiles.cu).  The FP8 tiling keeps tile = 8 rows and
+// window = 32 k, one byte per element: element (row 8*tile + g, k 32*w + 8*t + e) sits at byte
+// ((tile * K/32 + w) * 32 + 4*g + t) * 8 + e, and the roundup8(N) row scales follow the codes of the matrix.  A ring unit
+// is one 4 KB bulk copy in both formats, i.e. 512 k of a tile in FP8.  The cut of a projection into warp items
+// (gemv_make_plan_ex) counts k elements, not bytes, and is therefore the same for both formats: an FP8 projection sums the
+// same products in the same order as the 16-bit one.
+template <bool F8> constexpr int gv_uk_log = F8 ? 9 : 8;                    // log2(k elements per ring unit)
+template <bool F8> constexpr int gv_uk = 1 << gv_uk_log<F8>;
+template <bool F8> constexpr int gv_elem_bytes = F8 ? 1 : 2;
+static_assert(gv_uk<false> == GV_UK && GV_ROWS * gv_uk<true> * gv_elem_bytes<true> == GV_SLOT_BYTES, "a ring unit fills a slot");
+// the row scales of an FP8 matrix [N, K] (whole rows: K = row length)
+__device__ __forceinline__ const float* gemv_f8_scales(const void* W, int N, int K) {
+  return reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(W) + (size_t)((N + GV_ROWS - 1) & ~(GV_ROWS - 1)) * K);
+}
 
 // ---- dynamic shared-memory layout shared by the decode kernels (host computes the same numbers) ----------
 //   [ xh : B x (kmax + GV_XPAD) 16-bit | the fp32 copy used for norm statistics aliases its tail ]
@@ -404,7 +421,7 @@ static __device__ __noinline__ void stage_rows_copy(const T* x, int B, int K, T*
 enum GemvEpi { EPI_STORE = 0, EPI_GELU = 1, EPI_RESID = 2, EPI_QKV = 3, EPI_LOGITS = 4,
                EPI_QKV_ROPE = 5 /* row pairs */, EPI_SWIGLU = 6 /* row pairs */ };
 struct GemvArgs {
-  const void* W; int N, K;     // W: TILED weights (see above), N rows (storage padded to a multiple of 8), K % 32 == 0
+  const void* W; int N, K;     // W: TILED weights (see above; FP8: codes + row scales), N rows (storage padded to a multiple of 8), K % 32 == 0
   const float* bias;           // [N] or null
   int mode;
   float* out; int ldo;         // STORE / RESID (in-place residual stream) / QKV (q rows): fp32
@@ -568,6 +585,29 @@ __device__ __forceinline__ uint4 lds16(uint32_t addr) {
   asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr));
   return r;
 }
+__device__ __forceinline__ uint2 lds8(uint32_t addr) {
+  uint2 r;
+  asm volatile("ld.shared.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "r"(addr));
+  return r;
+}
+// two E4M3 codes -> a bf16 pair (low code in the low half).  Exact: E4M3 is a subset of f16 and of bf16 (3 mantissa bits,
+// exponents -9..8), so neither conversion rounds.  4 instructions per pair (F2FP unpack, 2 x HADD2.F32, F2FP pack).
+__device__ __forceinline__ uint32_t e4m3x2_to_bf16x2(uint32_t codes /* low 16 bits */) {
+  uint32_t h;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"((unsigned short)codes));
+  const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+  return DT<__nv_bfloat16>::pack2(f.x, f.y);
+}
+// the B fragments of one k window: this lane's 8 weights of row g (16-bit: one 16-byte load; FP8: 8 bytes, widened)
+template <bool F8>
+__device__ __forceinline__ uint4 gemv_load_window(uint32_t addr) {
+  if constexpr (F8) {
+    const uint2 q = lds8(addr);
+    return make_uint4(e4m3x2_to_bf16x2(q.x), e4m3x2_to_bf16x2(q.x >> 16), e4m3x2_to_bf16x2(q.y), e4m3x2_to_bf16x2(q.y >> 16));
+  } else {
+    return lds16(addr);
+  }
+}
 __device__ __forceinline__ void mbar_wait_s(uint32_t bar, uint32_t parity) {
   uint32_t ok, spins = 0;
   do {
@@ -639,31 +679,33 @@ __host__ __device__ __forceinline__ bool gemv_item(const GemvPlan& pl, int K, in
 }
 
 // producer side of unit u of item j (whole warp calls; lane 0 issues one contiguous bulk copy)
-template <typename T>
+template <typename T, bool F8 = false>
 __device__ __forceinline__ void gemv_issue_unit(const T* __restrict__ Wt, int K, const GemvPlan& pl, int j, int u,
                                                 uint32_t dst, uint32_t bar) {
+  constexpr int UK = gv_uk<F8>;
   int tile, k0, klen;
   gemv_item(pl, K, j, threadIdx.x >> 5, tile, k0, klen);
-  const int kb = k0 + u * GV_UK;
-  const int len = min(GV_UK, k0 + klen - kb);
+  const int kb = k0 + u * UK;
+  const int len = min(UK, k0 + klen - kb);
   if ((threadIdx.x & 31) == 0) {
-    const uint32_t bytes = (uint32_t)(GV_ROWS * len * 2);
+    const uint32_t bytes = (uint32_t)(GV_ROWS * len * gv_elem_bytes<F8>);
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // earlier generic-proxy reads of the slot are done
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-    bulk_g2s(dst, Wt + ((long long)gemv_global_tile(pl, tile) * pl.k_full + pl.k_off + kb) * GV_ROWS, bytes, bar);
+    const long long elem = ((long long)gemv_global_tile(pl, tile) * pl.k_full + pl.k_off + kb) * GV_ROWS;
+    bulk_g2s(dst, reinterpret_cast<const unsigned char*>(Wt) + elem * gv_elem_bytes<F8>, bytes, bar);
   }
 }
 
+template <bool F8 = false>
 __host__ __device__ __forceinline__ int gemv_units_of(const GemvPlan& pl, int K, int j) {
-  return ((j < pl.main_rounds ? K : pl.slice) + GV_UK - 1) >> 8;
+  return ((j < pl.main_rounds ? K : pl.slice) + gv_uk<F8> - 1) >> gv_uk_log<F8>;
 }
 
 // Plan the gemv and issue its first `slots` units into the (empty) ring.  Called between grid_arrive and
 // grid_wait of the phase BEFORE the one that consumes them: the weight stream of the next projection is already
 // landing in shared memory while the chip synchronises.
-template <typename T>
+template <typename T, bool F8 = false>
 __device__ __forceinline__ void gemv_prefetch(const GemvArgs& a, GemvRing& ring) {
-  static_assert(GV_UK == 256, "gemv_units_of shifts by 8");
   // the ring state is ONE copy per warp in shared memory: lane 0 writes it, __syncwarp publishes it to the other lanes
   // (every lane writing the same values is the same hardware behaviour but a data race on paper -- racecheck flags it)
   const int lane0 = (threadIdx.x & 31) == 0;
@@ -682,8 +724,8 @@ __device__ __forceinline__ void gemv_prefetch(const GemvArgs& a, GemvRing& ring)
   unsigned int pslot = ring.slot;
 #pragma unroll 1
   for (int n = 0; n < ring.slots && pj < nv; ++n) {
-    gemv_issue_unit<T>(reinterpret_cast<const T*>(a.W), a.K, pl, pj, pu, ring.base_s + pslot * GV_SLOT_BYTES, ring.bars_s + pslot * 8);
-    if (++pu == gemv_units_of(pl, a.K, pj)) { pu = 0; ++pj; }
+    gemv_issue_unit<T, F8>(reinterpret_cast<const T*>(a.W), a.K, pl, pj, pu, ring.base_s + pslot * GV_SLOT_BYTES, ring.bars_s + pslot * 8);
+    if (++pu == gemv_units_of<F8>(pl, a.K, pj)) { pu = 0; ++pj; }
     if (++pslot == (unsigned)ring.slots) pslot = 0;
   }
   __syncwarp();
@@ -692,11 +734,12 @@ __device__ __forceinline__ void gemv_prefetch(const GemvArgs& a, GemvRing& ring)
 }
 
 // Wait for prefetched units that will never be consumed (early exit) so no bulk copy is in flight at CTA exit.
+template <bool F8 = false>
 __device__ __forceinline__ void gemv_drain(int K, GemvRing& ring) {
   if (!ring.pre_valid) return;
   const GemvPlan& pl = ring.plan;
   int total = 0;
-  for (int j = 0; j < ring.pre_nvalid && total < ring.slots; ++j) total += gemv_units_of(pl, K, j);
+  for (int j = 0; j < ring.pre_nvalid && total < ring.slots; ++j) total += gemv_units_of<F8>(pl, K, j);
   const int n_units = min(ring.slots, total);
   unsigned int cslot = ring.slot, cpar = ring.parity;
   for (int u = 0; u < n_units; ++u) {
@@ -710,14 +753,18 @@ __device__ __forceinline__ void gemv_drain(int K, GemvRing& ring) {
 
 // best_v / best_i: running argmax of this lane for sessions g and g + 8 (EPI_LOGITS).
 // red_s: 2 * DEC_THREADS float4 (tail-round partial fragments, double-buffered by round parity).
-template <typename T, bool LLAMA>
+// F8: W holds E4M3 codes and row scales (T must be bf16, which represents every scaled weight exactly); the row pair's
+// scales multiply the merged accumulator before the bias and the epilogue.
+template <typename T, bool LLAMA, bool F8 = false>
 __device__ __noinline__ void gemv_mma(const GemvArgs& a, uint32_t xh_s, int B, float (&best_v)[2], int (&best_i)[2],
                                       GemvRing& ring, float4* red_s) {
+  static_assert(!F8 || std::is_same<T, __nv_bfloat16>::value, "FP8 weights are widened to bf16");
+  constexpr int UK = gv_uk<F8>, UK_LOG = gv_uk_log<F8>, WIN_STEP = GV_ROWS * gv_elem_bytes<F8>;   // bytes per k of a tile
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
   const T* __restrict__ W = reinterpret_cast<const T*>(a.W);
   const int N = a.N, K = a.K, mode = a.mode;
   if (ring.pre_valid && ring.pre_W != a.W) __trap();  // prefetch bookkeeping bug: the ring holds another matrix
-  if (!ring.pre_valid) gemv_prefetch<T>(a, ring);
+  if (!ring.pre_valid) gemv_prefetch<T, F8>(a, ring);
   const GemvPlan pl = ring.plan;
   int pj = ring.pre_pj, pu = ring.pre_pu;  // producer cursor (uniform over the warp)
   const int n_valid = ring.pre_nvalid;
@@ -730,7 +777,8 @@ __device__ __noinline__ void gemv_mma(const GemvArgs& a, uint32_t xh_s, int B, f
   const uint32_t xrow_lo = xh_s + (uint32_t)(g * (K + GV_XPAD) + t * 8) * 2;
   const uint32_t xrow_hi = xrow_lo + (uint32_t)(8 * (K + GV_XPAD)) * 2;
   const bool lo = g < B, hi = g + 8 < B;
-  const uint32_t wlane = (uint32_t)lane * 16;
+  const uint32_t wlane = (uint32_t)lane * (8 * gv_elem_bytes<F8>);
+  const float* wscale = F8 ? gemv_f8_scales(a.W, N, K) : nullptr;
 #pragma unroll 1
   for (int j = 0; j < n_items; ++j) {
     int tile, k0, klen;
@@ -740,9 +788,10 @@ __device__ __noinline__ void gemv_mma(const GemvArgs& a, uint32_t xh_s, int B, f
     const int row0 = gemv_global_tile(pl, tile) * GV_ROWS + 2 * t;  // this lane's row pair
     const bool rows_ok = owner && row0 < N;
     // epilogue operands first: their round trip overlaps the weight stream
-    float bias0 = 0.f, bias1 = 0.f, rl0 = 0.f, rl1 = 0.f, rh0 = 0.f, rh1 = 0.f;
+    float bias0 = 0.f, bias1 = 0.f, rl0 = 0.f, rl1 = 0.f, rh0 = 0.f, rh1 = 0.f, ws0 = 1.f, ws1 = 1.f;
     int sup0 = 0, sup1 = 0;
     if (rows_ok) {
+      if constexpr (F8) { const float2 ss = __ldg(reinterpret_cast<const float2*>(wscale + row0)); ws0 = ss.x; ws1 = ss.y; }
       if (a.bias) { const float2 bb = __ldg(reinterpret_cast<const float2*>(a.bias + row0)); bias0 = bb.x; bias1 = bb.y; }
       if (mode == EPI_RESID) {
         if (lo) { const float2 r = __ldcg(reinterpret_cast<const float2*>(a.out + (long long)g * a.ldo + row0)); rl0 = r.x; rl1 = r.y; }
@@ -754,16 +803,16 @@ __device__ __noinline__ void gemv_mma(const GemvArgs& a, uint32_t xh_s, int B, f
     }
     float c[4] = {0.f, 0.f, 0.f, 0.f}, e[4] = {0.f, 0.f, 0.f, 0.f};  // two independent accumulator fragments
     if (valid) {
-      const int upi = (klen + GV_UK - 1) >> 8;
+      const int upi = (klen + UK - 1) >> UK_LOG;
 #pragma unroll 1
       for (int u = 0; u < upi; ++u) {
         mbar_wait_s(ring.bars_s + cslot * 8, cpar);
         const uint32_t wsrc = ring.base_s + cslot * GV_SLOT_BYTES + wlane;
-        const int len = min(GV_UK, klen - u * GV_UK);
-        const uint32_t xk = (uint32_t)(k0 + u * GV_UK) * 2;
+        const int len = min(UK, klen - u * UK);
+        const uint32_t xk = (uint32_t)(k0 + u * UK) * 2;
 #pragma unroll 4
         for (int kk = 0; kk < len; kk += 32) {
-          const uint4 w = lds16(wsrc + kk * (GV_WIN_BYTES / 32));
+          const uint4 w = gemv_load_window<F8>(wsrc + kk * WIN_STEP);
           uint4 xl = make_uint4(0u, 0u, 0u, 0u), xu = make_uint4(0u, 0u, 0u, 0u);
           if (lo) xl = lds16(xrow_lo + xk + kk * 2);
           if (hi) xu = lds16(xrow_hi + xk + kk * 2);
@@ -772,8 +821,8 @@ __device__ __noinline__ void gemv_mma(const GemvArgs& a, uint32_t xh_s, int B, f
         }
         __syncwarp();
         if (pj < n_valid) {  // refill the slot just drained
-          gemv_issue_unit<T>(W, K, pl, pj, pu, ring.base_s + cslot * GV_SLOT_BYTES, ring.bars_s + cslot * 8);
-          if (++pu == gemv_units_of(pl, K, pj)) { pu = 0; ++pj; }
+          gemv_issue_unit<T, F8>(W, K, pl, pj, pu, ring.base_s + cslot * GV_SLOT_BYTES, ring.bars_s + cslot * 8);
+          if (++pu == gemv_units_of<F8>(pl, K, pj)) { pu = 0; ++pj; }
         }
         if (++cslot == (unsigned)ring.slots) { cslot = 0; cpar ^= 1u; }
       }
@@ -792,6 +841,7 @@ __device__ __noinline__ void gemv_mma(const GemvArgs& a, uint32_t xh_s, int B, f
         }
       }
     }
+    if constexpr (F8) { c[0] *= ws0; c[1] *= ws1; c[2] *= ws0; c[3] *= ws1; }
     if (rows_ok) {
       if (lo) gemv_pair_epilogue<T, LLAMA>(a, mode, row0, g, c[0] + bias0, c[1] + bias1, rl0, rl1, sup0, sup1, best_v[0], best_i[0]);
       if (hi) gemv_pair_epilogue<T, LLAMA>(a, mode, row0, g + 8, c[2] + bias0, c[3] + bias1, rh0, rh1, sup0, sup1, best_v[1], best_i[1]);
@@ -820,9 +870,11 @@ __host__ __device__ inline bool gemv_chunk_ok(int N, int K, int kc, int grid) {
   return (last % (32 << pl.ks_log)) == 0;                   // the short last chunk still splits into whole k-windows
 }
 
-template <typename T, bool LLAMA>
+template <typename T, bool LLAMA, bool F8 = false>
 __device__ __noinline__ void gemv_mma_chunked(const GemvArgs& a, T* xh, int B, float (&best_v)[2], int (&best_i)[2], GemvRing& ring,
                                               float4* red_s) {
+  static_assert(!F8 || std::is_same<T, __nv_bfloat16>::value, "FP8 weights are widened to bf16");
+  constexpr int UK = gv_uk<F8>, UK_LOG = gv_uk_log<F8>, WIN_STEP = GV_ROWS * gv_elem_bytes<F8>;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, g = lane >> 2, t = lane & 3;
   const T* __restrict__ W = reinterpret_cast<const T*>(a.W);
   const T* __restrict__ X = reinterpret_cast<const T*>(a.xsrc);
@@ -838,9 +890,10 @@ __device__ __noinline__ void gemv_mma_chunked(const GemvArgs& a, T* xh, int B, f
   const bool owner = valid && sl == 0;
   const int row0 = tile * GV_ROWS + 2 * t;
   const bool rows_ok = owner && row0 < N;
-  float bias0 = 0.f, bias1 = 0.f, rl0 = 0.f, rl1 = 0.f, rh0 = 0.f, rh1 = 0.f;
+  float bias0 = 0.f, bias1 = 0.f, rl0 = 0.f, rl1 = 0.f, rh0 = 0.f, rh1 = 0.f, ws0 = 1.f, ws1 = 1.f;
   const bool lo = g < B, hi = g + 8 < B;
   if (rows_ok) {
+    if constexpr (F8) { const float2 ss = __ldg(reinterpret_cast<const float2*>(gemv_f8_scales(a.W, N, K) + row0)); ws0 = ss.x; ws1 = ss.y; }
     if (a.bias) { const float2 bb = __ldg(reinterpret_cast<const float2*>(a.bias + row0)); bias0 = bb.x; bias1 = bb.y; }
     if (mode == EPI_RESID) {
       if (lo) { const float2 r = __ldcg(reinterpret_cast<const float2*>(a.out + (long long)g * a.ldo + row0)); rl0 = r.x; rl1 = r.y; }
@@ -854,15 +907,15 @@ __device__ __noinline__ void gemv_mma_chunked(const GemvArgs& a, T* xh, int B, f
   unsigned int pslot = slot_in;
   auto issue_next = [&](uint32_t dst, uint32_t bar) {
     const int slice = slice_of(pc);
-    const int kb = pc * KC + sl * slice + pu * GV_UK;
-    const int len = min(GV_UK, slice - pu * GV_UK);
+    const int kb = pc * KC + sl * slice + pu * UK;
+    const int len = min(UK, slice - pu * UK);
     if (lane == 0) {
-      const uint32_t bytes = (uint32_t)(GV_ROWS * len * 2);
+      const uint32_t bytes = (uint32_t)(GV_ROWS * len * gv_elem_bytes<F8>);
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
       asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-      bulk_g2s(dst, W + ((long long)tile * K + kb) * GV_ROWS, bytes, bar);
+      bulk_g2s(dst, reinterpret_cast<const unsigned char*>(W) + ((long long)tile * K + kb) * (GV_ROWS * gv_elem_bytes<F8>), bytes, bar);
     }
-    if (++pu * GV_UK >= slice) { pu = 0; ++pc; }
+    if (++pu * UK >= slice) { pu = 0; ++pc; }
   };
   if (valid)
     for (int n = 0; n < ring.slots && pc < n_chunks; ++n) {
@@ -874,7 +927,7 @@ __device__ __noinline__ void gemv_mma_chunked(const GemvArgs& a, T* xh, int B, f
   const uint32_t row_bytes = (uint32_t)(KC + GV_XPAD) * 2;
   const uint32_t xrow_lo = xh_s + (uint32_t)g * row_bytes + (uint32_t)t * 16;
   const uint32_t xrow_hi = xrow_lo + 8u * row_bytes;
-  const uint32_t wlane = (uint32_t)lane * 16;
+  const uint32_t wlane = (uint32_t)lane * (8 * gv_elem_bytes<F8>);
   float c[4] = {0.f, 0.f, 0.f, 0.f}, e[4] = {0.f, 0.f, 0.f, 0.f};
 #pragma unroll 1
   for (int ch = 0; ch < n_chunks; ++ch) {
@@ -893,16 +946,16 @@ __device__ __noinline__ void gemv_mma_chunked(const GemvArgs& a, T* xh, int B, f
       __syncthreads();
     }
     if (valid) {
-      const int slice = kcc >> pl.ks_log, k0 = sl * slice, upi = (slice + GV_UK - 1) >> 8;
+      const int slice = kcc >> pl.ks_log, k0 = sl * slice, upi = (slice + UK - 1) >> UK_LOG;
 #pragma unroll 1
       for (int u = 0; u < upi; ++u) {
         mbar_wait_s(ring.bars_s + cslot * 8, cpar);
         const uint32_t wsrc = ring.base_s + cslot * GV_SLOT_BYTES + wlane;
-        const int len = min(GV_UK, slice - u * GV_UK);
-        const uint32_t xk = (uint32_t)(k0 + u * GV_UK) * 2;
+        const int len = min(UK, slice - u * UK);
+        const uint32_t xk = (uint32_t)(k0 + u * UK) * 2;
 #pragma unroll 4
         for (int kk = 0; kk < len; kk += 32) {
-          const uint4 w = lds16(wsrc + kk * (GV_WIN_BYTES / 32));
+          const uint4 w = gemv_load_window<F8>(wsrc + kk * WIN_STEP);
           uint4 xl = make_uint4(0u, 0u, 0u, 0u), xu = make_uint4(0u, 0u, 0u, 0u);
           if (lo) xl = lds16(xrow_lo + xk + kk * 2);
           if (hi) xu = lds16(xrow_hi + xk + kk * 2);
@@ -927,6 +980,7 @@ __device__ __noinline__ void gemv_mma_chunked(const GemvArgs& a, T* xh, int B, f
         c[0] += o.x; c[1] += o.y; c[2] += o.z; c[3] += o.w;
       }
   }
+  if constexpr (F8) { c[0] *= ws0; c[1] *= ws1; c[2] *= ws0; c[3] *= ws1; }
   if (rows_ok) {
     if (lo) gemv_pair_epilogue<T, LLAMA>(a, mode, row0, g, c[0] + bias0, c[1] + bias1, rl0, rl1, 0, 0, best_v[0], best_i[0]);
     if (hi) gemv_pair_epilogue<T, LLAMA>(a, mode, row0, g + 8, c[2] + bias0, c[3] + bias1, rh0, rh1, 0, 0, best_v[1], best_i[1]);
@@ -1260,6 +1314,7 @@ struct DecNorm { const float *w, *b; };   // norm weights (and LayerNorm bias) o
 //   prefetch_l2(step, ph)         L2 warm-up for the next phase (may be empty)
 //   phase(step, ph, sm, ring, ready, scratch, wb_ready, tr)  the phase body; ready: its prepared arguments or null
 //   stamps_barrier                the loop records trace stamps 2 and 3 (else the phase body may use them)
+//   f8_weights                    the projections stream FP8 weights (the format of the look-ahead's weight units)
 // Between a phase's grid_arrive and grid_wait the CTA prepares the next target phase up to 3 phases ahead, when the ring
 // holds nothing yet: its arguments and first weight units (not for a K-chunked projection, which starts its own stream) and
 // its norm weights (once per target phase).  Argument structs and ring state live in shared memory, written by one thread.
@@ -1301,7 +1356,7 @@ __device__ __forceinline__ void dec_run(const P& p, const Model& m, const DecVie
               if (m.has_gemv(nstep, nph)) {
                 if (threadIdx.x == 0) m.gemv_args(nstep, nph, pre_args);  // one thread writes the shared struct
                 __syncthreads();
-                if (pre_args.kc == 0) gemv_prefetch<T>(pre_args, ring);   // plan + first weight units -> shared memory
+                if (pre_args.kc == 0) gemv_prefetch<T, Model::f8_weights>(pre_args, ring);   // plan + first weight units -> shared memory
                 pre_tag = ntag;
               }
               const DecNorm nw = m.norm_of(nph);   // wb is idle until that phase stages its input
@@ -1319,7 +1374,7 @@ __device__ __forceinline__ void dec_run(const P& p, const Model& m, const DecVie
     }
     if (coop && !p.forced && *reinterpret_cast<volatile int*>(p.n_done) >= p.B) break;
   }
-  gemv_drain(pre_args.K, ring);  // early exit: never leave a bulk copy in flight
+  gemv_drain<Model::f8_weights>(pre_args.K, ring);  // early exit: never leave a bulk copy in flight
 }
 
 // init kernels, one CTA per session b: its bookkeeping (done, out_len, attention split counters; CTA 0 also the finished

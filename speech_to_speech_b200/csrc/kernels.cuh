@@ -30,3 +30,7 @@ int fill_random_launch(void* dst, long long n, int dtype, float scale, float off
 // row-major 16-bit [N, K] -> fragment-major tiled layout streamed by the decode kernels (see decode_common.cuh)
 size_t tiled_weight_elems(int N, int K);
 int tile_weights_launch(const void* W, int N, int K, void* Wt, cudaStream_t stream);
+// FP8 E4M3 weight-only quantisation with a power-of-two scale per row: W (row-major bf16 [N, K]) -> Wq = tiled E4M3 codes
+// followed by roundup8(N) fp32 row scales (tiled_fp8_weight_bytes), and W is overwritten with the dequantised values
+size_t tiled_fp8_weight_bytes(int N, int K);
+int quantize_tile_weights_fp8_launch(void* W, int N, int K, void* Wq, cudaStream_t stream);

@@ -284,7 +284,7 @@ GemmProblem lgemm(const void* a, int64_t lda, const void* w, int64_t ldw, int64_
 }  // namespace
 
 int llama_max_decode_batch_of(const s2s_llama* m) {
-  return std::min(MAX_DEC_B, llama_decode_max_batch(m->ctx->device, m->cfg.compute_dtype, m->cfg.d_model, m->cfg.ffn,
+  return std::min(MAX_DEC_B, llama_decode_max_batch(m->ctx->device, m->cfg.compute_dtype, m->weight_format, m->cfg.d_model, m->cfg.ffn,
                                                     m->cfg.heads * m->cfg.head_dim, dec_grid(m->ctx)));
 }
 
@@ -504,6 +504,7 @@ int s2s_llama_create(s2s_ctx* ctx, const s2s_llama_config* cfg, s2s_llama** out)
   s2s_llama* m = new s2s_llama();
   m->ctx = ctx;
   m->cfg = *cfg;
+  m->weight_format = cfg->compute_dtype;
   int r = build(m);
   if (r != S2S_OK) { s2s_llama_destroy(m); return r; }
   const char* dbg = getenv("S2S_DEBUG_PHASES");
@@ -587,6 +588,22 @@ int s2s_llama_init_random(s2s_llama* m, uint64_t seed) {
   return S2S_OK;
 }
 
+int s2s_llama_set_weight_format(s2s_llama* m, int32_t format) {
+  S2S_REQUIRE(m, "llama set_weight_format: null model");
+  S2S_REQUIRE(!m->finalized, "llama set_weight_format: the weight format is fixed once the model is finalized");
+  if (format != m->cfg.compute_dtype) {
+    if (format != S2S_FP8_E4M3 || m->cfg.compute_dtype != S2S_BF16 || m->n_tables != 1) {
+      // the dequantised weights are exact in bf16, not in f16; multi-table models (TTS code predictor) stay 16-bit
+      s2s_set_error("llama set_weight_format: format %d needs a single-table model with bf16 compute, or must equal compute_dtype", format);
+      return S2S_ERR_UNSUPPORTED;
+    }
+  }
+  m->weight_format = format;
+  return S2S_OK;
+}
+
+int32_t s2s_llama_weight_format(s2s_llama* m) { return m ? m->weight_format : S2S_ERR_INVALID; }
+
 int s2s_llama_finalize(s2s_llama* m) {
   S2S_REQUIRE(m, "llama finalize: null model");
   if (m->n_tables == 1 && !m->lm_head_bound && m->slots["model.embed_tokens.weight"].bound) {
@@ -599,8 +616,15 @@ int s2s_llama_finalize(s2s_llama* m) {
       s2s_set_error("llama finalize: tensor '%s' was never bound", kv.first.c_str());
       return S2S_ERR_INVALID;
     }
-  // decode-side weight layout: fragment-major tiles (weight_tiles.cu), built once per (re)load
+  // decode-side weight layout: fragment-major tiles (weight_tiles.cu), built once per (re)load.  FP8: the tiles hold E4M3
+  // codes + row scales and the row-major matrices become the dequantised values, so prefill and decode share one model.
   {
+    const bool f8 = m->weight_format == S2S_FP8_E4M3;
+    auto tbytes = [f8](int N, int K) { return f8 ? tiled_fp8_weight_bytes(N, K) : tiled_weight_elems(N, K) * 2; };
+    auto tile = [f8](const void* W, int N, int K, const void* Wt) {
+      return f8 ? quantize_tile_weights_fp8_launch(const_cast<void*>(W), N, K, const_cast<void*>(Wt), 0)
+                : tile_weights_launch(W, N, K, const_cast<void*>(Wt), 0);
+    };
     const auto& c = m->cfg;
     const int d = c.d_model, qd = c.heads * c.head_dim, kvd = c.kv_heads * c.head_dim, f = c.ffn;
     S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
@@ -609,27 +633,27 @@ int s2s_llama_finalize(s2s_llama* m) {
       for (int i = 0; i < c.layers; ++i) {
         LlamaDecLayer& T = m->tiled_h[i];
         void *a, *b, *g, *dn;
-        S2S_CHECK(lalloc(m, &a, tiled_weight_elems(qd + 2 * kvd, d) * 2));
-        S2S_CHECK(lalloc(m, &b, tiled_weight_elems(d, qd) * 2));
-        S2S_CHECK(lalloc(m, &g, tiled_weight_elems(2 * f, d) * 2));
-        S2S_CHECK(lalloc(m, &dn, tiled_weight_elems(d, f) * 2));
+        S2S_CHECK(lalloc(m, &a, tbytes(qd + 2 * kvd, d)));
+        S2S_CHECK(lalloc(m, &b, tbytes(d, qd)));
+        S2S_CHECK(lalloc(m, &g, tbytes(2 * f, d)));
+        S2S_CHECK(lalloc(m, &dn, tbytes(d, f)));
         T.w_qkv = a; T.w_o = b; T.w_gu = g; T.w_down = dn;
       }
       m->head_t_table_elems = tiled_weight_elems(c.vocab, d);
-      S2S_CHECK(lalloc(m, &m->lm_head_t, m->n_tables * m->head_t_table_elems * 2));
+      S2S_CHECK(lalloc(m, &m->lm_head_t, f8 ? tbytes(c.vocab, d) : m->n_tables * m->head_t_table_elems * 2));
       S2S_CHECK_CUDA(cudaMemcpy(m->layers_d, m->tiled_h.data(), sizeof(LlamaDecLayer) * c.layers, cudaMemcpyHostToDevice));
     }
     for (int i = 0; i < c.layers; ++i) {
       const LlamaDecLayer& R = m->layers_h[i];
       const LlamaDecLayer& T = m->tiled_h[i];
-      S2S_CHECK(tile_weights_launch(R.w_qkv, qd + 2 * kvd, d, const_cast<void*>(T.w_qkv), 0));
-      S2S_CHECK(tile_weights_launch(R.w_o, d, qd, const_cast<void*>(T.w_o), 0));
-      S2S_CHECK(tile_weights_launch(R.w_gu, 2 * f, d, const_cast<void*>(T.w_gu), 0));
-      S2S_CHECK(tile_weights_launch(R.w_down, d, f, const_cast<void*>(T.w_down), 0));
+      S2S_CHECK(tile(R.w_qkv, qd + 2 * kvd, d, T.w_qkv));
+      S2S_CHECK(tile(R.w_o, d, qd, T.w_o));
+      S2S_CHECK(tile(R.w_gu, 2 * f, d, T.w_gu));
+      S2S_CHECK(tile(R.w_down, d, f, T.w_down));
     }
-    for (int t = 0; t < m->n_tables; ++t)
-      S2S_CHECK(tile_weights_launch(reinterpret_cast<char*>(m->lm_head) + (size_t)t * m->head_table_elems * 2, c.vocab, d,
-                                    reinterpret_cast<char*>(m->lm_head_t) + (size_t)t * m->head_t_table_elems * 2, 0));
+    for (int t = 0; t < m->n_tables; ++t)   // FP8: n_tables == 1
+      S2S_CHECK(tile(reinterpret_cast<char*>(m->lm_head) + (size_t)t * m->head_table_elems * 2, c.vocab, d,
+                     reinterpret_cast<char*>(m->lm_head_t) + (size_t)t * m->head_t_table_elems * 2));
     S2S_CHECK_CUDA(cudaDeviceSynchronize());
   }
   m->finalized = true;
@@ -731,7 +755,7 @@ int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int3
   p.B = B; p.slot = m->slot_d; p.pos = m->pos_d; p.max_len = max_len;
   p.first_ids = first_ids_d; p.n_steps = n_steps; p.eos = eos_id; p.out_ids = ids_out_d; p.out_len = len_out_d;
   p.forced = forced_d; p.logits_out = logits_out_d; p.samp = any_samp ? m->samp_d : nullptr;
-  S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->debug_phases, st));
+  S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->weight_format, m->debug_phases, st));
   for (int b = 0; b < B; ++b) m->len[slots_h[b]] += n_steps;
   return S2S_OK;
 }

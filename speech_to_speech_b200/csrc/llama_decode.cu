@@ -15,6 +15,8 @@
 // layer (a sixth phase would add one grid barrier per layer and step to the TTS frame loop).
 // Projections are swap-AB tensor-core GEMVs (sessions on m) fed from per-warp bulk-copy rings of fragment-major weights
 // (decode_common.cuh, weight_tiles.cu); HBM-bound: 15.0 GB / token for Llama-3-8B (SURVEY.md Appendix A).
+// F8 instantiation: the same kernel over FP8 E4M3 weights with power-of-two row scales (7.5 GB / token), bf16 compute only.
+// Every projection of the launch, lm_head included, is FP8, so the kernel still holds one GEMV routine.
 #include <algorithm>
 
 #include "llama_decode.cuh"
@@ -170,9 +172,10 @@ __device__ __noinline__ void ld_select(const LlamaDecParams& p, int step, float*
 }
 
 // The kernel's phases for dec_run (decode_common.cuh).  Holds a reference to the kernel's shared copy of the parameters.
-template <typename T>
+template <typename T, bool F8>
 struct LdModel {
   static constexpr bool stamps_barrier = true;
+  static constexpr bool f8_weights = F8;
   const LlamaDecParams& p;
   int n_phases;
 
@@ -246,17 +249,17 @@ struct LdModel {
         case 2: stage_rows_copy<T>(reinterpret_cast<const T*>(p.attn16), B, p.heads * p.hd, sm.xh); break;
         case 3: stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 2, w.norm2, nullptr, p.eps, sm.s_red, sm.wb, wb_ready, p.norm_rg); break;
         default:
-          if (a.kc > 0) { gemv_mma_chunked<T, true>(a, sm.xh, B, best_v, best_i, ring, sm.red); return; }
+          if (a.kc > 0) { gemv_mma_chunked<T, true, F8>(a, sm.xh, B, best_v, best_i, ring, sm.red); return; }
           stage_rows_copy<T>(reinterpret_cast<const T*>(p.h), B, p.ffn, sm.xh); break;
       }
-      gemv_mma<T, true>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
+      gemv_mma<T, true, F8>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
       return;
     }
     if (kind == 6) {
       if (p.hidden_out && blockIdx.x == 0)  // the residual stream before the final norm (Qwen3-TTS: input of the code predictor)
         for (int i = threadIdx.x; i < B * d; i += DEC_THREADS) p.hidden_out[(long long)step * B * d + i] = __ldcg(p.x + i);
       stage_rows_norm<T>(p.x, B, d, sm.xs, sm.xh, 2, p.norm_f, nullptr, p.eps, sm.s_red, sm.wb, wb_ready, p.norm_rg);
-      gemv_mma<T, true>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
+      gemv_mma<T, true, F8>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
       gemv_argmax_candidates(best_v, best_i, B, sm.sv, sm.si, p.cand_val, p.cand_idx);
     } else {
       static_assert(sizeof(SampShared) <= 2 * DEC_THREADS * 16, "sampling scratch must fit the tail-round buffer");
@@ -265,7 +268,7 @@ struct LdModel {
   }
 };
 
-template <typename T>
+template <typename T, bool F8>
 __global__ void __launch_bounds__(DEC_THREADS, 1)
 llama_decode_kernel(const LlamaDecParams p, int step_begin, int step_end, int ph_begin, int ph_end, int coop) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -285,7 +288,7 @@ llama_decode_kernel(const LlamaDecParams p, int step_begin, int step_end, int ph
   const DecSmem lay = dec_smem_layout(p.B, p.d, kmax_whole, p.d, p.norm_rg);
   GemvRing& ring = s_rings[threadIdx.x >> 5];
   gemv_ring_init(ring, smem_raw + lay.ring_off, p.ring_slots, s_plans);
-  const LdModel<T> model{sp, ld_nsub(p) * p.layers + 2};
+  const LdModel<T, F8> model{sp, ld_nsub(p) * p.layers + 2};
   dec_run<T>(p, model, dec_views<T>(smem_raw, lay), ring, s_args, step_begin, step_end, ph_begin, ph_end, coop);
 }
 
@@ -308,14 +311,14 @@ __global__ void llama_decode_init_kernel(const LlamaDecParams p) {
   dec_init_session(p, b, p.n_steps);
 }
 
-template <typename T>
+template <typename T, bool F8>
 int launch_t(s2s_ctx* ctx, const LlamaDecParams& p, int debug_phases, cudaStream_t stream) {
   int grid = dec_grid(ctx);                          // the context's SM partition (s2s_set_sm_partition)
   if (const char* e = getenv("S2S_DECODE_CTAS")) {   // developer knob: override for experiments (tests/dev/dev_lanes.py)
     const int v = atoi(e);
     if (v >= 8 && v < ctx->num_sms) grid = v;
   }
-  auto kern = llama_decode_kernel<T>;
+  auto kern = llama_decode_kernel<T, F8>;
   long long max_dyn = 0;
   S2S_CHECK_CUDA(s2s_max_dyn_smem(kern, ctx->device, &max_dyn));
   LlamaDecPlan pl;
@@ -336,22 +339,27 @@ int launch_t(s2s_ctx* ctx, const LlamaDecParams& p, int debug_phases, cudaStream
 
 }  // namespace
 
-int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int debug_phases, cudaStream_t stream) {
+int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int weight_format, int debug_phases, cudaStream_t stream) {
   S2S_REQUIRE(p.hd == 64 || p.hd == 128, "llama decode: head_dim must be 64 or 128");
   S2S_REQUIRE(p.layers <= 64, "llama decode: at most 64 layers");
   S2S_REQUIRE(p.n_steps >= 1, "llama decode: n_steps must be >= 1");
   S2S_REQUIRE(p.B >= 1 && p.B <= DEC_MAX_B, "llama decode: batch %d > %d must be split by the caller", p.B, DEC_MAX_B);
   S2S_REQUIRE(p.d % 64 == 0 && p.ffn % 64 == 0 && (p.heads * p.hd) % 64 == 0, "llama decode: d, ffn, heads*hd must be multiples of 64");
-  if (dtype == S2S_BF16) return launch_t<__nv_bfloat16>(ctx, p, debug_phases, stream);
-  if (dtype == S2S_F16) return launch_t<__half>(ctx, p, debug_phases, stream);
-  s2s_set_error("llama decode: unsupported dtype %d", dtype);
+  if (weight_format == S2S_FP8_E4M3) {
+    if (dtype == S2S_BF16 && p.head_stride == 0) return launch_t<__nv_bfloat16, true>(ctx, p, debug_phases, stream);
+  } else if (weight_format == dtype) {
+    if (dtype == S2S_BF16) return launch_t<__nv_bfloat16, false>(ctx, p, debug_phases, stream);
+    if (dtype == S2S_F16) return launch_t<__half, false>(ctx, p, debug_phases, stream);
+  }
+  s2s_set_error("llama decode: unsupported dtype %d with weight format %d", dtype, weight_format);
   return S2S_ERR_UNSUPPORTED;
 }
 
-int llama_decode_max_batch(int device, int dtype, int d, int ffn, int qd, int grid) {
+int llama_decode_max_batch(int device, int dtype, int weight_format, int d, int ffn, int qd, int grid) {
   long long max_dyn = 0;
-  const cudaError_t e = dtype == S2S_F16 ? s2s_max_dyn_smem(llama_decode_kernel<__half>, device, &max_dyn)
-                                         : s2s_max_dyn_smem(llama_decode_kernel<__nv_bfloat16>, device, &max_dyn);
+  const cudaError_t e = weight_format == S2S_FP8_E4M3 ? s2s_max_dyn_smem(llama_decode_kernel<__nv_bfloat16, true>, device, &max_dyn)
+                        : dtype == S2S_F16            ? s2s_max_dyn_smem(llama_decode_kernel<__half, false>, device, &max_dyn)
+                                                      : s2s_max_dyn_smem(llama_decode_kernel<__nv_bfloat16, false>, device, &max_dyn);
   if (e != cudaSuccess) return 0;
   return llama_decode_plan_max_batch(d, ffn, qd, grid, max_dyn);
 }

@@ -3,7 +3,8 @@
 #include "common.cuh"
 #include "sampling.cuh"
 
-struct LlamaDecLayer {          // device pointers; 16-bit weights [out, in]: TILED layout (weight_tiles.cu) in the kernel's table
+struct LlamaDecLayer {          // device pointers; 16-bit weights [out, in]: TILED layout (weight_tiles.cu) in the kernel's table,
+                                // or (weight format S2S_FP8_E4M3) tiled E4M3 codes followed by the fp32 row scales
   const void* w_qkv;            // [(H + 2 KV) * hd, d]; q and k rows stored pair-adjacent for RoPE (see llama.cu)
   const void* w_o;              // [d, H * hd]
   const void* w_gu;             // [2 * ffn, d], rows interleaved (gate_i, up_i)
@@ -17,7 +18,7 @@ struct LlamaDecParams {
   float eps;
   const LlamaDecLayer* lw;      // [layers] device
   const void* embed;            // [vocab, d] 16-bit
-  const void* lm_head;          // [vocab, d] 16-bit, TILED layout
+  const void* lm_head;          // [vocab, d] TILED layout, 16-bit or FP8 like the layers' matrices
   const float* norm_f;          // [d]
   const float2* rope;           // [max_pos][hd/2] (cos, sin)
   // state
@@ -72,6 +73,7 @@ struct LlamaDecParams {
   int seen_fixed;               // 1: the caller maintains the seen sets (Qwen3-TTS talker); the launch adds no fed id
 };
 
-int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int debug_phases, cudaStream_t stream);
+// dtype: the compute type (S2S_BF16 / S2S_F16); weight_format: dtype, or S2S_FP8_E4M3 (bf16 compute, single-table only)
+int llama_decode_launch(s2s_ctx* ctx, const LlamaDecParams& p, int dtype, int weight_format, int debug_phases, cudaStream_t stream);
 // largest batch per launch on `grid` CTAs that has a shared-memory plan (llama_decode_plan.cuh) on `device`
-int llama_decode_max_batch(int device, int dtype, int d, int ffn, int qd, int grid);
+int llama_decode_max_batch(int device, int dtype, int weight_format, int d, int ffn, int qd, int grid);

@@ -24,6 +24,7 @@ struct s2s_llama {
   s2s_ctx* ctx = nullptr;
   s2s_llama_config cfg{};
   bool finalized = false;
+  int weight_format = 0;                 // storage of the matrices the decode launch streams: cfg.compute_dtype, or S2S_FP8_E4M3
   int debug_phases = 0;
   std::vector<void*> allocs;
   std::unordered_map<std::string, LSlot> slots;
@@ -32,7 +33,7 @@ struct s2s_llama {
   void *embed = nullptr, *lm_head = nullptr;
   float* norm_f = nullptr;
   std::vector<LlamaDecLayer> layers_h;   // row-major weights (prefill GEMMs)
-  std::vector<LlamaDecLayer> tiled_h;    // fragment-major copies streamed by the decode kernel
+  std::vector<LlamaDecLayer> tiled_h;    // fragment-major copies streamed by the decode kernel (16-bit, or FP8 codes + row scales)
   LlamaDecLayer* layers_d = nullptr;     // device copy of tiled_h
   void* lm_head_t = nullptr;
   float2* rope = nullptr;

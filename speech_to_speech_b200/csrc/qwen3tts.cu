@@ -506,7 +506,7 @@ int s2s_qwen3tts_decode_frames_logits(s2s_qwen3tts* m, const int32_t* slots_h, i
       p.hidden_out = m->hidden; p.suppress = m->suppress;
       p.samp = tsamp_d; p.seen_fixed = 1;
       p.logits_out = talker_logits_out_d ? talker_logits_out_d + (long long)f * B * c.vocab : nullptr;
-      S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->talker->debug_phases, st));
+      S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->talker->weight_format, m->talker->debug_phases, st));
     }
     frame_mid_kernel<<<B, 256, 0, st>>>(m->hidden, m->talker->norm_f, c.rms_eps, d, m->x_in_p, m->pslot_d, m->ppos_d, m->code0,
                                         forced_codes_d, f, n_frames, G, m->code0_feed, m->forced_frame, psamp_d, tb);
@@ -520,7 +520,7 @@ int s2s_qwen3tts_decode_frames_logits(s2s_qwen3tts* m, const int32_t* slots_h, i
       p.embed0 = m->talker->embed; p.embed_stride = (long long)m->pred->embed_table_elems; p.head_stride = (long long)m->pred->head_t_table_elems;
       p.samp = psamp_d;
       p.logits_out = pred_logits_out_d ? pred_logits_out_d + (long long)f * G * B * c.cp_vocab : nullptr;
-      S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->pred->debug_phases, st));
+      S2S_CHECK(llama_decode_launch(m->ctx, p, c.compute_dtype, m->pred->weight_format, m->pred->debug_phases, st));
     }
     const int* ff = forced_codes_d ? m->forced_frame : nullptr;
     if (bf) frame_finish_kernel<__nv_bfloat16><<<B, 256, 0, st>>>(tb, f, n_frames, G, m->pcodes, m->code0, ff, (const __nv_bfloat16*)m->talker->embed,

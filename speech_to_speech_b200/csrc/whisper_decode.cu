@@ -132,6 +132,7 @@ __device__ __noinline__ void wd_select(const WhisperDecParams& p, int g, int pos
 template <typename T>
 struct WdModel {
   static constexpr bool stamps_barrier = true;
+  static constexpr bool f8_weights = false;
   const WhisperDecParams& p;
   int n_phases;
 
@@ -309,6 +310,7 @@ __device__ __forceinline__ void wdc_out_args(const WhisperDecParams& p, const Wd
 template <typename T>
 struct WdcModel {
   static constexpr bool stamps_barrier = false;
+  static constexpr bool f8_weights = false;
   const WhisperDecParams& p;
   WdcCtx cx;
   int n_phases;

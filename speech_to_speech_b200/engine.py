@@ -288,11 +288,18 @@ class LlamaEngine:
     """Llama-family LLM on one H100: wgmma prefill + persistent decode (greedy, or sampled per slot) with a per-session KV cache."""
 
     def __init__(self, geometry: Mapping[str, float], dtype: str = "bfloat16", max_sessions: int = 1,
-                 max_positions: int = 2048, max_prefill: int = 512, device: int = 0, lane: int = 0, lanes: int = 1):
+                 max_positions: int = 2048, max_prefill: int = 512, device: int = 0, lane: int = 0, lanes: int = 1,
+                 weight_dtype: Optional[str] = None):
+        """weight_dtype: None = the projections are stored as `dtype`; "float8_e4m3" = weight-only FP8 with a power-of-two
+        scale per row (bfloat16 compute only), quantised from the 16-bit weights when they are loaded.  Halves the bytes a
+        decode step streams; the engine then computes, bit for bit, what a 16-bit engine bound to the dequantised weights does."""
+        if weight_dtype is not None and weight_dtype not in _lib.WEIGHT_FORMAT_CODES:
+            raise ValueError(f"weight_dtype {weight_dtype!r}: supported values are None and {sorted(_lib.WEIGHT_FORMAT_CODES)}")
         self.lib = _lib.load()
         self.device = device
         self.ctx = get_context(device, lane, lanes)
         self.geometry = dict(geometry)
+        self.weight_dtype = weight_dtype
         g = self.geometry
         self.cfg = LlamaConfig(
             int(g["d_model"]), int(g["layers"]), int(g["heads"]), int(g["kv_heads"]), int(g["head_dim"]), int(g["ffn"]),
@@ -303,6 +310,9 @@ class LlamaEngine:
         self.max_positions = self.cfg.max_positions
         self.handle = C.c_void_p()
         check(self.lib.s2s_llama_create(self.ctx, C.byref(self.cfg), C.byref(self.handle)), "s2s_llama_create")
+        if weight_dtype is not None:
+            check(self.lib.s2s_llama_set_weight_format(self.handle, _lib.WEIGHT_FORMAT_CODES[weight_dtype]),
+                  "s2s_llama_set_weight_format")
 
     def load_state_dict(self, weights: Mapping[str, "np.ndarray | torch.Tensor"]) -> None:
         for name, w in weights.items():
@@ -367,6 +377,10 @@ class LlamaEngine:
         check(self.lib.s2s_llama_decode(self.handle, sl, B, _ptr(first_ids), n_steps, eos_id, _ptr(ids), _ptr(lens),
                                         _ptr(forced), _ptr(logits), _stream_ptr(self.device)), "s2s_llama_decode")
         return (ids, lens, logits) if return_logits else (ids, lens)
+
+    def weight_format(self) -> int:
+        """The S2S_* code of the streamed projections' storage (S2S_FP8_E4M3, or the compute dtype's code)."""
+        return int(self.lib.s2s_llama_weight_format(self.handle))
 
     def max_decode_batch(self) -> int:
         """Sessions one decode launch can carry for this geometry (shared-memory budget of the kernel)."""

@@ -344,12 +344,17 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
         if lane is None:   # not pinned by the caller: units join the lanes round-robin in construction order
             lane = assign_lane(("llama", model_name, dev), lanes)
         lane = int(lane) % lanes
+        # weight-only FP8 for the decode launch's projections (engine.LlamaEngine; INTEGRATION.md): off unless asked for
+        weight_dtype = self.gen_kwargs.pop("weight_dtype", None)
+        if weight_dtype not in (None, "float8_e4m3"):
+            raise ValueError(f"weight_dtype={weight_dtype!r}: supported values are None (weights stored as torch_dtype) and 'float8_e4m3'")
+        fmt = {"weight_dtype": weight_dtype} if weight_dtype else {}
 
         def build() -> _LlamaBundle:
             if model_name.startswith("random:"):
                 parts = model_name.split(":")
                 geom = LLAMA_GEOMETRIES[parts[1]]
-                engine = E.LlamaEngine(geom, dtype=torch_dtype, max_sessions=max_sessions, max_positions=max_pos, max_prefill=512, device=dev, lane=lane, lanes=lanes)
+                engine = E.LlamaEngine(geom, dtype=torch_dtype, max_sessions=max_sessions, max_positions=max_pos, max_prefill=512, device=dev, lane=lane, lanes=lanes, **fmt)
                 engine.init_random(int(parts[2]) if len(parts) > 2 else 0)
                 return _LlamaBundle(engine, _IdTokenizer(geom["vocab"]), [geom["vocab"] - 1], max_sessions, batch_wait_s, lane, lanes, batch_gap_s)
             # the checkpoint is read before the weights are loaded so that unsupported options fail fast
@@ -363,7 +368,7 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
             hf = AutoModelForCausalLM.from_pretrained(model_name)
             c = hf.config
             geom = geometry_from_hf_config(c, max_pos)
-            engine = E.LlamaEngine(geom, dtype=torch_dtype, max_sessions=max_sessions, max_positions=max_pos, max_prefill=512, device=dev, lane=lane, lanes=lanes)
+            engine = E.LlamaEngine(geom, dtype=torch_dtype, max_sessions=max_sessions, max_positions=max_pos, max_prefill=512, device=dev, lane=lane, lanes=lanes, **fmt)
             engine.load_state_dict(hf.state_dict())
             eos = hf.generation_config.eos_token_id
             eos_ids = list(eos) if isinstance(eos, (list, tuple)) else [int(eos)]
@@ -372,7 +377,7 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
 
         if model_name.startswith("random:"):
             resolve_generation(self.gen_kwargs)
-        self._shared_key = ("llama", model_name, torch_dtype, dev, max_sessions, max_pos, lane, lanes) if max_sessions > 1 else None
+        self._shared_key = ("llama", model_name, torch_dtype, weight_dtype, dev, max_sessions, max_pos, lane, lanes) if max_sessions > 1 else None
         self.bundle = acquire_shared(self._shared_key, build, lambda b: b.close()) if self._shared_key else build()
         self.engine, self.tokenizer, self.eos_ids = self.bundle.engine, self.bundle.tokenizer, self.bundle.eos_ids
         self.sampling = resolve_generation(self.gen_kwargs, getattr(self.bundle, "generation_config", None))
