@@ -251,6 +251,32 @@ int s2s_codec_decode(s2s_codec* m, const int32_t* codes_d, int32_t T, int32_t ct
 int32_t s2s_codec_samples(s2s_codec* m, int32_t T);   /* waveform length of a T-frame decode before the context drop */
 int32_t s2s_codec_total_upsample(s2s_codec* m);       /* samples per frame (1920) */
 
+/* One contraction of the codec decoder (exposed for tests / benches), on a chosen kernel:
+ *   Y[t, n] = epi( bias[n % bias_mod] + sum_{j < k} sum_{c < C_in} X[t + x_row0 + j * dil, c] * W[j][c][n] )
+ * for t in [t0, T_out) and n < N of each of `batch` sequences (sequence b: x + b * x_bs, y + b * y_bs, resid + b * r_bs;
+ * all strides in elements).  Rows of X outside [0, T_in) read as zero.  X is [T_in rows, ldx] f32, W is [k][C_in][N] f32
+ * (tap-major; a transposed convolution of stride s with kernel 2 s is the 2-tap contraction with N = s * C_out whose
+ * [T_in - 1, s * C_out] output is the time-major [(T_in - 1) * s, C_out] result), bias [bias_mod] or NULL.  epi: act
+ * (0 none, 1 exact GELU, 2 SiLU), then * scale[n] (scale NULL = 1), then + resid[t, n] (resid may alias y; NULL = 0).
+ * Rows below t0, columns in [N, ldy) and rows past T_out are not written.
+ * path 0: fp32 FMA (conv1d_f32_kernel); 1: tensor cores, fp16 operands converted while staged (conv1d_tc_kernel);
+ * 2: tensor cores fed from x16, an fp16 copy of X with the same shape and strides (conv1d_tc16_kernel; needs
+ * C_in % 8 == 0, N % 4 == 0, ldx % 8 == 0, x_bs % 8 == 0).  Paths 1 and 2 pack W into fp16 k-pairs in scratch memory of
+ * their own.  Synchronous: returns after the stream has finished the contraction. */
+typedef struct {
+  const float* x; int64_t ldx; int32_t T_in; int32_t x_row0;
+  const void* x16;
+  const float* w; int32_t k, dil, C_in, N;
+  const float* bias; int32_t bias_mod;
+  int32_t act;
+  const float* scale;
+  const float* resid; int64_t ldr;
+  float* y; int64_t ldy; int32_t T_out;
+  int32_t t0;
+  int32_t batch; int64_t x_bs, y_bs, r_bs;
+} s2s_conv_args;
+int s2s_codec_contract(s2s_ctx* ctx, const s2s_conv_args* args, int32_t path, void* stream);
+
 /* ---- Qwen3-TTS talker + code predictor: text -> codebook ids, 12.5 frames per second of speech ------------------
  * Replaces the autoregressive half of faster-qwen3-tts' `generate_custom_voice_streaming(text, speaker, language,
  * instruct, chunk_size, max_new_tokens, non_streaming_mode)` (S/TTS/qwen3_tts_handler.py:946-978; warm-up :555-572).

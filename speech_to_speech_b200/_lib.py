@@ -25,7 +25,7 @@ EXPORTED = [
     "s2s_llama_set_weight_format", "s2s_llama_weight_format",
     "s2s_tts_postproc",
     "s2s_codec_create", "s2s_codec_destroy", "s2s_codec_bind_tensor", "s2s_codec_init_random", "s2s_codec_finalize",
-    "s2s_codec_decode", "s2s_codec_samples", "s2s_codec_total_upsample",
+    "s2s_codec_decode", "s2s_codec_samples", "s2s_codec_total_upsample", "s2s_codec_contract",
     "s2s_qwen3tts_create", "s2s_qwen3tts_destroy", "s2s_qwen3tts_bind_tensor", "s2s_qwen3tts_init_random",
     "s2s_qwen3tts_finalize", "s2s_qwen3tts_prefill", "s2s_qwen3tts_set_sampling", "s2s_qwen3tts_decode_frames",
     "s2s_qwen3tts_decode_frames_logits", "s2s_qwen3tts_decode_audio", "s2s_qwen3tts_decode_audio_batch",
@@ -72,6 +72,22 @@ class CodecConfig(C.Structure):
         ("n_upsampling_ratios", C.c_int32), ("upsampling_ratios", C.c_int32 * 4),
         ("decoder_dim", C.c_int32), ("sliding_window", C.c_int32), ("rope_theta", C.c_float), ("rms_eps", C.c_float),
         ("max_frames", C.c_int32), ("max_batch", C.c_int32), ("precision", C.c_int32)]
+
+
+class ConvArgs(C.Structure):
+    """s2s_conv_args: one codec-decoder contraction (s2s_codec_contract)."""
+    _fields_ = [
+        ("x", C.c_void_p), ("ldx", C.c_int64), ("T_in", C.c_int32), ("x_row0", C.c_int32),
+        ("x16", C.c_void_p),
+        ("w", C.c_void_p), ("k", C.c_int32), ("dil", C.c_int32), ("C_in", C.c_int32), ("N", C.c_int32),
+        ("bias", C.c_void_p), ("bias_mod", C.c_int32),
+        ("act", C.c_int32),
+        ("scale", C.c_void_p),
+        ("resid", C.c_void_p), ("ldr", C.c_int64),
+        ("y", C.c_void_p), ("ldy", C.c_int64), ("T_out", C.c_int32),
+        ("t0", C.c_int32),
+        ("batch", C.c_int32), ("x_bs", C.c_int64), ("y_bs", C.c_int64), ("r_bs", C.c_int64),
+    ]
 
 
 class Qwen3TTSConfig(C.Structure):
@@ -153,6 +169,7 @@ def load() -> C.CDLL:
     lib.s2s_codec_samples.restype = i32
     lib.s2s_codec_total_upsample.argtypes = [vp]
     lib.s2s_codec_total_upsample.restype = i32
+    lib.s2s_codec_contract.argtypes = [vp, C.POINTER(ConvArgs), i32, vp]
     lib.s2s_qwen3tts_create.argtypes = [vp, C.POINTER(Qwen3TTSConfig), C.POINTER(vp)]
     lib.s2s_qwen3tts_destroy.argtypes = [vp]
     lib.s2s_qwen3tts_bind_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]

@@ -513,9 +513,12 @@ __global__ void clamp_out_kernel(const float* __restrict__ x, long long x_bs, in
   if (i < n) wav[(long long)blockIdx.y * wav_bs + i] = fminf(1.0f, fmaxf(-1.0f, x[(long long)blockIdx.y * x_bs + skip + i]));
 }
 
-__global__ void exp_prep_kernel(float* a, float* b, int n) {   // alpha -> exp(alpha); beta -> 1 / (exp(beta) + 1e-9)
+// alpha -> exp(alpha); beta -> 1 / (exp(beta) + 1e-9); a null pointer leaves that parameter as it is
+__global__ void exp_prep_kernel(float* a, float* b, int n) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) { a[i] = expf(a[i]); b[i] = 1.0f / (expf(b[i]) + 1e-9f); }
+  if (i >= n) return;
+  if (a) a[i] = expf(a[i]);
+  if (b) b[i] = 1.0f / (expf(b[i]) + 1e-9f);
 }
 
 inline float src_f32(const void* data, int64_t i, int dtype) {
@@ -533,6 +536,7 @@ struct CSlot {
   int kind = C_PLAIN;
   int d0 = 0, d1 = 0, d2 = 0, stride = 0;   // source dims
   bool bound = false;
+  bool raw = false;   // written by bind / init_random since the last finalize (SnakeBeta parameters are transformed there)
   float rnd_scale = 0.02f, rnd_offset = 0.f;
 };
 
@@ -590,8 +594,7 @@ struct s2s_codec {
   bool finalized = false;
   std::vector<void*> allocs;
   std::unordered_map<std::string, CSlot> slots;
-  std::vector<std::pair<float*, float*>> snake_pairs;   // (alpha, beta) buffers and their length, transformed at finalize
-  std::vector<int> snake_len;
+  std::vector<std::pair<CSlot*, CSlot*>> snake_pairs;   // SnakeBeta (alpha, beta) slots, transformed in place at finalize
   float* embed = nullptr;
   std::vector<CodecLayer> layers;
   float* norm_f = nullptr;
@@ -702,8 +705,7 @@ int build(CodecDecoder* m) {
   auto snake = [&](const std::string& pa, const std::string& pb, float** a, float** b, int n) -> int {
     S2S_CHECK(cslot(m, pa, a, C_PLAIN, n, 0, 0, 0, 0.2f));
     S2S_CHECK(cslot(m, pb, b, C_PLAIN, n, 0, 0, 0, 0.2f));
-    m->snake_pairs.push_back({*a, *b});
-    m->snake_len.push_back(n);
+    m->snake_pairs.push_back({&m->slots[pa], &m->slots[pb]});   // unordered_map element addresses are stable
     return S2S_OK;
   };
   for (int i = 0; i < c.n_upsample_rates; ++i) {
@@ -849,7 +851,7 @@ int codec_bind_tensor(CodecDecoder* m, const char* name, const void* data_h, con
     for (int nn = 0; nn < N; ++nn)
       for (int k = 0; k < K; ++k) tmp[(size_t)k * N + nn] = src_f32(data_h, (int64_t)nn * K + k, dtype);
     S2S_CHECK_CUDA(cudaMemcpy2D(s.dst + col0, (size_t)Nt * 4, tmp.data(), (size_t)N * 4, (size_t)N * 4, K, cudaMemcpyHostToDevice));
-    s.bound = true;
+    s.bound = s.raw = true;
     return S2S_OK;
   }
   std::vector<float> tmp((size_t)n);
@@ -879,7 +881,7 @@ int codec_bind_tensor(CodecDecoder* m, const char* name, const void* data_h, con
     for (int64_t i = 0; i < n; ++i) tmp[(size_t)i] = src_f32(data_h, i, dtype);
   }
   S2S_CHECK_CUDA(cudaMemcpy(s.dst, tmp.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
-  s.bound = true;
+  s.bound = s.raw = true;
   return S2S_OK;
 }
 
@@ -899,7 +901,7 @@ int codec_init_random(CodecDecoder* m, uint64_t seed) {
     } else {
       S2S_CHECK(fill_random_launch(s.dst, s.n, S2S_F32, s.rnd_scale, s.rnd_offset, seed ^ hsh, 0));
     }
-    s.bound = true;
+    s.bound = s.raw = true;
   }
   S2S_CHECK_CUDA(cudaDeviceSynchronize());
   return S2S_OK;
@@ -910,11 +912,15 @@ int codec_finalize(CodecDecoder* m) {
   for (auto& kv : m->slots)
     if (!kv.second.bound) { s2s_set_error("codec finalize: tensor '%s' was never bound", kv.first.c_str()); return S2S_ERR_INVALID; }
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  if (!m->finalized)   // SnakeBeta parameters -> (exp(alpha), 1 / (exp(beta) + 1e-9)), once
-    for (size_t i = 0; i < m->snake_pairs.size(); ++i) {
-      exp_prep_kernel<<<(m->snake_len[i] + 255) / 256, 256>>>(m->snake_pairs[i].first, m->snake_pairs[i].second, m->snake_len[i]);
-      S2S_LAUNCH_CHECK();
-    }
+  // SnakeBeta parameters -> (exp(alpha), 1 / (exp(beta) + 1e-9)): exactly those written since the last finalize, so a
+  // reload (or a partial one) leaves every buffer transformed once
+  for (auto& p : m->snake_pairs) {
+    CSlot &sa = *p.first, &sb = *p.second;
+    if (!sa.raw && !sb.raw) continue;
+    exp_prep_kernel<<<(unsigned)((sa.n + 255) / 256), 256>>>(sa.raw ? sa.dst : nullptr, sb.raw ? sb.dst : nullptr, (int)sa.n);
+    S2S_LAUNCH_CHECK();
+    sa.raw = sb.raw = false;
+  }
   // fp16 k-pair copies for the tensor-core contraction (rebuilt on every (re)load)
   for (auto& kv : m->tc_w) {
     CodecDecoder::TcW& t = kv.second;
@@ -1111,4 +1117,50 @@ int s2s_codec_decode(s2s_codec* m, const int32_t* codes_d, int32_t T, int32_t ct
 }
 int32_t s2s_codec_samples(s2s_codec* m, int32_t T) { return m ? codec_samples_for(m, T) : 0; }
 int32_t s2s_codec_total_upsample(s2s_codec* m) { return m ? codec_total_upsample(m) : 0; }
+
+// test / bench entry point: one contraction on the kernel `path` names, not on the one contract() would pick
+int s2s_codec_contract(s2s_ctx* ctx, const s2s_conv_args* args, int32_t path, void* stream) {
+  S2S_REQUIRE(ctx && args, "s2s_codec_contract: null argument");
+  const s2s_conv_args& c = *args;
+  S2S_REQUIRE(path >= 0 && path <= 2, "s2s_codec_contract: path %d not in {0, 1, 2}", path);
+  S2S_REQUIRE(c.w && c.y && (path == 2 ? c.x16 != nullptr : c.x != nullptr), "s2s_codec_contract: null x%s / w / y",
+              path == 2 ? "16" : "");
+  S2S_REQUIRE(c.k >= 1 && c.C_in >= 1 && c.N >= 1 && c.dil >= 1, "s2s_codec_contract: k %d / C_in %d / N %d / dil %d must be >= 1",
+              c.k, c.C_in, c.N, c.dil);
+  S2S_REQUIRE(c.T_in >= 0 && c.T_out >= 0 && c.t0 >= 0, "s2s_codec_contract: negative T_in / T_out / t0");
+  S2S_REQUIRE(c.batch >= 1 && c.batch <= 65535 && c.x_bs >= 0 && c.y_bs >= 0 && c.r_bs >= 0,
+              "s2s_codec_contract: batch %d / negative sequence stride", c.batch);
+  S2S_REQUIRE(c.ldx >= c.C_in && c.ldy >= c.N && (!c.resid || c.ldr >= c.N), "s2s_codec_contract: row stride below the row width");
+  S2S_REQUIRE(!c.bias || c.bias_mod >= 1, "s2s_codec_contract: bias_mod %d < 1", c.bias_mod);
+  S2S_REQUIRE(c.act >= 0 && c.act <= 2, "s2s_codec_contract: act %d not in {0, 1, 2}", c.act);
+  S2S_REQUIRE(path != 2 || (c.C_in % 8 == 0 && c.N % 4 == 0 && c.ldx % 8 == 0 && c.x_bs % 8 == 0 &&
+                            (reinterpret_cast<uintptr_t>(c.x16) & 15) == 0),
+              "s2s_codec_contract: path 2 needs C_in %% 8 == 0, N %% 4 == 0, ldx and x_bs %% 8 == 0 and a 16-byte aligned x16");
+  ConvArgs a{};
+  a.x = c.x; a.ldx = c.ldx; a.T_in = c.T_in; a.x_row0 = c.x_row0; a.x16 = path == 2 ? c.x16 : nullptr;
+  a.w = c.w; a.k = c.k; a.dil = c.dil; a.C_in = c.C_in; a.N = c.N;
+  a.bias = c.bias; a.bias_mod = c.bias_mod; a.act = c.act; a.scale = c.scale; a.resid = c.resid; a.ldr = c.ldr;
+  a.y = c.y; a.ldy = c.ldy; a.T_out = c.T_out; a.t0 = c.t0;
+  a.batch = c.batch; a.x_bs = c.x_bs; a.y_bs = c.y_bs; a.r_bs = c.r_bs;
+  S2S_CHECK_CUDA(cudaSetDevice(ctx->device));
+  const cudaStream_t st = (cudaStream_t)stream;
+  void* packed = nullptr;   // fp16 k-pairs of w, packed as codec_finalize packs the model's weights
+  auto run = [&]() -> int {
+    if (path == 0) return conv1d_f32_launch(a, st);
+    const size_t words = (size_t)c.k * ((c.C_in + 1) / 2) * c.N;
+    S2S_CHECK_CUDA(cudaMalloc(&packed, words * 4));
+    pack_weight_pairs_kernel<<<(unsigned)std::min<size_t>((words + 255) / 256, 4096), 256, 0, st>>>(c.w, c.k, c.C_in, c.N,
+                                                                                                   reinterpret_cast<__half2*>(packed));
+    S2S_LAUNCH_CHECK();
+    return conv1d_tc_launch(a, packed, st);
+  };
+  int rc = run();
+  const cudaError_t e = cudaStreamSynchronize(st);
+  if (rc == S2S_OK && e != cudaSuccess) {
+    s2s_set_error("s2s_codec_contract: %s", cudaGetErrorString(e));
+    rc = S2S_ERR_CUDA;
+  }
+  cudaFree(packed);
+  return rc;
+}
 }  // extern "C"

@@ -284,6 +284,35 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, kv_
     return o
 
 
+def codec_contract(x: Optional[torch.Tensor], w: torch.Tensor, y: torch.Tensor, *, path: int = 0,
+                   x16: Optional[torch.Tensor] = None, T_in: Optional[int] = None, T_out: Optional[int] = None, x_row0: int = 0,
+                   dil: int = 1, bias: Optional[torch.Tensor] = None, bias_mod: Optional[int] = None, act: int = 0,
+                   scale: Optional[torch.Tensor] = None, resid: Optional[torch.Tensor] = None, t0: int = 0) -> None:
+    """One codec-decoder contraction written into `y` on kernel `path` (0 fp32, 1 tensor cores converting, 2 tensor cores
+    reading `x16`; include/s2s_b200.h s2s_codec_contract).  Contiguous cuda tensors: x f32 / x16 f16 [B, rows, ldx] (or
+    [rows, ldx]), w f32 [k, C_in, N], y and resid f32 [B, rows, ld]; resid may be y.  Row and sequence strides come from the
+    shapes; T_in / T_out default to the row counts of x and y.  Synchronous."""
+    xs = x if x is not None else x16
+    for t in (xs, w, y, x16, bias, scale, resid):
+        assert t is None or (t.is_cuda and t.is_contiguous())
+    assert w.dtype == torch.float32 and w.dim() == 3 and xs.dim() == y.dim() and xs.dim() in (2, 3)
+    k, C_in, N = w.shape
+    batch = xs.shape[0] if xs.dim() == 3 else 1
+    if x16 is not None:
+        assert x16.dtype == torch.float16 and (x is None or x16.shape == x.shape)
+    if resid is not None:
+        assert resid.dim() == y.dim() and (resid.dim() == 2 or resid.shape[0] == batch)
+    seq = lambda t: t.shape[-2] * t.shape[-1] if t is not None and t.dim() == 3 else 0
+    a = _lib.ConvArgs(
+        x=_ptr(x).value, ldx=xs.shape[-1], T_in=xs.shape[-2] if T_in is None else T_in, x_row0=x_row0, x16=_ptr(x16).value,
+        w=w.data_ptr(), k=k, dil=dil, C_in=C_in, N=N, bias=_ptr(bias).value, bias_mod=N if bias_mod is None else bias_mod,
+        act=act, scale=_ptr(scale).value, resid=_ptr(resid).value, ldr=0 if resid is None else resid.shape[-1],
+        y=y.data_ptr(), ldy=y.shape[-1], T_out=y.shape[-2] if T_out is None else T_out, t0=t0,
+        batch=batch, x_bs=seq(xs), y_bs=seq(y), r_bs=seq(resid))
+    dev = y.device.index or 0
+    check(_lib.load().s2s_codec_contract(get_context(dev), C.byref(a), path, _stream_ptr(dev)), "s2s_codec_contract")
+
+
 class LlamaEngine:
     """Llama-family LLM on one H100: wgmma prefill + persistent decode (greedy, or sampled per slot) with a per-session KV cache."""
 
