@@ -28,6 +28,7 @@
 
 #include "codec_decode.cuh"
 #include "kernels.cuh"
+#include "weight_arena.cuh"
 
 namespace {
 
@@ -521,25 +522,6 @@ __global__ void exp_prep_kernel(float* a, float* b, int n) {
   if (b) b[i] = 1.0f / (expf(b[i]) + 1e-9f);
 }
 
-inline float src_f32(const void* data, int64_t i, int dtype) {
-  if (dtype == S2S_F32) return reinterpret_cast<const float*>(data)[i];
-  uint16_t u = reinterpret_cast<const uint16_t*>(data)[i];
-  if (dtype == S2S_BF16) { uint32_t w = (uint32_t)u << 16; float f; memcpy(&f, &w, 4); return f; }
-  __half h; memcpy(&h, &u, 2); return __half2float(h);
-}
-
-enum CSlotKind { C_PLAIN = 0, C_LINEAR = 1 /* [N,K] -> [K][N] */, C_CONV = 2 /* [O,C,k] -> [k][C][O] */,
-                 C_TCONV = 3 /* [C,O,k] -> taps x [C][s*O] */ };
-struct CSlot {
-  float* dst = nullptr;
-  int64_t n = 0;
-  int kind = C_PLAIN;
-  int d0 = 0, d1 = 0, d2 = 0, stride = 0;   // source dims
-  bool bound = false;
-  bool raw = false;   // written by bind / init_random since the last finalize (SnakeBeta parameters are transformed there)
-  float rnd_scale = 0.02f, rnd_offset = 0.f;
-};
-
 }  // namespace
 
 int conv1d_tc_launch(const ConvArgs& a, const void* w_pairs, cudaStream_t st) {
@@ -592,9 +574,8 @@ struct s2s_codec {
   s2s_ctx* ctx = nullptr;
   s2s_codec_config cfg{};
   bool finalized = false;
-  std::vector<void*> allocs;
-  std::unordered_map<std::string, CSlot> slots;
-  std::vector<std::pair<CSlot*, CSlot*>> snake_pairs;   // SnakeBeta (alpha, beta) slots, transformed in place at finalize
+  WeightArena arena;
+  std::vector<std::pair<WeightSlot*, WeightSlot*>> snake_pairs;   // SnakeBeta (alpha, beta) slots, transformed in place at finalize
   float* embed = nullptr;
   std::vector<CodecLayer> layers;
   float* norm_f = nullptr;
@@ -616,26 +597,6 @@ namespace {
 
 void tc_register(CodecDecoder* m, const float* w, int k, int C_in, int N) { m->tc_w[w] = CodecDecoder::TcW{k, C_in, N, nullptr}; }
 
-int calloc_f(CodecDecoder* m, float** out, size_t n) {
-  void* p = nullptr;
-  S2S_CHECK_CUDA(cudaMalloc(&p, (n ? n : 4) * 4));
-  S2S_CHECK_CUDA(cudaMemset(p, 0, (n ? n : 4) * 4));
-  m->allocs.push_back(p);
-  *out = reinterpret_cast<float*>(p);
-  return S2S_OK;
-}
-
-int cslot(CodecDecoder* m, const std::string& name, float** out, int kind, int d0, int d1, int d2, int stride, float rs,
-          float ro = 0.f) {
-  CSlot s;
-  s.kind = kind; s.d0 = d0; s.d1 = d1; s.d2 = d2; s.stride = stride; s.rnd_scale = rs; s.rnd_offset = ro;
-  s.n = (int64_t)d0 * (d1 ? d1 : 1) * (d2 ? d2 : 1);
-  S2S_CHECK(calloc_f(m, &s.dst, (size_t)s.n));
-  *out = s.dst;
-  m->slots[name] = s;
-  return S2S_OK;
-}
-
 // sequence lengths along the decoder for T frames
 void codec_lengths(const s2s_codec_config& c, int T, std::vector<int>& L) {
   int len = T;
@@ -648,35 +609,38 @@ void codec_lengths(const s2s_codec_config& c, int T, std::vector<int>& L) {
 int build(CodecDecoder* m) {
   const auto& c = m->cfg;
   const int H = c.hidden, hd = H / c.heads, qd = c.heads * hd, kvd = c.kv_heads * hd, I = c.inter;
-  float* dummy;
-  S2S_CHECK(cslot(m, "code_embedding.weight", &m->embed, C_PLAIN, c.codebook_size * c.quantizers, H, 0, 0, 1.0f));
+  WeightArena& A = m->arena;
+  // a tensor with an fp32 buffer of its own: d0 * max(d1, 1) * max(d2, 1) elements
+  auto slot = [&](const std::string& name, float** out, int layout, int d0, int d1, int d2, int p, float rs, float ro = 0.f) -> int {
+    const int64_t n = (int64_t)d0 * (d1 ? d1 : 1) * (d2 ? d2 : 1);
+    S2S_CHECK(A.alloc(out, (size_t)n * 4));
+    A.add(name, *out, false, n, rs, ro).as(layout, d0, d1, d2, p);
+    return S2S_OK;
+  };
+  S2S_CHECK(slot("code_embedding.weight", &m->embed, W_PLAIN, c.codebook_size * c.quantizers, H, 0, 0, 1.0f));
   m->layers.resize(c.layers);
   const float sh = 1.0f / sqrtf((float)H);
   for (int l = 0; l < c.layers; ++l) {
     const std::string p = "pre_transformer.layers." + std::to_string(l) + ".";
     CodecLayer& L = m->layers[l];
     // q, k, v share one [H][qd + 2 kvd] matrix; gate and up one [H][2 I] matrix (column blocks)
-    S2S_CHECK(calloc_f(m, &L.w_qkv, (size_t)H * (qd + 2 * kvd)));
-    S2S_CHECK(calloc_f(m, &L.w_gu, (size_t)H * 2 * I));
-    auto sub = [&](const std::string& name, float* base, int N_total, int col0, int N, int K, float rs) {
-      CSlot s; s.dst = base; s.kind = C_LINEAR; s.d0 = N; s.d1 = K; s.d2 = N_total; s.stride = col0; s.n = (int64_t)N * K; s.rnd_scale = rs;
-      m->slots[name] = s;
-    };
-    sub(p + "self_attn.q_proj.weight", L.w_qkv, qd + 2 * kvd, 0, qd, H, sh);
-    sub(p + "self_attn.k_proj.weight", L.w_qkv, qd + 2 * kvd, qd, kvd, H, sh);
-    sub(p + "self_attn.v_proj.weight", L.w_qkv, qd + 2 * kvd, qd + kvd, kvd, H, sh);
-    sub(p + "mlp.gate_proj.weight", L.w_gu, 2 * I, 0, I, H, sh);
-    sub(p + "mlp.up_proj.weight", L.w_gu, 2 * I, I, I, H, sh);
-    S2S_CHECK(cslot(m, p + "self_attn.o_proj.weight", &L.w_o, C_LINEAR, H, qd, 0, 0, sh));
-    S2S_CHECK(cslot(m, p + "mlp.down_proj.weight", &L.w_down, C_LINEAR, H, I, 0, 0, 1.0f / sqrtf((float)I)));
+    S2S_CHECK(A.alloc(&L.w_qkv, (size_t)H * (qd + 2 * kvd) * 4));
+    S2S_CHECK(A.alloc(&L.w_gu, (size_t)H * 2 * I * 4));
+    A.add(p + "self_attn.q_proj.weight", L.w_qkv, false, (int64_t)qd * H, sh).as(W_LINEAR, qd, H, 0, 0, qd + 2 * kvd);
+    A.add(p + "self_attn.k_proj.weight", L.w_qkv, false, (int64_t)kvd * H, sh).as(W_LINEAR, kvd, H, 0, qd, qd + 2 * kvd);
+    A.add(p + "self_attn.v_proj.weight", L.w_qkv, false, (int64_t)kvd * H, sh).as(W_LINEAR, kvd, H, 0, qd + kvd, qd + 2 * kvd);
+    A.add(p + "mlp.gate_proj.weight", L.w_gu, false, (int64_t)I * H, sh).as(W_LINEAR, I, H, 0, 0, 2 * I);
+    A.add(p + "mlp.up_proj.weight", L.w_gu, false, (int64_t)I * H, sh).as(W_LINEAR, I, H, 0, I, 2 * I);
+    S2S_CHECK(slot(p + "self_attn.o_proj.weight", &L.w_o, W_LINEAR, H, qd, 0, 0, sh));
+    S2S_CHECK(slot(p + "mlp.down_proj.weight", &L.w_down, W_LINEAR, H, I, 0, 0, 1.0f / sqrtf((float)I)));
     tc_register(m, L.w_qkv, 1, H, qd + 2 * kvd); tc_register(m, L.w_gu, 1, H, 2 * I);
     tc_register(m, L.w_o, 1, qd, H); tc_register(m, L.w_down, 1, I, H);
-    S2S_CHECK(cslot(m, p + "input_layernorm.weight", &L.n1, C_PLAIN, H, 0, 0, 0, 0.1f, 1.0f));
-    S2S_CHECK(cslot(m, p + "post_attention_layernorm.weight", &L.n2, C_PLAIN, H, 0, 0, 0, 0.1f, 1.0f));
-    S2S_CHECK(cslot(m, p + "self_attn_layer_scale.scale", &L.ls_attn, C_PLAIN, H, 0, 0, 0, 0.1f, 0.5f));
-    S2S_CHECK(cslot(m, p + "mlp_layer_scale.scale", &L.ls_mlp, C_PLAIN, H, 0, 0, 0, 0.1f, 0.5f));
+    S2S_CHECK(slot(p + "input_layernorm.weight", &L.n1, W_PLAIN, H, 0, 0, 0, 0.1f, 1.0f));
+    S2S_CHECK(slot(p + "post_attention_layernorm.weight", &L.n2, W_PLAIN, H, 0, 0, 0, 0.1f, 1.0f));
+    S2S_CHECK(slot(p + "self_attn_layer_scale.scale", &L.ls_attn, W_PLAIN, H, 0, 0, 0, 0.1f, 0.5f));
+    S2S_CHECK(slot(p + "mlp_layer_scale.scale", &L.ls_mlp, W_PLAIN, H, 0, 0, 0, 0.1f, 0.5f));
   }
-  S2S_CHECK(cslot(m, "pre_transformer.norm.weight", &m->norm_f, C_PLAIN, H, 0, 0, 0, 0.1f, 1.0f));
+  S2S_CHECK(slot("pre_transformer.norm.weight", &m->norm_f, W_PLAIN, H, 0, 0, 0, 0.1f, 1.0f));
   m->ups.resize(c.n_upsampling_ratios);
   m->total_up = 1;
   for (int i = 0; i < c.n_upsampling_ratios; ++i) {
@@ -684,28 +648,28 @@ int build(CodecDecoder* m) {
     m->total_up *= f;
     const std::string p = "upsample." + std::to_string(i) + ".";
     CodecConvNeXt& U = m->ups[i];
-    S2S_CHECK(cslot(m, p + "0.conv.weight", &U.up_w, C_TCONV, H, H, f, f, sh));
-    S2S_CHECK(cslot(m, p + "0.conv.bias", &U.up_b, C_PLAIN, H, 0, 0, 0, 0.02f));
-    S2S_CHECK(cslot(m, p + "1.dwconv.conv.weight", &U.dw_w, C_PLAIN, H, 7, 0, 0, 0.378f));
-    S2S_CHECK(cslot(m, p + "1.dwconv.conv.bias", &U.dw_b, C_PLAIN, H, 0, 0, 0, 0.02f));
-    S2S_CHECK(cslot(m, p + "1.norm.weight", &U.ln_w, C_PLAIN, H, 0, 0, 0, 0.1f, 1.0f));
-    S2S_CHECK(cslot(m, p + "1.norm.bias", &U.ln_b, C_PLAIN, H, 0, 0, 0, 0.05f));
-    S2S_CHECK(cslot(m, p + "1.pwconv1.weight", &U.pw1_w, C_LINEAR, 4 * H, H, 0, 0, sh));
-    S2S_CHECK(cslot(m, p + "1.pwconv1.bias", &U.pw1_b, C_PLAIN, 4 * H, 0, 0, 0, 0.02f));
-    S2S_CHECK(cslot(m, p + "1.pwconv2.weight", &U.pw2_w, C_LINEAR, H, 4 * H, 0, 0, 0.5f * sh));
-    S2S_CHECK(cslot(m, p + "1.pwconv2.bias", &U.pw2_b, C_PLAIN, H, 0, 0, 0, 0.02f));
-    S2S_CHECK(cslot(m, p + "1.gamma", &U.gamma, C_PLAIN, H, 0, 0, 0, 0.05f, 0.3f));
+    S2S_CHECK(slot(p + "0.conv.weight", &U.up_w, W_TCONV, H, H, f, f, sh));
+    S2S_CHECK(slot(p + "0.conv.bias", &U.up_b, W_PLAIN, H, 0, 0, 0, 0.02f));
+    S2S_CHECK(slot(p + "1.dwconv.conv.weight", &U.dw_w, W_PLAIN, H, 7, 0, 0, 0.378f));
+    S2S_CHECK(slot(p + "1.dwconv.conv.bias", &U.dw_b, W_PLAIN, H, 0, 0, 0, 0.02f));
+    S2S_CHECK(slot(p + "1.norm.weight", &U.ln_w, W_PLAIN, H, 0, 0, 0, 0.1f, 1.0f));
+    S2S_CHECK(slot(p + "1.norm.bias", &U.ln_b, W_PLAIN, H, 0, 0, 0, 0.05f));
+    S2S_CHECK(slot(p + "1.pwconv1.weight", &U.pw1_w, W_LINEAR, 4 * H, H, 0, 0, sh));
+    S2S_CHECK(slot(p + "1.pwconv1.bias", &U.pw1_b, W_PLAIN, 4 * H, 0, 0, 0, 0.02f));
+    S2S_CHECK(slot(p + "1.pwconv2.weight", &U.pw2_w, W_LINEAR, H, 4 * H, 0, 0, 0.5f * sh));
+    S2S_CHECK(slot(p + "1.pwconv2.bias", &U.pw2_b, W_PLAIN, H, 0, 0, 0, 0.02f));
+    S2S_CHECK(slot(p + "1.gamma", &U.gamma, W_PLAIN, H, 0, 0, 0, 0.05f, 0.3f));
     tc_register(m, U.up_w, 1, H, f * H); tc_register(m, U.pw1_w, 1, H, 4 * H); tc_register(m, U.pw2_w, 1, 4 * H, H);
   }
   const int D = c.decoder_dim;
-  S2S_CHECK(cslot(m, "decoder.0.conv.weight", &m->d0_w, C_CONV, D, H, 7, 0, 1.0f / sqrtf(7.0f * H)));
-  S2S_CHECK(cslot(m, "decoder.0.conv.bias", &m->d0_b, C_PLAIN, D, 0, 0, 0, 0.02f));
+  S2S_CHECK(slot("decoder.0.conv.weight", &m->d0_w, W_CONV, D, H, 7, 0, 1.0f / sqrtf(7.0f * H)));
+  S2S_CHECK(slot("decoder.0.conv.bias", &m->d0_b, W_PLAIN, D, 0, 0, 0, 0.02f));
   tc_register(m, m->d0_w, 7, H, D);
   m->blocks.resize(c.n_upsample_rates);
   auto snake = [&](const std::string& pa, const std::string& pb, float** a, float** b, int n) -> int {
-    S2S_CHECK(cslot(m, pa, a, C_PLAIN, n, 0, 0, 0, 0.2f));
-    S2S_CHECK(cslot(m, pb, b, C_PLAIN, n, 0, 0, 0, 0.2f));
-    m->snake_pairs.push_back({&m->slots[pa], &m->slots[pb]});   // unordered_map element addresses are stable
+    S2S_CHECK(slot(pa, a, W_PLAIN, n, 0, 0, 0, 0.2f));
+    S2S_CHECK(slot(pb, b, W_PLAIN, n, 0, 0, 0, 0.2f));
+    m->snake_pairs.push_back({A.find(pa), A.find(pb)});   // unordered_map element addresses are stable
     return S2S_OK;
   };
   for (int i = 0; i < c.n_upsample_rates; ++i) {
@@ -714,26 +678,25 @@ int build(CodecDecoder* m) {
     m->total_up *= B.rate;
     const std::string p = "decoder." + std::to_string(i + 1) + ".block.";
     S2S_CHECK(snake(p + "0.alpha", p + "0.beta", &B.a0, &B.b0, B.cin));
-    S2S_CHECK(cslot(m, p + "1.conv.weight", &B.tc_w, C_TCONV, B.cin, B.cout, 2 * B.rate, B.rate, 1.0f / sqrtf(2.0f * B.cin)));
-    S2S_CHECK(cslot(m, p + "1.conv.bias", &B.tc_b, C_PLAIN, B.cout, 0, 0, 0, 0.02f));
+    S2S_CHECK(slot(p + "1.conv.weight", &B.tc_w, W_TCONV, B.cin, B.cout, 2 * B.rate, B.rate, 1.0f / sqrtf(2.0f * B.cin)));
+    S2S_CHECK(slot(p + "1.conv.bias", &B.tc_b, W_PLAIN, B.cout, 0, 0, 0, 0.02f));
     tc_register(m, B.tc_w, 2, B.cin, B.rate * B.cout);
     for (int u = 0; u < 3; ++u) {
       const std::string q = p + std::to_string(u + 2) + ".";
       CodecResUnit& R = B.u[u];
       S2S_CHECK(snake(q + "act1.alpha", q + "act1.beta", &R.a1, &R.b1, B.cout));
-      S2S_CHECK(cslot(m, q + "conv1.conv.weight", &R.c1_w, C_CONV, B.cout, B.cout, 7, 0, 1.0f / sqrtf(7.0f * B.cout)));
-      S2S_CHECK(cslot(m, q + "conv1.conv.bias", &R.c1_b, C_PLAIN, B.cout, 0, 0, 0, 0.02f));
+      S2S_CHECK(slot(q + "conv1.conv.weight", &R.c1_w, W_CONV, B.cout, B.cout, 7, 0, 1.0f / sqrtf(7.0f * B.cout)));
+      S2S_CHECK(slot(q + "conv1.conv.bias", &R.c1_b, W_PLAIN, B.cout, 0, 0, 0, 0.02f));
       S2S_CHECK(snake(q + "act2.alpha", q + "act2.beta", &R.a2, &R.b2, B.cout));
-      S2S_CHECK(cslot(m, q + "conv2.conv.weight", &R.c2_w, C_CONV, B.cout, B.cout, 1, 0, 1.0f / sqrtf((float)B.cout)));
-      S2S_CHECK(cslot(m, q + "conv2.conv.bias", &R.c2_b, C_PLAIN, B.cout, 0, 0, 0, 0.02f));
+      S2S_CHECK(slot(q + "conv2.conv.weight", &R.c2_w, W_CONV, B.cout, B.cout, 1, 0, 1.0f / sqrtf((float)B.cout)));
+      S2S_CHECK(slot(q + "conv2.conv.bias", &R.c2_b, W_PLAIN, B.cout, 0, 0, 0, 0.02f));
       tc_register(m, R.c1_w, 7, B.cout, B.cout); tc_register(m, R.c2_w, 1, B.cout, B.cout);
     }
   }
   const int n = c.n_upsample_rates, cl = D >> n;
   S2S_CHECK(snake("decoder." + std::to_string(n + 1) + ".alpha", "decoder." + std::to_string(n + 1) + ".beta", &m->fa, &m->fb, cl));
-  S2S_CHECK(cslot(m, "decoder." + std::to_string(n + 2) + ".conv.weight", &m->f_w, C_CONV, 1, cl, 7, 0, 0.5f / sqrtf(7.0f * cl)));
-  S2S_CHECK(cslot(m, "decoder." + std::to_string(n + 2) + ".conv.bias", &m->f_b, C_PLAIN, 1, 0, 0, 0, 0.02f));
-  (void)dummy;
+  S2S_CHECK(slot("decoder." + std::to_string(n + 2) + ".conv.weight", &m->f_w, W_CONV, 1, cl, 7, 0, 0.5f / sqrtf(7.0f * cl)));
+  S2S_CHECK(slot("decoder." + std::to_string(n + 2) + ".conv.bias", &m->f_b, W_PLAIN, 1, 0, 0, 0, 0.02f));
   // workspace for max_batch sequences of max_frames
   const int T = c.max_frames * (c.max_batch > 0 ? c.max_batch : 1);
   std::vector<int> L;
@@ -744,15 +707,15 @@ int build(CodecDecoder* m) {
   for (int i = 0; i < c.n_upsample_rates; ++i) mx = std::max(mx, (size_t)L[i + 1] * (size_t)(D >> (i + 1)));
   mx = std::max(mx, (size_t)L[0] * (size_t)D);
   m->buf_elems = mx;
-  S2S_CHECK(calloc_f(m, &m->bufX, mx));
-  S2S_CHECK(calloc_f(m, &m->bufA, mx));
-  S2S_CHECK(calloc_f(m, &m->bufH, mx));
-  S2S_CHECK(calloc_f(m, &m->x, (size_t)T * H));
-  S2S_CHECK(calloc_f(m, &m->xn, (size_t)T * H));
-  S2S_CHECK(calloc_f(m, &m->qkv, (size_t)T * (qd + 2 * kvd)));
-  S2S_CHECK(calloc_f(m, &m->att, (size_t)T * qd));
-  S2S_CHECK(calloc_f(m, &m->gu, (size_t)T * 2 * I));
-  S2S_CHECK(calloc_f(m, &m->hmid, (size_t)T * I));
+  S2S_CHECK(A.alloc(&m->bufX, mx * 4));
+  S2S_CHECK(A.alloc(&m->bufA, mx * 4));
+  S2S_CHECK(A.alloc(&m->bufH, mx * 4));
+  S2S_CHECK(A.alloc(&m->x, (size_t)T * H * 4));
+  S2S_CHECK(A.alloc(&m->xn, (size_t)T * H * 4));
+  S2S_CHECK(A.alloc(&m->qkv, (size_t)T * (qd + 2 * kvd) * 4));
+  S2S_CHECK(A.alloc(&m->att, (size_t)T * qd * 4));
+  S2S_CHECK(A.alloc(&m->gu, (size_t)T * 2 * I * 4));
+  S2S_CHECK(A.alloc(&m->hmid, (size_t)T * I * 4));
   return S2S_OK;
 }
 
@@ -830,94 +793,33 @@ int codec_create(s2s_ctx* ctx, const s2s_codec_config* cfg, CodecDecoder** out) 
 
 int codec_destroy(CodecDecoder* m) {
   if (!m) return S2S_OK;
-  for (void* p : m->allocs) cudaFree(p);
   delete m;
   return S2S_OK;
 }
 
 int codec_bind_tensor(CodecDecoder* m, const char* name, const void* data_h, const int64_t* shape, int ndim, int dtype) {
   S2S_REQUIRE(m && name && data_h && shape, "codec bind_tensor: null argument");
-  auto it = m->slots.find(name);
-  if (it == m->slots.end()) { s2s_set_error("codec bind_tensor: unknown tensor '%s'", name); return S2S_ERR_NOT_FOUND; }
-  CSlot& s = it->second;
-  int64_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= shape[i];
-  S2S_REQUIRE(n == s.n, "codec bind_tensor: '%s' has %lld elements, expected %lld", name, (long long)n, (long long)s.n);
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  if (s.kind == C_LINEAR && s.d2 > 0) {
-    // column block [col0, col0 + N) of a shared [K][N_total] matrix: one strided 2-D copy
-    const int N = s.d0, K = s.d1, Nt = s.d2, col0 = s.stride;
-    std::vector<float> tmp((size_t)K * N);
-    for (int nn = 0; nn < N; ++nn)
-      for (int k = 0; k < K; ++k) tmp[(size_t)k * N + nn] = src_f32(data_h, (int64_t)nn * K + k, dtype);
-    S2S_CHECK_CUDA(cudaMemcpy2D(s.dst + col0, (size_t)Nt * 4, tmp.data(), (size_t)N * 4, (size_t)N * 4, K, cudaMemcpyHostToDevice));
-    s.bound = s.raw = true;
-    return S2S_OK;
-  }
-  std::vector<float> tmp((size_t)n);
-  if (s.kind == C_LINEAR) {
-    const int N = s.d0, K = s.d1;
-    for (int nn = 0; nn < N; ++nn)
-      for (int k = 0; k < K; ++k) tmp[(size_t)k * N + nn] = src_f32(data_h, (int64_t)nn * K + k, dtype);
-  } else if (s.kind == C_CONV) {
-    const int O = s.d0, C = s.d1, k = s.d2;
-    for (int o = 0; o < O; ++o)
-      for (int c = 0; c < C; ++c)
-        for (int j = 0; j < k; ++j) tmp[((size_t)j * C + c) * O + o] = src_f32(data_h, ((int64_t)o * C + c) * k + j, dtype);
-  } else if (s.kind == C_TCONV) {
-    // [C, O, k] with k = s or 2 s.  k = s: one tap, W'[c][r * O + o] = W[c][o][r].
-    // k = 2 s: tap 0 multiplies X[t0 - 1] -> W[c][o][r + s]; tap 1 multiplies X[t0] -> W[c][o][r].
-    const int C = s.d0, O = s.d1, k = s.d2, st = s.stride, taps = k / st;
-    for (int c = 0; c < C; ++c)
-      for (int o = 0; o < O; ++o)
-        for (int r = 0; r < st; ++r) {
-          if (taps == 1) tmp[(size_t)c * st * O + (size_t)r * O + o] = src_f32(data_h, ((int64_t)c * O + o) * k + r, dtype);
-          else {
-            tmp[((size_t)0 * C + c) * st * O + (size_t)r * O + o] = src_f32(data_h, ((int64_t)c * O + o) * k + r + st, dtype);
-            tmp[((size_t)1 * C + c) * st * O + (size_t)r * O + o] = src_f32(data_h, ((int64_t)c * O + o) * k + r, dtype);
-          }
-        }
-  } else {
-    for (int64_t i = 0; i < n; ++i) tmp[(size_t)i] = src_f32(data_h, i, dtype);
-  }
-  S2S_CHECK_CUDA(cudaMemcpy(s.dst, tmp.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
-  s.bound = s.raw = true;
-  return S2S_OK;
+  return m->arena.bind("codec", name, data_h, shape, ndim, dtype, S2S_F32);
 }
 
 int codec_init_random(CodecDecoder* m, uint64_t seed) {
   S2S_REQUIRE(m, "codec init_random: null model");
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  for (auto& kv : m->slots) {
-    CSlot& s = kv.second;
-    uint64_t hsh = 1469598103934665603ull;
-    for (char ch : kv.first) hsh = (hsh ^ (uint64_t)(unsigned char)ch) * 1099511628211ull;
-    if (s.kind == C_LINEAR && s.d2 > 0) {
-      // column block of a shared matrix: fill row by row
-      std::vector<float> tmp((size_t)s.d0 * s.d1);
-      uint64_t st = seed ^ hsh;
-      for (auto& v : tmp) { st = st * 6364136223846793005ull + 1442695040888963407ull; v = s.rnd_scale * (((st >> 40) & 0xffff) / 32768.0f - 1.0f); }
-      S2S_CHECK_CUDA(cudaMemcpy2D(s.dst + s.stride, (size_t)s.d2 * 4, tmp.data(), (size_t)s.d0 * 4, (size_t)s.d0 * 4, s.d1, cudaMemcpyHostToDevice));
-    } else {
-      S2S_CHECK(fill_random_launch(s.dst, s.n, S2S_F32, s.rnd_scale, s.rnd_offset, seed ^ hsh, 0));
-    }
-    s.bound = s.raw = true;
-  }
-  S2S_CHECK_CUDA(cudaDeviceSynchronize());
-  return S2S_OK;
+  return m->arena.init_random(seed, S2S_F32);
 }
 
 int codec_finalize(CodecDecoder* m) {
   S2S_REQUIRE(m, "codec finalize: null model");
-  for (auto& kv : m->slots)
-    if (!kv.second.bound) { s2s_set_error("codec finalize: tensor '%s' was never bound", kv.first.c_str()); return S2S_ERR_INVALID; }
+  S2S_CHECK(m->arena.check_all_bound("codec"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   // SnakeBeta parameters -> (exp(alpha), 1 / (exp(beta) + 1e-9)): exactly those written since the last finalize, so a
   // reload (or a partial one) leaves every buffer transformed once
   for (auto& p : m->snake_pairs) {
-    CSlot &sa = *p.first, &sb = *p.second;
+    WeightSlot &sa = *p.first, &sb = *p.second;
     if (!sa.raw && !sb.raw) continue;
-    exp_prep_kernel<<<(unsigned)((sa.n + 255) / 256), 256>>>(sa.raw ? sa.dst : nullptr, sb.raw ? sb.dst : nullptr, (int)sa.n);
+    exp_prep_kernel<<<(unsigned)((sa.n + 255) / 256), 256>>>(sa.raw ? (float*)sa.dst : nullptr, sb.raw ? (float*)sb.dst : nullptr,
+                                                             (int)sa.n);
     S2S_LAUNCH_CHECK();
     sa.raw = sb.raw = false;
   }
@@ -925,10 +827,7 @@ int codec_finalize(CodecDecoder* m) {
   for (auto& kv : m->tc_w) {
     CodecDecoder::TcW& t = kv.second;
     const size_t words = (size_t)t.k * ((t.C_in + 1) / 2) * t.N;
-    if (!t.packed) {
-      S2S_CHECK_CUDA(cudaMalloc(&t.packed, words * 4));
-      m->allocs.push_back(t.packed);
-    }
+    if (!t.packed) S2S_CHECK(m->arena.alloc(&t.packed, words * 4, false));
     pack_weight_pairs_kernel<<<(unsigned)std::min<size_t>((words + 255) / 256, 4096), 256>>>(kv.first, t.k, t.C_in, t.N,
                                                                                                reinterpret_cast<__half2*>(t.packed));
     S2S_LAUNCH_CHECK();

@@ -13,7 +13,6 @@
 #include <string.h>
 
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "common.cuh"
@@ -122,42 +121,7 @@ __global__ void seen_set_kernel(const int* __restrict__ ids, int n, unsigned int
   if (i < n) atomicOr(seen + (ids[i] >> 5), 1u << (ids[i] & 31));
 }
 
-inline uint16_t f2h(float f) { __half h = __float2half_rn(f); uint16_t u; memcpy(&u, &h, 2); return u; }
-inline uint16_t f2bf(float f) {
-  uint32_t u; memcpy(&u, &f, 4);
-  if ((u & 0x7fffffffu) > 0x7f800000u) return 0x7fc0;
-  u += 0x7fffu + ((u >> 16) & 1u);
-  return (uint16_t)(u >> 16);
-}
-inline float src_f32(const void* data, int64_t i, int dtype) {
-  if (dtype == S2S_F32) return reinterpret_cast<const float*>(data)[i];
-  uint16_t u = reinterpret_cast<const uint16_t*>(data)[i];
-  if (dtype == S2S_BF16) { uint32_t w = (uint32_t)u << 16; float f; memcpy(&f, &w, 4); return f; }
-  __half h; memcpy(&h, &u, 2); return __half2float(h);
-}
-
-}  // namespace
-
-namespace {
-
 constexpr int MAX_DEC_B = LLAMA_MAX_DEC_B;
-
-template <typename P> int lalloc(s2s_llama* m, P** out, size_t bytes, bool zero = true) {
-  void* p = nullptr;
-  S2S_CHECK_CUDA(cudaMalloc(&p, bytes ? bytes : 16));
-  if (zero) S2S_CHECK_CUDA(cudaMemset(p, 0, bytes ? bytes : 16));
-  m->allocs.push_back(p);
-  *out = reinterpret_cast<P*>(p);
-  return S2S_OK;
-}
-
-void lslot(s2s_llama* m, const std::string& name, void* dst, bool half, int64_t rows, int64_t cols, float rnd_scale,
-           float rnd_offset = 0.f, int kind = L_PLAIN, int hd = 0, int parity = 0) {
-  LSlot s;
-  s.dst = dst; s.half = half; s.rows = rows; s.cols = cols; s.kind = kind; s.hd = hd; s.parity = parity;
-  s.rnd_scale = rnd_scale; s.rnd_offset = rnd_offset;
-  m->slots[name] = s;
-}
 
 int build(s2s_llama* m) {
   const auto& c = m->cfg;
@@ -167,50 +131,51 @@ int build(s2s_llama* m) {
   m->n_tables = c.n_tables > 1 ? c.n_tables : 1;
   m->embed_table_elems = (size_t)c.vocab * d;
   m->head_table_elems = (size_t)c.vocab * d;
-  S2S_CHECK(lalloc(m, &m->embed, m->n_tables * m->embed_table_elems * esz));
-  S2S_CHECK(lalloc(m, &m->lm_head, m->n_tables * m->head_table_elems * esz));
-  S2S_CHECK(lalloc(m, &m->norm_f, d * 4));
+  S2S_CHECK(m->arena.alloc(&m->embed, m->n_tables * m->embed_table_elems * esz));
+  S2S_CHECK(m->arena.alloc(&m->lm_head, m->n_tables * m->head_table_elems * esz));
+  S2S_CHECK(m->arena.alloc(&m->norm_f, d * 4));
+  WeightArena& A = m->arena;
   if (m->n_tables == 1) {
-    lslot(m, "model.embed_tokens.weight", m->embed, true, c.vocab, d, 0.02f);
-    lslot(m, "lm_head.weight", m->lm_head, true, c.vocab, d, 0.02f);
+    A.add("model.embed_tokens.weight", m->embed, true, (int64_t)c.vocab * d);
+    A.add("lm_head.weight", m->lm_head, true, (int64_t)c.vocab * d);
   } else {  // code predictor: one table / head per codebook (Qwen3OmniMoeTalkerCodePredictorModel.codec_embedding, .lm_head)
     for (int t = 0; t < m->n_tables; ++t) {
-      lslot(m, "model.embed_tokens." + std::to_string(t) + ".weight", off(m->embed, (int64_t)t * m->embed_table_elems), true, c.vocab, d, 0.02f);
-      lslot(m, "lm_head." + std::to_string(t) + ".weight", off(m->lm_head, (int64_t)t * m->head_table_elems), true, c.vocab, d, 0.02f);
+      A.add("model.embed_tokens." + std::to_string(t) + ".weight", off(m->embed, (int64_t)t * m->embed_table_elems), true, (int64_t)c.vocab * d);
+      A.add("lm_head." + std::to_string(t) + ".weight", off(m->lm_head, (int64_t)t * m->head_table_elems), true, (int64_t)c.vocab * d);
     }
   }
-  lslot(m, "model.norm.weight", m->norm_f, false, d, 1, 0.1f, 1.0f);
+  A.add("model.norm.weight", m->norm_f, false, d, 0.1f, 1.0f);
   m->layers_h.resize(c.layers);
   const float sd = 1.0f / sqrtf((float)d);
   for (int i = 0; i < c.layers; ++i) {
     const std::string p = "model.layers." + std::to_string(i) + ".";
     void *w_qkv, *w_o, *w_gu, *w_down;
     float *n1, *n2, *qn = nullptr, *kn = nullptr;
-    S2S_CHECK(lalloc(m, &w_qkv, (size_t)(qd + 2 * kvd) * d * esz));
-    S2S_CHECK(lalloc(m, &w_o, (size_t)d * qd * esz));
-    S2S_CHECK(lalloc(m, &w_gu, (size_t)2 * f * d * esz));
-    S2S_CHECK(lalloc(m, &w_down, (size_t)d * f * esz));
-    S2S_CHECK(lalloc(m, &n1, d * 4));
-    S2S_CHECK(lalloc(m, &n2, d * 4));
-    lslot(m, p + "self_attn.q_proj.weight", w_qkv, true, qd, d, 2.0f * sd, 0.f, L_ROPE_PERM, hd);
-    lslot(m, p + "self_attn.k_proj.weight", off(w_qkv, (int64_t)qd * d), true, kvd, d, 2.0f * sd, 0.f, L_ROPE_PERM, hd);
-    lslot(m, p + "self_attn.v_proj.weight", off(w_qkv, (int64_t)(qd + kvd) * d), true, kvd, d, 0.8f * sd);
-    lslot(m, p + "self_attn.o_proj.weight", w_o, true, d, qd, 1.0f * sd);
-    lslot(m, p + "mlp.gate_proj.weight", w_gu, true, f, d, 1.0f * sd, 0.f, L_INTERLEAVE, 0, 0);
-    lslot(m, p + "mlp.up_proj.weight", w_gu, true, f, d, 1.0f * sd, 0.f, L_INTERLEAVE, 0, 1);
-    lslot(m, p + "mlp.down_proj.weight", w_down, true, d, f, 0.7f / sqrtf((float)f));
-    lslot(m, p + "input_layernorm.weight", n1, false, d, 1, 0.1f, 1.0f);
-    lslot(m, p + "post_attention_layernorm.weight", n2, false, d, 1, 0.1f, 1.0f);
+    S2S_CHECK(A.alloc(&w_qkv, (size_t)(qd + 2 * kvd) * d * esz));
+    S2S_CHECK(A.alloc(&w_o, (size_t)d * qd * esz));
+    S2S_CHECK(A.alloc(&w_gu, (size_t)2 * f * d * esz));
+    S2S_CHECK(A.alloc(&w_down, (size_t)d * f * esz));
+    S2S_CHECK(A.alloc(&n1, d * 4));
+    S2S_CHECK(A.alloc(&n2, d * 4));
+    A.add(p + "self_attn.q_proj.weight", w_qkv, true, (int64_t)qd * d, 2.0f * sd).as(W_ROPE_PERM, qd, d, 0, hd);
+    A.add(p + "self_attn.k_proj.weight", off(w_qkv, (int64_t)qd * d), true, (int64_t)kvd * d, 2.0f * sd).as(W_ROPE_PERM, kvd, d, 0, hd);
+    A.add(p + "self_attn.v_proj.weight", off(w_qkv, (int64_t)(qd + kvd) * d), true, (int64_t)kvd * d, 0.8f * sd);
+    A.add(p + "self_attn.o_proj.weight", w_o, true, (int64_t)d * qd, 1.0f * sd);
+    A.add(p + "mlp.gate_proj.weight", w_gu, true, (int64_t)f * d, 1.0f * sd).as(W_INTERLEAVE, f, d, 0, 0);
+    A.add(p + "mlp.up_proj.weight", w_gu, true, (int64_t)f * d, 1.0f * sd).as(W_INTERLEAVE, f, d, 0, 1);
+    A.add(p + "mlp.down_proj.weight", w_down, true, (int64_t)d * f, 0.7f / sqrtf((float)f));
+    A.add(p + "input_layernorm.weight", n1, false, d, 0.1f, 1.0f);
+    A.add(p + "post_attention_layernorm.weight", n2, false, d, 0.1f, 1.0f);
     if (c.qk_norm) {  // Qwen3Attention.q_norm / k_norm: RMSNorm(head_dim), permuted like the q/k rows
-      S2S_CHECK(lalloc(m, &qn, hd * 4));
-      S2S_CHECK(lalloc(m, &kn, hd * 4));
-      lslot(m, p + "self_attn.q_norm.weight", qn, false, hd, 1, 0.1f, 1.0f, L_ROPE_PERM, hd);
-      lslot(m, p + "self_attn.k_norm.weight", kn, false, hd, 1, 0.1f, 1.0f, L_ROPE_PERM, hd);
+      S2S_CHECK(A.alloc(&qn, hd * 4));
+      S2S_CHECK(A.alloc(&kn, hd * 4));
+      A.add(p + "self_attn.q_norm.weight", qn, false, hd, 0.1f, 1.0f).as(W_ROPE_PERM, hd, 1, 0, hd);
+      A.add(p + "self_attn.k_norm.weight", kn, false, hd, 0.1f, 1.0f).as(W_ROPE_PERM, hd, 1, 0, hd);
     }
     LlamaDecLayer& L = m->layers_h[i];
     L.w_qkv = w_qkv; L.w_o = w_o; L.w_gu = w_gu; L.w_down = w_down; L.norm1 = n1; L.norm2 = n2; L.q_norm = qn; L.k_norm = kn;
   }
-  S2S_CHECK(lalloc(m, &m->layers_d, sizeof(LlamaDecLayer) * c.layers));
+  S2S_CHECK(m->arena.alloc(&m->layers_d, sizeof(LlamaDecLayer) * c.layers));
   S2S_CHECK_CUDA(cudaMemcpy(m->layers_d, m->layers_h.data(), sizeof(LlamaDecLayer) * c.layers, cudaMemcpyHostToDevice));
 
   // RoPE table, float32 arithmetic like LlamaRotaryEmbedding (modeling_llama.py:73-137)
@@ -223,54 +188,54 @@ int build(s2s_llama* m) {
         tab[(size_t)p * (hd / 2) + j] = make_float2(cosf(ang), sinf(ang));
       }
     }
-    S2S_CHECK(lalloc(m, &m->rope, tab.size() * sizeof(float2)));
+    S2S_CHECK(m->arena.alloc(&m->rope, tab.size() * sizeof(float2)));
     S2S_CHECK_CUDA(cudaMemcpy(m->rope, tab.data(), tab.size() * sizeof(float2), cudaMemcpyHostToDevice));
   }
   // KV cache [slot][layer][2][max_pos][kvd]
   m->kv_which_stride = (long long)c.max_positions * kvd;
   m->kv_layer_stride = 2 * m->kv_which_stride;
   m->kv_slot_stride = (long long)c.layers * m->kv_layer_stride;
-  S2S_CHECK(lalloc(m, &m->kv, (size_t)c.max_sessions * m->kv_slot_stride * esz));
+  S2S_CHECK(m->arena.alloc(&m->kv, (size_t)c.max_sessions * m->kv_slot_stride * esz));
   m->len.assign(c.max_sessions, 0);
   // prefill workspace
   const int P = c.max_prefill;
-  S2S_CHECK(lalloc(m, &m->ids_d, (size_t)P * 4));
-  S2S_CHECK(lalloc(m, &m->x, (size_t)P * d * 4));
-  S2S_CHECK(lalloc(m, &m->xn, (size_t)P * d * esz));
-  S2S_CHECK(lalloc(m, &m->qkv, (size_t)P * (qd + 2 * kvd) * esz));
-  S2S_CHECK(lalloc(m, &m->attn, (size_t)P * qd * esz));
-  S2S_CHECK(lalloc(m, &m->hbuf, (size_t)P * f * esz));
-  S2S_CHECK(lalloc(m, &m->last_logits, (size_t)c.vocab * 4));
-  S2S_CHECK(lalloc(m, &m->batch_logits, (size_t)MAX_DEC_B * c.vocab * 4));
+  S2S_CHECK(m->arena.alloc(&m->ids_d, (size_t)P * 4));
+  S2S_CHECK(m->arena.alloc(&m->x, (size_t)P * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->xn, (size_t)P * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->qkv, (size_t)P * (qd + 2 * kvd) * esz));
+  S2S_CHECK(m->arena.alloc(&m->attn, (size_t)P * qd * esz));
+  S2S_CHECK(m->arena.alloc(&m->hbuf, (size_t)P * f * esz));
+  S2S_CHECK(m->arena.alloc(&m->last_logits, (size_t)c.vocab * 4));
+  S2S_CHECK(m->arena.alloc(&m->batch_logits, (size_t)MAX_DEC_B * c.vocab * 4));
   m->vt_elems = attention_tc_scratch_elems(1, c.max_positions, c.kv_heads, hd);
-  S2S_CHECK(lalloc(m, &m->vt, m->vt_elems * esz));
+  S2S_CHECK(m->arena.alloc(&m->vt, m->vt_elems * esz));
   // decode state
   m->s_max = (c.max_positions + 63) / 64;
   const int grid = m->ctx->num_sms;
-  S2S_CHECK(lalloc(m, &m->dx, (size_t)MAX_DEC_B * d * 4));
-  S2S_CHECK(lalloc(m, &m->dq, (size_t)MAX_DEC_B * qd * 4));
-  S2S_CHECK(lalloc(m, &m->dh, (size_t)MAX_DEC_B * f * 4));
-  S2S_CHECK(lalloc(m, &m->part, (size_t)MAX_DEC_B * c.heads * m->s_max * (hd + 4) * 4));
-  S2S_CHECK(lalloc(m, &m->attn16, (size_t)MAX_DEC_B * qd * 2));
-  S2S_CHECK(lalloc(m, &m->attn_cnt, (size_t)MAX_DEC_B * c.heads * 4));
-  S2S_CHECK(lalloc(m, &m->slot_d, MAX_DEC_B * 4));
-  S2S_CHECK(lalloc(m, &m->pos_d, MAX_DEC_B * 4));
-  S2S_CHECK(lalloc(m, &m->done, MAX_DEC_B * 4));
-  S2S_CHECK(lalloc(m, &m->n_done, 16));
-  S2S_CHECK(lalloc(m, &m->cand_val, (size_t)MAX_DEC_B * grid * 4));
-  S2S_CHECK(lalloc(m, &m->cand_idx, (size_t)MAX_DEC_B * grid * 4));
-  S2S_CHECK(lalloc(m, &m->out_ids, (size_t)MAX_DEC_B * c.max_positions * 4));
-  S2S_CHECK(lalloc(m, &m->out_len, MAX_DEC_B * 4));
-  S2S_CHECK(lalloc(m, &m->next_id, 16));
-  S2S_CHECK(lalloc(m, &m->sync_counter, 16));
-  S2S_CHECK(lalloc(m, &m->kraw, (size_t)MAX_DEC_B * kvd * 4));
-  S2S_CHECK(lalloc(m, &m->qn, (size_t)MAX_DEC_B * qd * 4));
+  S2S_CHECK(m->arena.alloc(&m->dx, (size_t)MAX_DEC_B * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->dq, (size_t)MAX_DEC_B * qd * 4));
+  S2S_CHECK(m->arena.alloc(&m->dh, (size_t)MAX_DEC_B * f * 4));
+  S2S_CHECK(m->arena.alloc(&m->part, (size_t)MAX_DEC_B * c.heads * m->s_max * (hd + 4) * 4));
+  S2S_CHECK(m->arena.alloc(&m->attn16, (size_t)MAX_DEC_B * qd * 2));
+  S2S_CHECK(m->arena.alloc(&m->attn_cnt, (size_t)MAX_DEC_B * c.heads * 4));
+  S2S_CHECK(m->arena.alloc(&m->slot_d, MAX_DEC_B * 4));
+  S2S_CHECK(m->arena.alloc(&m->pos_d, MAX_DEC_B * 4));
+  S2S_CHECK(m->arena.alloc(&m->done, MAX_DEC_B * 4));
+  S2S_CHECK(m->arena.alloc(&m->n_done, 16));
+  S2S_CHECK(m->arena.alloc(&m->cand_val, (size_t)MAX_DEC_B * grid * 4));
+  S2S_CHECK(m->arena.alloc(&m->cand_idx, (size_t)MAX_DEC_B * grid * 4));
+  S2S_CHECK(m->arena.alloc(&m->out_ids, (size_t)MAX_DEC_B * c.max_positions * 4));
+  S2S_CHECK(m->arena.alloc(&m->out_len, MAX_DEC_B * 4));
+  S2S_CHECK(m->arena.alloc(&m->next_id, 16));
+  S2S_CHECK(m->arena.alloc(&m->sync_counter, 16));
+  S2S_CHECK(m->arena.alloc(&m->kraw, (size_t)MAX_DEC_B * kvd * 4));
+  S2S_CHECK(m->arena.alloc(&m->qn, (size_t)MAX_DEC_B * qd * 4));
   m->samp.assign(c.max_sessions, samp_greedy());
   m->seen_words = (c.vocab + 31) / 32;
   m->seen_stale.assign(c.max_sessions, 0);
-  S2S_CHECK(lalloc(m, &m->samp_d, MAX_DEC_B * sizeof(SampSlot)));
-  S2S_CHECK(lalloc(m, &m->samp_rows, (size_t)MAX_DEC_B * c.vocab * 4));
-  S2S_CHECK(lalloc(m, &m->seen, (size_t)c.max_sessions * m->seen_words * 4));
+  S2S_CHECK(m->arena.alloc(&m->samp_d, MAX_DEC_B * sizeof(SampSlot)));
+  S2S_CHECK(m->arena.alloc(&m->samp_rows, (size_t)MAX_DEC_B * c.vocab * 4));
+  S2S_CHECK(m->arena.alloc(&m->seen, (size_t)c.max_sessions * m->seen_words * 4));
   return S2S_OK;
 }
 
@@ -515,7 +480,6 @@ int s2s_llama_create(s2s_ctx* ctx, const s2s_llama_config* cfg, s2s_llama** out)
 
 int s2s_llama_destroy(s2s_llama* m) {
   if (!m) return S2S_OK;
-  for (void* p : m->allocs) cudaFree(p);
   delete m;
   return S2S_OK;
 }
@@ -523,46 +487,8 @@ int s2s_llama_destroy(s2s_llama* m) {
 int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, const int64_t* shape, int32_t ndim,
                           int32_t dtype) {
   S2S_REQUIRE(m && name && data_h && shape, "llama bind_tensor: null argument");
-  auto it = m->slots.find(name);
-  if (it == m->slots.end()) {
-    s2s_set_error("llama bind_tensor: unknown tensor '%s'", name);
-    return S2S_ERR_NOT_FOUND;
-  }
-  LSlot& s = it->second;
-  int64_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= shape[i];
-  S2S_REQUIRE(n == s.rows * s.cols, "llama bind_tensor: '%s' has %lld elements, expected %lld", name, (long long)n,
-              (long long)(s.rows * s.cols));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  const bool bf = m->cfg.compute_dtype == S2S_BF16;
-  if (!s.half) {
-    std::vector<float> tmp((size_t)n);
-    for (int64_t i = 0; i < n; ++i) {
-      int64_t di = i;
-      if (s.kind == L_ROPE_PERM) { const int64_t half = s.hd / 2, j = i % s.hd; di = (i / s.hd) * s.hd + (j < half ? 2 * j : 2 * (j - half) + 1); }
-      tmp[(size_t)di] = src_f32(data_h, i, dtype);
-    }
-    S2S_CHECK_CUDA(cudaMemcpy(s.dst, tmp.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
-  } else {
-    // row-wise conversion + placement
-    std::vector<uint16_t> rowbuf((size_t)s.cols);
-    for (int64_t r = 0; r < s.rows; ++r) {
-      for (int64_t c = 0; c < s.cols; ++c) {
-        const float v = src_f32(data_h, r * s.cols + c, dtype);
-        rowbuf[(size_t)c] = bf ? f2bf(v) : f2h(v);
-      }
-      int64_t dr = r;
-      if (s.kind == L_ROPE_PERM) {
-        const int64_t h = r / s.hd, j = r % s.hd, half = s.hd / 2;
-        dr = h * s.hd + (j < half ? 2 * j : 2 * (j - half) + 1);
-      } else if (s.kind == L_INTERLEAVE) {
-        dr = 2 * r + s.parity;
-      }
-      S2S_CHECK_CUDA(cudaMemcpy(reinterpret_cast<char*>(s.dst) + dr * s.cols * 2, rowbuf.data(), (size_t)s.cols * 2,
-                                cudaMemcpyHostToDevice));
-    }
-  }
-  s.bound = true;
+  S2S_CHECK(m->arena.bind("llama", name, data_h, shape, ndim, dtype, m->cfg.compute_dtype));
   if (strncmp(name, "lm_head.", 8) == 0) m->lm_head_bound = true;
   return S2S_OK;
 }
@@ -570,21 +496,8 @@ int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, co
 int s2s_llama_init_random(s2s_llama* m, uint64_t seed) {
   S2S_REQUIRE(m, "llama init_random: null model");
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  for (auto& kv : m->slots) {
-    LSlot& s = kv.second;
-    uint64_t hsh = 1469598103934665603ull;
-    for (char ch : kv.first) hsh = (hsh ^ (uint64_t)(unsigned char)ch) * 1099511628211ull;
-    if (s.kind == L_INTERLEAVE) {
-      if (s.parity == 1) { s.bound = true; continue; }  // gate slot fills the whole interleaved [2*ffn, d] block
-      S2S_CHECK(fill_random_launch(s.dst, 2 * s.rows * s.cols, m->cfg.compute_dtype, s.rnd_scale, 0.f, seed ^ hsh, 0));
-    } else {
-      S2S_CHECK(fill_random_launch(s.dst, s.rows * s.cols, s.half ? m->cfg.compute_dtype : S2S_F32, s.rnd_scale,
-                                   s.rnd_offset, seed ^ hsh, 0));
-    }
-    s.bound = true;
-  }
+  S2S_CHECK(m->arena.init_random(seed, m->cfg.compute_dtype));
   m->lm_head_bound = true;
-  S2S_CHECK_CUDA(cudaDeviceSynchronize());
   return S2S_OK;
 }
 
@@ -606,16 +519,12 @@ int32_t s2s_llama_weight_format(s2s_llama* m) { return m ? m->weight_format : S2
 
 int s2s_llama_finalize(s2s_llama* m) {
   S2S_REQUIRE(m, "llama finalize: null model");
-  if (m->n_tables == 1 && !m->lm_head_bound && m->slots["model.embed_tokens.weight"].bound) {
+  if (m->n_tables == 1 && !m->lm_head_bound && m->arena.find("model.embed_tokens.weight")->bound) {
     // tied embeddings (tie_word_embeddings=True): lm_head shares embed_tokens
     S2S_CHECK_CUDA(cudaMemcpy(m->lm_head, m->embed, (size_t)m->cfg.vocab * m->cfg.d_model * 2, cudaMemcpyDeviceToDevice));
-    m->slots["lm_head.weight"].bound = true;
+    m->arena.find("lm_head.weight")->bound = true;
   }
-  for (auto& kv : m->slots)
-    if (!kv.second.bound) {
-      s2s_set_error("llama finalize: tensor '%s' was never bound", kv.first.c_str());
-      return S2S_ERR_INVALID;
-    }
+  S2S_CHECK(m->arena.check_all_bound("llama"));
   // decode-side weight layout: fragment-major tiles (weight_tiles.cu), built once per (re)load.  FP8: the tiles hold E4M3
   // codes + row scales and the row-major matrices become the dequantised values, so prefill and decode share one model.
   {
@@ -633,14 +542,14 @@ int s2s_llama_finalize(s2s_llama* m) {
       for (int i = 0; i < c.layers; ++i) {
         LlamaDecLayer& T = m->tiled_h[i];
         void *a, *b, *g, *dn;
-        S2S_CHECK(lalloc(m, &a, tbytes(qd + 2 * kvd, d)));
-        S2S_CHECK(lalloc(m, &b, tbytes(d, qd)));
-        S2S_CHECK(lalloc(m, &g, tbytes(2 * f, d)));
-        S2S_CHECK(lalloc(m, &dn, tbytes(d, f)));
+        S2S_CHECK(m->arena.alloc(&a, tbytes(qd + 2 * kvd, d)));
+        S2S_CHECK(m->arena.alloc(&b, tbytes(d, qd)));
+        S2S_CHECK(m->arena.alloc(&g, tbytes(2 * f, d)));
+        S2S_CHECK(m->arena.alloc(&dn, tbytes(d, f)));
         T.w_qkv = a; T.w_o = b; T.w_gu = g; T.w_down = dn;
       }
       m->head_t_table_elems = tiled_weight_elems(c.vocab, d);
-      S2S_CHECK(lalloc(m, &m->lm_head_t, f8 ? tbytes(c.vocab, d) : m->n_tables * m->head_t_table_elems * 2));
+      S2S_CHECK(m->arena.alloc(&m->lm_head_t, f8 ? tbytes(c.vocab, d) : m->n_tables * m->head_t_table_elems * 2));
       S2S_CHECK_CUDA(cudaMemcpy(m->layers_d, m->tiled_h.data(), sizeof(LlamaDecLayer) * c.layers, cudaMemcpyHostToDevice));
     }
     for (int i = 0; i < c.layers; ++i) {

@@ -1,24 +1,11 @@
 // llama_model.cuh -- the Llama-family model object (internal to libs2s_b200): shared by llama.cu (C ABI of the LLM slot)
 // and qwen3tts.cu (Qwen3-TTS talker and code predictor are Qwen3-style decoders driven by embeddings).
 #pragma once
-#include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "common.cuh"
 #include "llama_decode.cuh"
-
-enum LSlotKind { L_PLAIN = 0, L_ROPE_PERM = 1, L_INTERLEAVE = 2 };
-struct LSlot {
-  void* dst = nullptr;
-  bool half = false;
-  int64_t rows = 0, cols = 0;
-  int kind = L_PLAIN;
-  int hd = 0;          // ROPE_PERM
-  int parity = 0;      // INTERLEAVE: 0 gate, 1 up
-  bool bound = false;
-  float rnd_scale = 0.02f, rnd_offset = 0.f;
-};
+#include "weight_arena.cuh"
 
 struct s2s_llama {
   s2s_ctx* ctx = nullptr;
@@ -26,8 +13,7 @@ struct s2s_llama {
   bool finalized = false;
   int weight_format = 0;                 // storage of the matrices the decode launch streams: cfg.compute_dtype, or S2S_FP8_E4M3
   int debug_phases = 0;
-  std::vector<void*> allocs;
-  std::unordered_map<std::string, LSlot> slots;
+  WeightArena arena;
   bool lm_head_bound = false;
   // weights
   void *embed = nullptr, *lm_head = nullptr;

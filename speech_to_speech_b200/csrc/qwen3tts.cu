@@ -27,6 +27,7 @@
 #include "codec_decode.cuh"
 #include "kernels.cuh"
 #include "llama_model.cuh"
+#include "weight_arena.cuh"
 
 extern "C" {
 int s2s_llama_create(s2s_ctx* ctx, const s2s_llama_config* cfg, s2s_llama** out);
@@ -147,20 +148,6 @@ __global__ void frame_finish_kernel(TtsBatch tb, int f, int n_frames, int G, con
   }
 }
 
-inline float src_f32(const void* data, int64_t i, int dtype) {
-  if (dtype == S2S_F32) return reinterpret_cast<const float*>(data)[i];
-  uint16_t u = reinterpret_cast<const uint16_t*>(data)[i];
-  if (dtype == S2S_BF16) { uint32_t w = (uint32_t)u << 16; float f; memcpy(&f, &w, 4); return f; }
-  __half h; memcpy(&h, &u, 2); return __half2float(h);
-}
-inline uint16_t f2h(float f) { __half h = __float2half_rn(f); uint16_t u; memcpy(&u, &h, 2); return u; }
-inline uint16_t f2bf(float f) {
-  uint32_t u; memcpy(&u, &f, 4);
-  if ((u & 0x7fffffffu) > 0x7f800000u) return 0x7fc0;
-  u += 0x7fffu + ((u >> 16) & 1u);
-  return (uint16_t)(u >> 16);
-}
-
 }  // namespace
 
 struct s2s_qwen3tts {
@@ -169,11 +156,10 @@ struct s2s_qwen3tts {
   bool finalized = false;
   s2s_llama *talker = nullptr, *pred = nullptr;
   CodecDecoder* codec = nullptr;
-  std::vector<void*> allocs;
+  WeightArena arena;   // the text side's tensors and every buffer below
   // text side
   void* text_embed = nullptr;                    // [text_vocab, text_hidden] 16-bit
   float *fc1_w = nullptr, *fc1_b = nullptr, *fc2_w = nullptr, *fc2_b = nullptr;   // [K][N] layouts
-  bool bound[5] = {false, false, false, false, false};
   // per session
   struct Sess { int n_trailing = 0, frames = 0, pos = 0; bool active = false; };
   std::vector<Sess> sess;
@@ -194,15 +180,6 @@ struct s2s_qwen3tts {
 };
 
 namespace {
-
-template <typename P> int talloc(s2s_qwen3tts* m, P** out, size_t bytes) {
-  void* p = nullptr;
-  S2S_CHECK_CUDA(cudaMalloc(&p, bytes ? bytes : 16));
-  S2S_CHECK_CUDA(cudaMemset(p, 0, bytes ? bytes : 16));
-  m->allocs.push_back(p);
-  *out = reinterpret_cast<P*>(p);
-  return S2S_OK;
-}
 
 int tts_max_batch(const s2s_qwen3tts* m) {
   return std::min(TTS_MAX_B, std::min(llama_max_decode_batch_of(m->talker), llama_max_decode_batch_of(m->pred)));
@@ -253,39 +230,47 @@ int s2s_qwen3tts_create(s2s_ctx* ctx, const s2s_qwen3tts_config* cfg, s2s_qwen3t
   if (r == S2S_OK && c.codec.quantizers != c.n_groups) { s2s_set_error("qwen3tts: codec quantizers %d != n_groups %d", c.codec.quantizers, c.n_groups); r = S2S_ERR_INVALID; }
   auto alloc_all = [&]() -> int {
     const int d = c.d_model, rows = c.max_text + 6;
-    S2S_CHECK(talloc(m, &m->text_embed, (size_t)c.text_vocab * c.text_hidden * 2));
-    S2S_CHECK(talloc(m, &m->fc1_w, (size_t)c.text_hidden * c.ffn * 4));
-    S2S_CHECK(talloc(m, &m->fc1_b, (size_t)c.ffn * 4));
-    S2S_CHECK(talloc(m, &m->fc2_w, (size_t)c.ffn * d * 4));
-    S2S_CHECK(talloc(m, &m->fc2_b, (size_t)d * 4));
+    WeightArena& A = m->arena;
+    S2S_CHECK(A.alloc(&m->text_embed, (size_t)c.text_vocab * c.text_hidden * 2));
+    S2S_CHECK(A.alloc(&m->fc1_w, (size_t)c.text_hidden * c.ffn * 4));
+    S2S_CHECK(A.alloc(&m->fc1_b, (size_t)c.ffn * 4));
+    S2S_CHECK(A.alloc(&m->fc2_w, (size_t)c.ffn * d * 4));
+    S2S_CHECK(A.alloc(&m->fc2_b, (size_t)d * 4));
+    // init_random: fixed seeds (seed ^ 1 .. 5) and scales of their own
+    A.add("text_embedding.weight", m->text_embed, true, (int64_t)c.text_vocab * c.text_hidden, 1.0f).seed = 1;
+    A.add("text_projection.linear_fc1.weight", m->fc1_w, false, (int64_t)c.ffn * c.text_hidden, 1.0f / sqrtf((float)c.text_hidden))
+        .as(W_LINEAR, c.ffn, c.text_hidden).seed = 2;
+    A.add("text_projection.linear_fc1.bias", m->fc1_b, false, c.ffn, 0.05f).seed = 3;
+    A.add("text_projection.linear_fc2.weight", m->fc2_w, false, (int64_t)d * c.ffn, 0.7f / sqrtf((float)c.ffn)).as(W_LINEAR, d, c.ffn).seed = 4;
+    A.add("text_projection.linear_fc2.bias", m->fc2_b, false, d, 0.05f).seed = 5;
     m->sess.assign(c.max_sessions, s2s_qwen3tts::Sess());
     m->trailing_stride = (long long)c.max_text * d;
     m->history_stride = (long long)c.max_positions * c.n_groups;
-    S2S_CHECK(talloc(m, &m->trailing, (size_t)c.max_sessions * m->trailing_stride * 4));
-    S2S_CHECK(talloc(m, &m->pad_embed, (size_t)c.max_sessions * d * 4));
-    S2S_CHECK(talloc(m, &m->xnext, (size_t)c.max_sessions * d * 4));
-    S2S_CHECK(talloc(m, &m->history, (size_t)c.max_sessions * m->history_stride * 4));
-    S2S_CHECK(talloc(m, &m->ids_d, (size_t)rows * 4));
-    S2S_CHECK(talloc(m, &m->emb_rows, (size_t)rows * c.text_hidden * 4));
-    S2S_CHECK(talloc(m, &m->proj_mid, (size_t)rows * c.ffn * 4));
-    S2S_CHECK(talloc(m, &m->proj_out, (size_t)rows * d * 4));
-    S2S_CHECK(talloc(m, &m->x_in_t, (size_t)TTS_MAX_B * d * 4));
-    S2S_CHECK(talloc(m, &m->hidden, (size_t)TTS_MAX_B * d * 4));
-    S2S_CHECK(talloc(m, &m->x_in_p, (size_t)TTS_MAX_B * d * 4));
-    S2S_CHECK(talloc(m, &m->tslot_d, TTS_MAX_B * 4));
-    S2S_CHECK(talloc(m, &m->tpos_d, TTS_MAX_B * 4));
-    S2S_CHECK(talloc(m, &m->pslot_d, TTS_MAX_B * 4));
-    S2S_CHECK(talloc(m, &m->ppos_d, TTS_MAX_B * 4));
-    S2S_CHECK(talloc(m, &m->code0, TTS_MAX_B * 4));
-    S2S_CHECK(talloc(m, &m->pcodes, (size_t)TTS_MAX_B * c.n_groups * 4));
-    S2S_CHECK(talloc(m, &m->tlen, TTS_MAX_B * 4));
-    S2S_CHECK(talloc(m, &m->plen, TTS_MAX_B * 4));
-    S2S_CHECK(talloc(m, &m->code0_feed, TTS_MAX_B * 4));
-    S2S_CHECK(talloc(m, &m->forced_frame, (size_t)TTS_MAX_B * c.n_groups * 4));
-    S2S_CHECK(talloc(m, &m->suppress, (size_t)c.vocab));
+    S2S_CHECK(A.alloc(&m->trailing, (size_t)c.max_sessions * m->trailing_stride * 4));
+    S2S_CHECK(A.alloc(&m->pad_embed, (size_t)c.max_sessions * d * 4));
+    S2S_CHECK(A.alloc(&m->xnext, (size_t)c.max_sessions * d * 4));
+    S2S_CHECK(A.alloc(&m->history, (size_t)c.max_sessions * m->history_stride * 4));
+    S2S_CHECK(A.alloc(&m->ids_d, (size_t)rows * 4));
+    S2S_CHECK(A.alloc(&m->emb_rows, (size_t)rows * c.text_hidden * 4));
+    S2S_CHECK(A.alloc(&m->proj_mid, (size_t)rows * c.ffn * 4));
+    S2S_CHECK(A.alloc(&m->proj_out, (size_t)rows * d * 4));
+    S2S_CHECK(A.alloc(&m->x_in_t, (size_t)TTS_MAX_B * d * 4));
+    S2S_CHECK(A.alloc(&m->hidden, (size_t)TTS_MAX_B * d * 4));
+    S2S_CHECK(A.alloc(&m->x_in_p, (size_t)TTS_MAX_B * d * 4));
+    S2S_CHECK(A.alloc(&m->tslot_d, TTS_MAX_B * 4));
+    S2S_CHECK(A.alloc(&m->tpos_d, TTS_MAX_B * 4));
+    S2S_CHECK(A.alloc(&m->pslot_d, TTS_MAX_B * 4));
+    S2S_CHECK(A.alloc(&m->ppos_d, TTS_MAX_B * 4));
+    S2S_CHECK(A.alloc(&m->code0, TTS_MAX_B * 4));
+    S2S_CHECK(A.alloc(&m->pcodes, (size_t)TTS_MAX_B * c.n_groups * 4));
+    S2S_CHECK(A.alloc(&m->tlen, TTS_MAX_B * 4));
+    S2S_CHECK(A.alloc(&m->plen, TTS_MAX_B * 4));
+    S2S_CHECK(A.alloc(&m->code0_feed, TTS_MAX_B * 4));
+    S2S_CHECK(A.alloc(&m->forced_frame, (size_t)TTS_MAX_B * c.n_groups * 4));
+    S2S_CHECK(A.alloc(&m->suppress, (size_t)c.vocab));
     m->tsamp.assign(c.max_sessions, samp_greedy());
     m->psamp.assign(c.max_sessions, samp_greedy());
-    S2S_CHECK(talloc(m, &m->samp_d, 2 * TTS_MAX_B * sizeof(SampSlot)));
+    S2S_CHECK(A.alloc(&m->samp_d, 2 * TTS_MAX_B * sizeof(SampSlot)));
     // transformers generate(): the last 1024 ids of the codec vocabulary except codec_eos are never predicted (TF:3954-3962)
     std::vector<unsigned char> mask((size_t)c.vocab, 0);
     for (int i = c.vocab - 1024; i < c.vocab; ++i) if (i != c.codec_eos) mask[(size_t)i] = 1;
@@ -303,7 +288,6 @@ int s2s_qwen3tts_destroy(s2s_qwen3tts* m) {
   if (m->talker) s2s_llama_destroy(m->talker);
   if (m->pred) s2s_llama_destroy(m->pred);
   if (m->codec) codec_destroy(m->codec);
-  for (void* p : m->allocs) cudaFree(p);
   delete m;
   return S2S_OK;
 }
@@ -322,68 +306,22 @@ int s2s_qwen3tts_bind_tensor(s2s_qwen3tts* m, const char* name, const void* data
   if (n == "model.codec_embedding.weight") return s2s_llama_bind_tensor(m->talker, "model.embed_tokens.weight", data_h, shape, ndim, dtype);
   if (n == "codec_head.weight") return s2s_llama_bind_tensor(m->talker, "lm_head.weight", data_h, shape, ndim, dtype);
   if (starts("model.")) return s2s_llama_bind_tensor(m->talker, name, data_h, shape, ndim, dtype);
-  const auto& c = m->cfg;
-  int64_t cnt = 1;
-  for (int i = 0; i < ndim; ++i) cnt *= shape[i];
-  S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  if (n == "text_embedding.weight") {
-    S2S_REQUIRE(cnt == (int64_t)c.text_vocab * c.text_hidden, "qwen3tts bind_tensor: text_embedding.weight has %lld elements", (long long)cnt);
-    std::vector<uint16_t> h((size_t)cnt);
-    const bool bf = c.compute_dtype == S2S_BF16;
-    for (int64_t i = 0; i < cnt; ++i) { const float v = src_f32(data_h, i, dtype); h[(size_t)i] = bf ? f2bf(v) : f2h(v); }
-    S2S_CHECK_CUDA(cudaMemcpy(m->text_embed, h.data(), (size_t)cnt * 2, cudaMemcpyHostToDevice));
-    m->bound[0] = true;
-    return S2S_OK;
-  }
-  struct { const char* nm; float* dst; int N, K; int idx; } lin[] = {
-      {"text_projection.linear_fc1.weight", m->fc1_w, c.ffn, c.text_hidden, 1}, {"text_projection.linear_fc2.weight", m->fc2_w, c.d_model, c.ffn, 3}};
-  for (auto& L : lin)
-    if (n == L.nm) {
-      S2S_REQUIRE(cnt == (int64_t)L.N * L.K, "qwen3tts bind_tensor: '%s' has %lld elements", name, (long long)cnt);
-      std::vector<float> t((size_t)cnt);
-      for (int nn = 0; nn < L.N; ++nn) for (int k = 0; k < L.K; ++k) t[(size_t)k * L.N + nn] = src_f32(data_h, (int64_t)nn * L.K + k, dtype);
-      S2S_CHECK_CUDA(cudaMemcpy(L.dst, t.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice));
-      m->bound[L.idx] = true;
-      return S2S_OK;
-    }
-  struct { const char* nm; float* dst; int N; int idx; } bias[] = {
-      {"text_projection.linear_fc1.bias", m->fc1_b, c.ffn, 2}, {"text_projection.linear_fc2.bias", m->fc2_b, c.d_model, 4}};
-  for (auto& L : bias)
-    if (n == L.nm) {
-      S2S_REQUIRE(cnt == L.N, "qwen3tts bind_tensor: '%s' has %lld elements", name, (long long)cnt);
-      std::vector<float> t((size_t)cnt);
-      for (int64_t i = 0; i < cnt; ++i) t[(size_t)i] = src_f32(data_h, i, dtype);
-      S2S_CHECK_CUDA(cudaMemcpy(L.dst, t.data(), (size_t)cnt * 4, cudaMemcpyHostToDevice));
-      m->bound[L.idx] = true;
-      return S2S_OK;
-    }
   if (starts("hidden_projection.")) return S2S_OK;   // multimodal path of the cousin: unused by a text-only TTS turn
-  s2s_set_error("qwen3tts bind_tensor: unknown tensor '%s'", name);
-  return S2S_ERR_NOT_FOUND;
+  S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
+  return m->arena.bind("qwen3tts", name, data_h, shape, ndim, dtype, m->cfg.compute_dtype);
 }
 
 int s2s_qwen3tts_init_random(s2s_qwen3tts* m, uint64_t seed) {
   S2S_REQUIRE(m, "qwen3tts init_random: null model");
-  const auto& c = m->cfg;
   S2S_CHECK(s2s_llama_init_random(m->talker, seed ^ 0x7a11ull));
   S2S_CHECK(s2s_llama_init_random(m->pred, seed ^ 0x9ed1ull));
   S2S_CHECK(codec_init_random(m->codec, seed ^ 0xc0decull));
-  S2S_CHECK(fill_random_launch(m->text_embed, (long long)c.text_vocab * c.text_hidden, c.compute_dtype, 1.0f, 0.f, seed ^ 1, 0));
-  S2S_CHECK(fill_random_launch(m->fc1_w, (long long)c.text_hidden * c.ffn, S2S_F32, 1.0f / sqrtf((float)c.text_hidden), 0.f, seed ^ 2, 0));
-  S2S_CHECK(fill_random_launch(m->fc1_b, c.ffn, S2S_F32, 0.05f, 0.f, seed ^ 3, 0));
-  S2S_CHECK(fill_random_launch(m->fc2_w, (long long)c.ffn * c.d_model, S2S_F32, 0.7f / sqrtf((float)c.ffn), 0.f, seed ^ 4, 0));
-  S2S_CHECK(fill_random_launch(m->fc2_b, c.d_model, S2S_F32, 0.05f, 0.f, seed ^ 5, 0));
-  for (bool& b : m->bound) b = true;
-  S2S_CHECK_CUDA(cudaDeviceSynchronize());
-  return S2S_OK;
+  return m->arena.init_random(seed, m->cfg.compute_dtype);
 }
 
 int s2s_qwen3tts_finalize(s2s_qwen3tts* m) {
   S2S_REQUIRE(m, "qwen3tts finalize: null model");
-  static const char* names[5] = {"text_embedding.weight", "text_projection.linear_fc1.weight", "text_projection.linear_fc1.bias",
-                                 "text_projection.linear_fc2.weight", "text_projection.linear_fc2.bias"};
-  for (int i = 0; i < 5; ++i)
-    if (!m->bound[i]) { s2s_set_error("qwen3tts finalize: tensor '%s' was never bound", names[i]); return S2S_ERR_INVALID; }
+  S2S_CHECK(m->arena.check_all_bound("qwen3tts"));
   S2S_CHECK(s2s_llama_finalize(m->talker));
   S2S_CHECK(s2s_llama_finalize(m->pred));
   S2S_CHECK(codec_finalize(m->codec));

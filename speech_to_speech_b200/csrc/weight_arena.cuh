@@ -1,0 +1,159 @@
+// weight_arena.cuh -- the host-side weight machinery every model object owns (internal to libs2s_b200): tracked device
+// allocations, the table of state-dict names -> kernel layouts, bind_tensor (convert, lay out, upload), init_random and the
+// finalize-time "every tensor was bound" check.  The layout step (weight_layout / weight_upload) is pure host code, so a
+// CPU program can check it against a numpy statement of each layout (tests/test_weight_layouts.py).
+#pragma once
+#include <string.h>
+
+#include <string>
+#include <unordered_map>
+#include <vector>
+
+#include "common.cuh"
+
+// Source shapes are those of the transformers state dict; d0, d1, d2, p and ld are read as listed.
+enum WeightLayout {
+  W_PLAIN = 0,
+  W_ROPE_PERM,    // [d0 rows][d1]: within each head of p rows, row j < p/2 -> 2j, row j >= p/2 -> 2(j - p/2) + 1
+  W_INTERLEAVE,   // [d0 rows][d1] -> rows 2r + p of a [2 d0][d1] block (p = 0 gate, 1 up)
+  W_LINEAR,       // [d0 = N][d1 = K] -> [K][N]; ld > 0: columns [p, p + N) of a shared [K][ld] matrix
+  W_CONV,         // [d0 = O][d1 = C][d2 = k] -> [k][C][O]
+  W_TCONV,        // [d0 = C][d1 = O][d2 = k], stride p, k = p or 2p -> k/p taps x [C][p*O]; tap 0 takes W[c][o][r + k - p]
+  W_CONV_ROWS,    // [d0 = O][d1 = C][d2 = k] -> [O][k][C] (Whisper's conv as a windowed GEMM: K = k*C)
+};
+
+struct WeightSlot {
+  void* dst = nullptr;
+  bool half = false;          // stored in the model's 16-bit compute dtype, else fp32
+  int layout = W_PLAIN;
+  int64_t n = 0;              // elements of the source tensor
+  int d0 = 0, d1 = 0, d2 = 0, p = 0, ld = 0;
+  float scale = 1.f;          // folded into every stored value, bound or random
+  float rnd_scale = 0.02f, rnd_offset = 0.f;
+  uint64_t seed = 0;          // != 0: init_random draws from its seed ^ this instead of its seed ^ FNV-1a(name)
+  bool bound = false;
+  bool raw = false;           // written by bind / init_random since the last finalize (the model clears it)
+  WeightSlot& as(int l, int a0, int a1, int a2 = 0, int pp = 0, int ldd = 0) {
+    layout = l; d0 = a0; d1 = a1; d2 = a2; p = pp; ld = ldd;
+    return *this;
+  }
+};
+
+// ---- host conversion (the one copy the models share) ----
+inline uint16_t f32_to_f16_bits(float f) { __half h = __float2half_rn(f); uint16_t u; memcpy(&u, &h, 2); return u; }
+inline uint16_t f32_to_bf16_bits(float f) {   // round to nearest even; every NaN -> 0x7fc0
+  uint32_t u; memcpy(&u, &f, 4);
+  if ((u & 0x7fffffffu) > 0x7f800000u) return 0x7fc0;
+  u += 0x7fffu + ((u >> 16) & 1u);
+  return (uint16_t)(u >> 16);
+}
+inline float src_to_f32(const void* data, int64_t i, int dtype) {
+  if (dtype == S2S_F32) return reinterpret_cast<const float*>(data)[i];
+  uint16_t u = reinterpret_cast<const uint16_t*>(data)[i];
+  if (dtype == S2S_BF16) { uint32_t w = (uint32_t)u << 16; float f; memcpy(&f, &w, 4); return f; }
+  __half h; memcpy(&h, &u, 2); return __half2float(h);
+}
+
+// init_random's seed for a tensor: seed ^ FNV-1a(name).  The offset basis is not FNV's published 0xcbf29ce484222325;
+// changing it would change every init_random weight.
+inline uint64_t weight_seed(uint64_t seed, const std::string& name) {
+  uint64_t h = 1469598103934665603ull;
+  for (char ch : name) h = (h ^ (uint64_t)(unsigned char)ch) * 1099511628211ull;
+  return seed ^ h;
+}
+
+// The slot's source tensor (dtype) -> the bytes bind uploads: times s.scale, laid out, stored as fp32 or as dtype16 (s.half).
+// INTERLEAVE and column-block LINEAR produce the slot's own rows; weight_upload places them.
+inline void weight_layout(const WeightSlot& s, const void* src, int dtype, int dtype16, std::vector<uint8_t>& out) {
+  out.resize((size_t)s.n * (s.half ? 2 : 4));
+  float* f32 = reinterpret_cast<float*>(out.data());
+  uint16_t* h16 = reinterpret_cast<uint16_t*>(out.data());
+  const bool bf = dtype16 == S2S_BF16;
+  auto put = [&](int64_t di, int64_t si) {
+    const float v = src_to_f32(src, si, dtype) * s.scale;
+    if (!s.half) f32[di] = v;
+    else h16[di] = bf ? f32_to_bf16_bits(v) : f32_to_f16_bits(v);
+  };
+  const int64_t A = s.d0, B = s.d1, K = s.d2;
+  switch (s.layout) {
+    case W_ROPE_PERM: {
+      const int64_t hd = s.p, half = hd / 2;
+      for (int64_t r = 0; r < A; ++r) {
+        const int64_t j = r % hd, dr = r - j + (j < half ? 2 * j : 2 * (j - half) + 1);
+        for (int64_t c = 0; c < B; ++c) put(dr * B + c, r * B + c);
+      }
+      break;
+    }
+    case W_LINEAR:
+      for (int64_t nn = 0; nn < A; ++nn)
+        for (int64_t k = 0; k < B; ++k) put(k * A + nn, nn * B + k);
+      break;
+    case W_CONV:
+      for (int64_t o = 0; o < A; ++o)
+        for (int64_t c = 0; c < B; ++c)
+          for (int64_t j = 0; j < K; ++j) put((j * B + c) * A + o, (o * B + c) * K + j);
+      break;
+    case W_TCONV: {
+      // k = 2 s: tap 0 multiplies X[t0 - 1] -> W[c][o][r + s]; tap 1 multiplies X[t0] -> W[c][o][r].  k = s: one tap.
+      const int64_t st = s.p, taps = K / st;
+      for (int64_t c = 0; c < A; ++c)
+        for (int64_t o = 0; o < B; ++o)
+          for (int64_t t = 0; t < K; ++t) put(((taps - 1 - t / st) * A + c) * st * B + (t % st) * B + o, (c * B + o) * K + t);
+      break;
+    }
+    case W_CONV_ROWS:
+      for (int64_t o = 0; o < A; ++o)
+        for (int64_t c = 0; c < B; ++c)
+          for (int64_t t = 0; t < K; ++t) put((o * K + t) * B + c, (o * B + c) * K + t);
+      break;
+    default:   // W_PLAIN, W_INTERLEAVE
+      for (int64_t i = 0; i < s.n; ++i) put(i, i);
+  }
+}
+
+// Where weight_layout's bytes go in s.dst: `height` rows of `width` bytes, `pitch` bytes apart, from byte `offset`.
+struct WeightUpload { size_t offset, pitch, width, height; };
+inline WeightUpload weight_upload(const WeightSlot& s) {
+  const size_t esz = s.half ? 2 : 4;
+  if (s.layout == W_INTERLEAVE) return {(size_t)s.p * s.d1 * esz, 2 * (size_t)s.d1 * esz, (size_t)s.d1 * esz, (size_t)s.d0};
+  if (s.layout == W_LINEAR && s.ld > 0) return {(size_t)s.p * esz, (size_t)s.ld * esz, (size_t)s.d0 * esz, (size_t)s.d1};
+  return {0, (size_t)s.n * esz, (size_t)s.n * esz, 1};
+}
+
+// One per model object.  Error messages start with `who`.
+struct WeightArena {
+  std::unordered_map<std::string, WeightSlot> slots;
+
+  WeightArena() = default;
+  WeightArena(const WeightArena&) = delete;
+  WeightArena& operator=(const WeightArena&) = delete;
+  ~WeightArena() { for (void* p : allocs_) cudaFree(p); }
+
+  // cudaMalloc (zeroed unless zero = false), freed with the arena
+  template <typename P> int alloc(P** out, size_t bytes, bool zero = true) {
+    void* p = nullptr;
+    S2S_CHECK_CUDA(cudaMalloc(&p, bytes ? bytes : 16));
+    allocs_.push_back(p);
+    if (zero) S2S_CHECK_CUDA(cudaMemset(p, 0, bytes ? bytes : 16));
+    *out = reinterpret_cast<P*>(p);
+    return S2S_OK;
+  }
+  WeightSlot& add(const std::string& name, void* dst, bool half, int64_t n, float rnd_scale = 0.02f, float rnd_offset = 0.f) {
+    WeightSlot& s = slots[name];
+    s = WeightSlot();
+    s.dst = dst; s.half = half; s.n = n; s.rnd_scale = rnd_scale; s.rnd_offset = rnd_offset;
+    return s;
+  }
+  WeightSlot* find(const std::string& name) {
+    auto it = slots.find(name);
+    return it == slots.end() ? nullptr : &it->second;
+  }
+  // lookup (S2S_ERR_NOT_FOUND), element count (S2S_ERR_INVALID), then weight_layout and one upload
+  int bind(const char* who, const char* name, const void* data_h, const int64_t* shape, int ndim, int dtype, int dtype16);
+  // every slot from fill_random_launch (seed ^ FNV-1a(name), or the slot's own seed), synchronised
+  int init_random(uint64_t seed, int dtype16);
+  int check_all_bound(const char* who) const;
+
+ private:
+  std::vector<void*> allocs_;
+};

@@ -7,30 +7,18 @@
 #include <string.h>
 
 #include <string>
-#include <unordered_map>
 #include <vector>
 
 #include "common.cuh"
 #include "gemm_tc.cuh"
 #include "kernels.cuh"
+#include "weight_arena.cuh"
 #include "whisper_decode.cuh"
 
 namespace {
 
 constexpr int N_FRAMES = 3000;
 constexpr int N_SAMPLES = 480000;
-
-enum SlotKind { SLOT_PLAIN = 0, SLOT_CONV = 1 };
-struct Slot {
-  void* dst = nullptr;
-  bool half = false;   // 16-bit compute dtype (else fp32)
-  int64_t n = 0;       // elements expected
-  int kind = SLOT_PLAIN;
-  int conv_out = 0, conv_in = 0;
-  float scale = 1.f;
-  bool bound = false;
-  float rnd_scale = 0.02f, rnd_offset = 0.f;
-};
 
 struct EncLayer {
   void *w_qkv, *w_o, *w_fc1, *w_fc2;
@@ -44,8 +32,7 @@ struct s2s_whisper {
   s2s_whisper_config cfg{};
   int esz = 2;
   bool finalized = false;
-  std::vector<void*> allocs;
-  std::unordered_map<std::string, Slot> slots;
+  WeightArena arena;
 
   // weights
   void *conv1_w = nullptr, *conv2_w = nullptr, *embed = nullptr, *ckv_w = nullptr;
@@ -88,39 +75,7 @@ struct s2s_whisper {
 
 namespace {
 
-template <typename P> int dev_alloc(s2s_whisper* m, P** out, size_t bytes, bool zero = true) {
-  void* p = nullptr;
-  S2S_CHECK_CUDA(cudaMalloc(&p, bytes ? bytes : 16));
-  if (zero) S2S_CHECK_CUDA(cudaMemset(p, 0, bytes ? bytes : 16));
-  m->allocs.push_back(p);
-  *out = reinterpret_cast<P*>(p);
-  return S2S_OK;
-}
-
-void add_slot(s2s_whisper* m, const std::string& name, void* dst, bool half, int64_t n, float scale = 1.f,
-              float rnd_scale = 0.02f, float rnd_offset = 0.f) {
-  Slot s;
-  s.dst = dst; s.half = half; s.n = n; s.scale = scale; s.rnd_scale = rnd_scale; s.rnd_offset = rnd_offset;
-  m->slots[name] = s;
-}
-
 inline char* off(void* base, int64_t elems, int esz) { return reinterpret_cast<char*>(base) + elems * esz; }
-
-// host conversion helpers
-inline uint16_t f32_to_f16_bits(float f) { __half h = __float2half_rn(f); uint16_t u; memcpy(&u, &h, 2); return u; }
-inline uint16_t f32_to_bf16_bits(float f) {
-  uint32_t u; memcpy(&u, &f, 4);
-  if ((u & 0x7fffffffu) > 0x7f800000u) return 0x7fc0;
-  const uint32_t lsb = (u >> 16) & 1u;
-  u += 0x7fffu + lsb;
-  return (uint16_t)(u >> 16);
-}
-inline float src_to_f32(const void* data, int64_t i, int dtype) {
-  if (dtype == S2S_F32) return reinterpret_cast<const float*>(data)[i];
-  uint16_t u = reinterpret_cast<const uint16_t*>(data)[i];
-  if (dtype == S2S_BF16) { uint32_t w = (uint32_t)u << 16; float f; memcpy(&f, &w, 4); return f; }
-  __half h; memcpy(&h, &u, 2); return __half2float(h);
-}
 
 int build_tables(s2s_whisper* m) {
   const int n_mels = m->cfg.n_mels;
@@ -152,10 +107,10 @@ int build_tables(s2s_whisper* m) {
     if (lo > hi) { lo = 0; hi = 0; }
     rg[j] = make_int2(lo, hi);
   }
-  S2S_CHECK(dev_alloc(m, &m->hann, 400 * 4));
-  S2S_CHECK(dev_alloc(m, &m->twiddle, 800 * 4));
-  S2S_CHECK(dev_alloc(m, &m->fb, fb.size() * 4));
-  S2S_CHECK(dev_alloc(m, &m->fb_range, rg.size() * sizeof(int2)));
+  S2S_CHECK(m->arena.alloc(&m->hann, 400 * 4));
+  S2S_CHECK(m->arena.alloc(&m->twiddle, 800 * 4));
+  S2S_CHECK(m->arena.alloc(&m->fb, fb.size() * 4));
+  S2S_CHECK(m->arena.alloc(&m->fb_range, rg.size() * sizeof(int2)));
   S2S_CHECK_CUDA(cudaMemcpy(m->hann, hann.data(), 400 * 4, cudaMemcpyHostToDevice));
   S2S_CHECK_CUDA(cudaMemcpy(m->twiddle, tw.data(), 800 * 4, cudaMemcpyHostToDevice));
   S2S_CHECK_CUDA(cudaMemcpy(m->fb, fb.data(), fb.size() * 4, cudaMemcpyHostToDevice));
@@ -167,31 +122,27 @@ int alloc_weights(s2s_whisper* m) {
   const auto& c = m->cfg;
   const int d = c.d_model, f = c.ffn, esz = m->esz;
   const float qscale = 1.0f / sqrtf((float)(d / c.heads));
+  WeightArena& A = m->arena;
   const float s_qk = 1.6f / sqrtf((float)d), s_v = 0.8f / sqrtf((float)d), s_o = 1.2f / sqrtf((float)d);
   const float s_fc1 = 1.0f / sqrtf((float)d), s_fc2 = 0.5f / sqrtf((float)f);
   auto wbytes = [&](int64_t n) { return (size_t)n * esz; };
 
-  S2S_CHECK(dev_alloc(m, &m->conv1_w, wbytes((int64_t)d * 3 * c.n_mels)));
-  S2S_CHECK(dev_alloc(m, &m->conv1_b, d * 4));
-  S2S_CHECK(dev_alloc(m, &m->conv2_w, wbytes((int64_t)d * 3 * d)));
-  S2S_CHECK(dev_alloc(m, &m->conv2_b, d * 4));
-  S2S_CHECK(dev_alloc(m, &m->enc_pos, (size_t)c.max_source_positions * d * 4));
-  {
-    Slot s; s.dst = m->conv1_w; s.half = true; s.n = (int64_t)d * c.n_mels * 3; s.kind = SLOT_CONV;
-    s.conv_out = d; s.conv_in = c.n_mels; s.rnd_scale = 0.05f;
-    m->slots["model.encoder.conv1.weight"] = s;
-    s.dst = m->conv2_w; s.n = (int64_t)d * d * 3; s.conv_in = d; s.rnd_scale = 0.03f;
-    m->slots["model.encoder.conv2.weight"] = s;
-  }
-  add_slot(m, "model.encoder.conv1.bias", m->conv1_b, false, d);
-  add_slot(m, "model.encoder.conv2.bias", m->conv2_b, false, d);
-  add_slot(m, "model.encoder.embed_positions.weight", m->enc_pos, false, (int64_t)c.max_source_positions * d, 1.f, 0.5f);
+  S2S_CHECK(m->arena.alloc(&m->conv1_w, wbytes((int64_t)d * 3 * c.n_mels)));
+  S2S_CHECK(m->arena.alloc(&m->conv1_b, d * 4));
+  S2S_CHECK(m->arena.alloc(&m->conv2_w, wbytes((int64_t)d * 3 * d)));
+  S2S_CHECK(m->arena.alloc(&m->conv2_b, d * 4));
+  S2S_CHECK(m->arena.alloc(&m->enc_pos, (size_t)c.max_source_positions * d * 4));
+  A.add("model.encoder.conv1.weight", m->conv1_w, true, (int64_t)d * c.n_mels * 3, 0.05f).as(W_CONV_ROWS, d, c.n_mels, 3);
+  A.add("model.encoder.conv2.weight", m->conv2_w, true, (int64_t)d * d * 3, 0.03f).as(W_CONV_ROWS, d, d, 3);
+  A.add("model.encoder.conv1.bias", m->conv1_b, false, d);
+  A.add("model.encoder.conv2.bias", m->conv2_b, false, d);
+  A.add("model.encoder.embed_positions.weight", m->enc_pos, false, (int64_t)c.max_source_positions * d, 0.5f);
 
   auto add_ln = [&](const std::string& nm, float** w, float** b) -> int {
-    S2S_CHECK(dev_alloc(m, w, d * 4));
-    S2S_CHECK(dev_alloc(m, b, d * 4));
-    add_slot(m, nm + ".weight", *w, false, d, 1.f, 0.1f, 1.0f);
-    add_slot(m, nm + ".bias", *b, false, d, 1.f, 0.05f);
+    S2S_CHECK(m->arena.alloc(w, d * 4));
+    S2S_CHECK(m->arena.alloc(b, d * 4));
+    A.add(nm + ".weight", *w, false, d, 0.1f, 1.0f);
+    A.add(nm + ".bias", *b, false, d, 0.05f);
     return S2S_OK;
   };
 
@@ -199,73 +150,73 @@ int alloc_weights(s2s_whisper* m) {
   for (int i = 0; i < c.enc_layers; ++i) {
     EncLayer& L = m->enc[i];
     const std::string p = "model.encoder.layers." + std::to_string(i) + ".";
-    S2S_CHECK(dev_alloc(m, &L.w_qkv, wbytes((int64_t)3 * d * d)));
-    S2S_CHECK(dev_alloc(m, &L.b_qkv, 3 * d * 4));
-    S2S_CHECK(dev_alloc(m, &L.w_o, wbytes((int64_t)d * d)));
-    S2S_CHECK(dev_alloc(m, &L.b_o, d * 4));
-    S2S_CHECK(dev_alloc(m, &L.w_fc1, wbytes((int64_t)f * d)));
-    S2S_CHECK(dev_alloc(m, &L.b_fc1, f * 4));
-    S2S_CHECK(dev_alloc(m, &L.w_fc2, wbytes((int64_t)d * f)));
-    S2S_CHECK(dev_alloc(m, &L.b_fc2, d * 4));
-    add_slot(m, p + "self_attn.q_proj.weight", L.w_qkv, true, (int64_t)d * d, qscale, s_qk);
-    add_slot(m, p + "self_attn.q_proj.bias", L.b_qkv, false, d, qscale);
-    add_slot(m, p + "self_attn.k_proj.weight", off(L.w_qkv, (int64_t)d * d, esz), true, (int64_t)d * d, 1.f, s_qk);
-    add_slot(m, p + "self_attn.v_proj.weight", off(L.w_qkv, (int64_t)2 * d * d, esz), true, (int64_t)d * d, 1.f, s_v);
-    add_slot(m, p + "self_attn.v_proj.bias", L.b_qkv + 2 * d, false, d);
-    add_slot(m, p + "self_attn.out_proj.weight", L.w_o, true, (int64_t)d * d, 1.f, s_o);
-    add_slot(m, p + "self_attn.out_proj.bias", L.b_o, false, d);
-    add_slot(m, p + "fc1.weight", L.w_fc1, true, (int64_t)f * d, 1.f, s_fc1);
-    add_slot(m, p + "fc1.bias", L.b_fc1, false, f);
-    add_slot(m, p + "fc2.weight", L.w_fc2, true, (int64_t)d * f, 1.f, s_fc2);
-    add_slot(m, p + "fc2.bias", L.b_fc2, false, d);
+    S2S_CHECK(m->arena.alloc(&L.w_qkv, wbytes((int64_t)3 * d * d)));
+    S2S_CHECK(m->arena.alloc(&L.b_qkv, 3 * d * 4));
+    S2S_CHECK(m->arena.alloc(&L.w_o, wbytes((int64_t)d * d)));
+    S2S_CHECK(m->arena.alloc(&L.b_o, d * 4));
+    S2S_CHECK(m->arena.alloc(&L.w_fc1, wbytes((int64_t)f * d)));
+    S2S_CHECK(m->arena.alloc(&L.b_fc1, f * 4));
+    S2S_CHECK(m->arena.alloc(&L.w_fc2, wbytes((int64_t)d * f)));
+    S2S_CHECK(m->arena.alloc(&L.b_fc2, d * 4));
+    A.add(p + "self_attn.q_proj.weight", L.w_qkv, true, (int64_t)d * d, s_qk).scale = qscale;
+    A.add(p + "self_attn.q_proj.bias", L.b_qkv, false, d).scale = qscale;
+    A.add(p + "self_attn.k_proj.weight", off(L.w_qkv, (int64_t)d * d, esz), true, (int64_t)d * d, s_qk);
+    A.add(p + "self_attn.v_proj.weight", off(L.w_qkv, (int64_t)2 * d * d, esz), true, (int64_t)d * d, s_v);
+    A.add(p + "self_attn.v_proj.bias", L.b_qkv + 2 * d, false, d);
+    A.add(p + "self_attn.out_proj.weight", L.w_o, true, (int64_t)d * d, s_o);
+    A.add(p + "self_attn.out_proj.bias", L.b_o, false, d);
+    A.add(p + "fc1.weight", L.w_fc1, true, (int64_t)f * d, s_fc1);
+    A.add(p + "fc1.bias", L.b_fc1, false, f);
+    A.add(p + "fc2.weight", L.w_fc2, true, (int64_t)d * f, s_fc2);
+    A.add(p + "fc2.bias", L.b_fc2, false, d);
     S2S_CHECK(add_ln(p + "self_attn_layer_norm", &L.ln1_w, &L.ln1_b));
     S2S_CHECK(add_ln(p + "final_layer_norm", &L.ln2_w, &L.ln2_b));
   }
   S2S_CHECK(add_ln("model.encoder.layer_norm", &m->enc_lnf_w, &m->enc_lnf_b));
 
   // decoder
-  S2S_CHECK(dev_alloc(m, &m->embed, wbytes((int64_t)c.vocab * d)));
-  S2S_CHECK(dev_alloc(m, &m->dec_pos, (size_t)c.max_target_positions * d * 4));
-  add_slot(m, "model.decoder.embed_tokens.weight", m->embed, true, (int64_t)c.vocab * d);
-  add_slot(m, "model.decoder.embed_positions.weight", m->dec_pos, false, (int64_t)c.max_target_positions * d);
-  S2S_CHECK(dev_alloc(m, &m->ckv_w, wbytes((int64_t)c.dec_layers * 2 * d * d)));
-  S2S_CHECK(dev_alloc(m, &m->ckv_b, (size_t)c.dec_layers * 2 * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->embed, wbytes((int64_t)c.vocab * d)));
+  S2S_CHECK(m->arena.alloc(&m->dec_pos, (size_t)c.max_target_positions * d * 4));
+  A.add("model.decoder.embed_tokens.weight", m->embed, true, (int64_t)c.vocab * d);
+  A.add("model.decoder.embed_positions.weight", m->dec_pos, false, (int64_t)c.max_target_positions * d);
+  S2S_CHECK(m->arena.alloc(&m->ckv_w, wbytes((int64_t)c.dec_layers * 2 * d * d)));
+  S2S_CHECK(m->arena.alloc(&m->ckv_b, (size_t)c.dec_layers * 2 * d * 4));
   m->dec_h.resize(c.dec_layers);
   for (int i = 0; i < c.dec_layers; ++i) {
     WhisperDecLayer& L = m->dec_h[i];
     const std::string p = "model.decoder.layers." + std::to_string(i) + ".";
     void *w_qkv, *w_o, *w_cq, *w_co, *w_fc1, *w_fc2;
     float *b_qkv, *b_o, *b_cq, *b_co, *b_fc1, *b_fc2, *l1w, *l1b, *l2w, *l2b, *l3w, *l3b;
-    S2S_CHECK(dev_alloc(m, &w_qkv, wbytes((int64_t)3 * d * d)));
-    S2S_CHECK(dev_alloc(m, &b_qkv, 3 * d * 4));
-    S2S_CHECK(dev_alloc(m, &w_o, wbytes((int64_t)d * d)));
-    S2S_CHECK(dev_alloc(m, &b_o, d * 4));
-    S2S_CHECK(dev_alloc(m, &w_cq, wbytes((int64_t)d * d)));
-    S2S_CHECK(dev_alloc(m, &b_cq, d * 4));
-    S2S_CHECK(dev_alloc(m, &w_co, wbytes((int64_t)d * d)));
-    S2S_CHECK(dev_alloc(m, &b_co, d * 4));
-    S2S_CHECK(dev_alloc(m, &w_fc1, wbytes((int64_t)f * d)));
-    S2S_CHECK(dev_alloc(m, &b_fc1, f * 4));
-    S2S_CHECK(dev_alloc(m, &w_fc2, wbytes((int64_t)d * f)));
-    S2S_CHECK(dev_alloc(m, &b_fc2, d * 4));
-    add_slot(m, p + "self_attn.q_proj.weight", w_qkv, true, (int64_t)d * d, qscale, s_qk);
-    add_slot(m, p + "self_attn.q_proj.bias", b_qkv, false, d, qscale);
-    add_slot(m, p + "self_attn.k_proj.weight", off(w_qkv, (int64_t)d * d, esz), true, (int64_t)d * d, 1.f, s_qk);
-    add_slot(m, p + "self_attn.v_proj.weight", off(w_qkv, (int64_t)2 * d * d, esz), true, (int64_t)d * d, 1.f, s_v);
-    add_slot(m, p + "self_attn.v_proj.bias", b_qkv + 2 * d, false, d);
-    add_slot(m, p + "self_attn.out_proj.weight", w_o, true, (int64_t)d * d, 1.f, s_o);
-    add_slot(m, p + "self_attn.out_proj.bias", b_o, false, d);
-    add_slot(m, p + "encoder_attn.q_proj.weight", w_cq, true, (int64_t)d * d, qscale, s_qk);
-    add_slot(m, p + "encoder_attn.q_proj.bias", b_cq, false, d, qscale);
-    add_slot(m, p + "encoder_attn.k_proj.weight", off(m->ckv_w, (int64_t)i * 2 * d * d, esz), true, (int64_t)d * d, 1.f, s_qk);
-    add_slot(m, p + "encoder_attn.v_proj.weight", off(m->ckv_w, (int64_t)(i * 2 + 1) * d * d, esz), true, (int64_t)d * d, 1.f, s_v);
-    add_slot(m, p + "encoder_attn.v_proj.bias", m->ckv_b + (int64_t)(i * 2 + 1) * d, false, d);
-    add_slot(m, p + "encoder_attn.out_proj.weight", w_co, true, (int64_t)d * d, 1.f, s_o);
-    add_slot(m, p + "encoder_attn.out_proj.bias", b_co, false, d);
-    add_slot(m, p + "fc1.weight", w_fc1, true, (int64_t)f * d, 1.f, s_fc1);
-    add_slot(m, p + "fc1.bias", b_fc1, false, f);
-    add_slot(m, p + "fc2.weight", w_fc2, true, (int64_t)d * f, 1.f, s_fc2);
-    add_slot(m, p + "fc2.bias", b_fc2, false, d);
+    S2S_CHECK(m->arena.alloc(&w_qkv, wbytes((int64_t)3 * d * d)));
+    S2S_CHECK(m->arena.alloc(&b_qkv, 3 * d * 4));
+    S2S_CHECK(m->arena.alloc(&w_o, wbytes((int64_t)d * d)));
+    S2S_CHECK(m->arena.alloc(&b_o, d * 4));
+    S2S_CHECK(m->arena.alloc(&w_cq, wbytes((int64_t)d * d)));
+    S2S_CHECK(m->arena.alloc(&b_cq, d * 4));
+    S2S_CHECK(m->arena.alloc(&w_co, wbytes((int64_t)d * d)));
+    S2S_CHECK(m->arena.alloc(&b_co, d * 4));
+    S2S_CHECK(m->arena.alloc(&w_fc1, wbytes((int64_t)f * d)));
+    S2S_CHECK(m->arena.alloc(&b_fc1, f * 4));
+    S2S_CHECK(m->arena.alloc(&w_fc2, wbytes((int64_t)d * f)));
+    S2S_CHECK(m->arena.alloc(&b_fc2, d * 4));
+    A.add(p + "self_attn.q_proj.weight", w_qkv, true, (int64_t)d * d, s_qk).scale = qscale;
+    A.add(p + "self_attn.q_proj.bias", b_qkv, false, d).scale = qscale;
+    A.add(p + "self_attn.k_proj.weight", off(w_qkv, (int64_t)d * d, esz), true, (int64_t)d * d, s_qk);
+    A.add(p + "self_attn.v_proj.weight", off(w_qkv, (int64_t)2 * d * d, esz), true, (int64_t)d * d, s_v);
+    A.add(p + "self_attn.v_proj.bias", b_qkv + 2 * d, false, d);
+    A.add(p + "self_attn.out_proj.weight", w_o, true, (int64_t)d * d, s_o);
+    A.add(p + "self_attn.out_proj.bias", b_o, false, d);
+    A.add(p + "encoder_attn.q_proj.weight", w_cq, true, (int64_t)d * d, s_qk).scale = qscale;
+    A.add(p + "encoder_attn.q_proj.bias", b_cq, false, d).scale = qscale;
+    A.add(p + "encoder_attn.k_proj.weight", off(m->ckv_w, (int64_t)i * 2 * d * d, esz), true, (int64_t)d * d, s_qk);
+    A.add(p + "encoder_attn.v_proj.weight", off(m->ckv_w, (int64_t)(i * 2 + 1) * d * d, esz), true, (int64_t)d * d, s_v);
+    A.add(p + "encoder_attn.v_proj.bias", m->ckv_b + (int64_t)(i * 2 + 1) * d, false, d);
+    A.add(p + "encoder_attn.out_proj.weight", w_co, true, (int64_t)d * d, s_o);
+    A.add(p + "encoder_attn.out_proj.bias", b_co, false, d);
+    A.add(p + "fc1.weight", w_fc1, true, (int64_t)f * d, s_fc1);
+    A.add(p + "fc1.bias", b_fc1, false, f);
+    A.add(p + "fc2.weight", w_fc2, true, (int64_t)d * f, s_fc2);
+    A.add(p + "fc2.bias", b_fc2, false, d);
     S2S_CHECK(add_ln(p + "self_attn_layer_norm", &l1w, &l1b));
     S2S_CHECK(add_ln(p + "encoder_attn_layer_norm", &l2w, &l2b));
     S2S_CHECK(add_ln(p + "final_layer_norm", &l3w, &l3b));
@@ -274,7 +225,7 @@ int alloc_weights(s2s_whisper* m) {
     L.ln1_w = l1w; L.ln1_b = l1b; L.ln2_w = l2w; L.ln2_b = l2b; L.ln3_w = l3w; L.ln3_b = l3b;
   }
   S2S_CHECK(add_ln("model.decoder.layer_norm", &m->dec_lnf_w, &m->dec_lnf_b));
-  S2S_CHECK(dev_alloc(m, &m->dec_d, sizeof(WhisperDecLayer) * c.dec_layers));
+  S2S_CHECK(m->arena.alloc(&m->dec_d, sizeof(WhisperDecLayer) * c.dec_layers));
   S2S_CHECK_CUDA(cudaMemcpy(m->dec_d, m->dec_h.data(), sizeof(WhisperDecLayer) * c.dec_layers, cudaMemcpyHostToDevice));
   return S2S_OK;
 }
@@ -283,44 +234,44 @@ int alloc_workspace(s2s_whisper* m) {
   const auto& c = m->cfg;
   const int d = c.d_model, f = c.ffn, B = c.max_batch, esz = m->esz;
   const int64_t rows = (int64_t)B * c.max_source_positions;
-  S2S_CHECK(dev_alloc(m, &m->pcm, (size_t)B * N_SAMPLES * 4, false));
-  S2S_CHECK(dev_alloc(m, &m->n_samples_d, B * 4));
-  S2S_CHECK(dev_alloc(m, &m->mel_f32, (size_t)B * c.n_mels * N_FRAMES * 4));
-  S2S_CHECK(dev_alloc(m, &m->mel_max, B * 4));
-  S2S_CHECK(dev_alloc(m, &m->mel_t, (size_t)B * (N_FRAMES + 2) * c.n_mels * esz));
-  S2S_CHECK(dev_alloc(m, &m->h1, (size_t)B * (N_FRAMES + 2) * d * esz));
-  S2S_CHECK(dev_alloc(m, &m->x, (size_t)rows * d * 4));
-  S2S_CHECK(dev_alloc(m, &m->xn, (size_t)rows * d * esz));
-  S2S_CHECK(dev_alloc(m, &m->qkv, (size_t)rows * 3 * d * esz));
-  S2S_CHECK(dev_alloc(m, &m->attn, (size_t)rows * d * esz));
-  S2S_CHECK(dev_alloc(m, &m->hbuf, (size_t)rows * f * esz));
-  S2S_CHECK(dev_alloc(m, &m->enc_out, (size_t)rows * d * esz));
-  S2S_CHECK(dev_alloc(m, &m->cross_kv, (size_t)rows * c.dec_layers * 2 * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->pcm, (size_t)B * N_SAMPLES * 4, false));
+  S2S_CHECK(m->arena.alloc(&m->n_samples_d, B * 4));
+  S2S_CHECK(m->arena.alloc(&m->mel_f32, (size_t)B * c.n_mels * N_FRAMES * 4));
+  S2S_CHECK(m->arena.alloc(&m->mel_max, B * 4));
+  S2S_CHECK(m->arena.alloc(&m->mel_t, (size_t)B * (N_FRAMES + 2) * c.n_mels * esz));
+  S2S_CHECK(m->arena.alloc(&m->h1, (size_t)B * (N_FRAMES + 2) * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->x, (size_t)rows * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->xn, (size_t)rows * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->qkv, (size_t)rows * 3 * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->attn, (size_t)rows * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->hbuf, (size_t)rows * f * esz));
+  S2S_CHECK(m->arena.alloc(&m->enc_out, (size_t)rows * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->cross_kv, (size_t)rows * c.dec_layers * 2 * d * esz));
   m->vt_elems = attention_tc_scratch_elems(B, c.max_source_positions, c.heads, 64);
-  S2S_CHECK(dev_alloc(m, &m->vt, m->vt_elems * esz));
+  S2S_CHECK(m->arena.alloc(&m->vt, m->vt_elems * esz));
   // decoder
   m->s_max = (c.max_source_positions + ATT_CHUNK_KEYS - 1) / ATT_CHUNK_KEYS;
   const int grid = m->ctx->num_sms;
-  S2S_CHECK(dev_alloc(m, &m->dx, (size_t)B * d * 4));
-  S2S_CHECK(dev_alloc(m, &m->dq, (size_t)B * d * 4));
-  S2S_CHECK(dev_alloc(m, &m->dh, (size_t)B * f * 4));
-  S2S_CHECK(dev_alloc(m, &m->part, (size_t)B * c.heads * m->s_max * 68 * 4));
-  S2S_CHECK(dev_alloc(m, &m->attn16, (size_t)B * d * esz));
-  S2S_CHECK(dev_alloc(m, &m->dx_alt, (size_t)2 * d * 4));
-  S2S_CHECK(dev_alloc(m, &m->part_x0, (size_t)c.heads * 2 * d * 4));
-  S2S_CHECK(dev_alloc(m, &m->part_x1, (size_t)c.heads * 2 * d * 4));
-  S2S_CHECK(dev_alloc(m, &m->attn_cnt, (size_t)B * c.heads * 4));
-  S2S_CHECK(dev_alloc(m, &m->self_kv, (size_t)B * c.dec_layers * 2 * c.max_target_positions * d * esz));
-  S2S_CHECK(dev_alloc(m, &m->tokens, (size_t)B * c.max_target_positions * 4));
-  S2S_CHECK(dev_alloc(m, &m->out_ids, (size_t)B * c.max_target_positions * 4));
-  S2S_CHECK(dev_alloc(m, &m->out_len, B * 4));
-  S2S_CHECK(dev_alloc(m, &m->done, B * 4));
-  S2S_CHECK(dev_alloc(m, &m->n_done, 16));
-  S2S_CHECK(dev_alloc(m, &m->cand_val, (size_t)B * grid * 4));
-  S2S_CHECK(dev_alloc(m, &m->cand_idx, (size_t)B * grid * 4));
-  S2S_CHECK(dev_alloc(m, &m->suppress, c.vocab));
-  S2S_CHECK(dev_alloc(m, &m->suppress_lang, c.vocab));
-  S2S_CHECK(dev_alloc(m, &m->sync_counter, 16));
+  S2S_CHECK(m->arena.alloc(&m->dx, (size_t)B * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->dq, (size_t)B * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->dh, (size_t)B * f * 4));
+  S2S_CHECK(m->arena.alloc(&m->part, (size_t)B * c.heads * m->s_max * 68 * 4));
+  S2S_CHECK(m->arena.alloc(&m->attn16, (size_t)B * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->dx_alt, (size_t)2 * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->part_x0, (size_t)c.heads * 2 * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->part_x1, (size_t)c.heads * 2 * d * 4));
+  S2S_CHECK(m->arena.alloc(&m->attn_cnt, (size_t)B * c.heads * 4));
+  S2S_CHECK(m->arena.alloc(&m->self_kv, (size_t)B * c.dec_layers * 2 * c.max_target_positions * d * esz));
+  S2S_CHECK(m->arena.alloc(&m->tokens, (size_t)B * c.max_target_positions * 4));
+  S2S_CHECK(m->arena.alloc(&m->out_ids, (size_t)B * c.max_target_positions * 4));
+  S2S_CHECK(m->arena.alloc(&m->out_len, B * 4));
+  S2S_CHECK(m->arena.alloc(&m->done, B * 4));
+  S2S_CHECK(m->arena.alloc(&m->n_done, 16));
+  S2S_CHECK(m->arena.alloc(&m->cand_val, (size_t)B * grid * 4));
+  S2S_CHECK(m->arena.alloc(&m->cand_idx, (size_t)B * grid * 4));
+  S2S_CHECK(m->arena.alloc(&m->suppress, c.vocab));
+  S2S_CHECK(m->arena.alloc(&m->suppress_lang, c.vocab));
+  S2S_CHECK(m->arena.alloc(&m->sync_counter, 16));
   return S2S_OK;
 }
 
@@ -364,7 +315,6 @@ int s2s_whisper_create(s2s_ctx* ctx, const s2s_whisper_config* cfg, s2s_whisper*
 
 int s2s_whisper_destroy(s2s_whisper* m) {
   if (!m) return S2S_OK;
-  for (void* p : m->allocs) cudaFree(p);
   if (m->tok_stage) cudaFreeHost(m->tok_stage);
   if (m->tok_event) cudaEventDestroy(m->tok_event);
   delete m;
@@ -373,66 +323,21 @@ int s2s_whisper_destroy(s2s_whisper* m) {
 
 int s2s_whisper_bind_tensor(s2s_whisper* m, const char* name, const void* data_h, const int64_t* shape, int32_t ndim,
                             int32_t dtype) {
-  S2S_REQUIRE(m && name && data_h && shape, "bind_tensor: null argument");
+  S2S_REQUIRE(m && name && data_h && shape, "whisper bind_tensor: null argument");
   if (strcmp(name, "proj_out.weight") == 0) return S2S_OK;  // tied to embed_tokens
-  auto it = m->slots.find(name);
-  if (it == m->slots.end()) {
-    s2s_set_error("bind_tensor: unknown tensor '%s'", name);
-    return S2S_ERR_NOT_FOUND;
-  }
-  Slot& s = it->second;
-  int64_t n = 1;
-  for (int i = 0; i < ndim; ++i) n *= shape[i];
-  S2S_REQUIRE(n == s.n, "bind_tensor: '%s' has %lld elements, expected %lld", name, (long long)n, (long long)s.n);
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  std::vector<float> tmp((size_t)n);
-  if (s.kind == SLOT_CONV) {
-    // [out, in, 3] -> [out, tap * in + c]
-    const int O = s.conv_out, C = s.conv_in;
-    for (int o = 0; o < O; ++o)
-      for (int c = 0; c < C; ++c)
-        for (int t = 0; t < 3; ++t)
-          tmp[((size_t)o * 3 + t) * C + c] = src_to_f32(data_h, ((int64_t)o * C + c) * 3 + t, dtype) * s.scale;
-  } else {
-    for (int64_t i = 0; i < n; ++i) tmp[(size_t)i] = src_to_f32(data_h, i, dtype) * s.scale;
-  }
-  if (s.half) {
-    std::vector<uint16_t> h((size_t)n);
-    if (m->cfg.compute_dtype == S2S_F16) for (int64_t i = 0; i < n; ++i) h[(size_t)i] = f32_to_f16_bits(tmp[(size_t)i]);
-    else for (int64_t i = 0; i < n; ++i) h[(size_t)i] = f32_to_bf16_bits(tmp[(size_t)i]);
-    S2S_CHECK_CUDA(cudaMemcpy(s.dst, h.data(), (size_t)n * 2, cudaMemcpyHostToDevice));
-  } else {
-    S2S_CHECK_CUDA(cudaMemcpy(s.dst, tmp.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
-  }
-  s.bound = true;
-  return S2S_OK;
+  return m->arena.bind("whisper", name, data_h, shape, ndim, dtype, m->cfg.compute_dtype);
 }
 
 int s2s_whisper_init_random(s2s_whisper* m, uint64_t seed) {
-  S2S_REQUIRE(m, "init_random: null model");
+  S2S_REQUIRE(m, "whisper init_random: null model");
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-  uint64_t k = 0;
-  for (auto& kv : m->slots) {
-    Slot& s = kv.second;
-    uint64_t hsh = 1469598103934665603ull;
-    for (char ch : kv.first) hsh = (hsh ^ (uint64_t)(unsigned char)ch) * 1099511628211ull;
-    S2S_CHECK(fill_random_launch(s.dst, s.n, s.half ? m->cfg.compute_dtype : S2S_F32, s.rnd_scale * s.scale, s.rnd_offset,
-                                 seed ^ hsh, 0));
-    s.bound = true;
-    ++k;
-  }
-  S2S_CHECK_CUDA(cudaDeviceSynchronize());
-  return S2S_OK;
+  return m->arena.init_random(seed, m->cfg.compute_dtype);
 }
 
 int s2s_whisper_finalize(s2s_whisper* m) {
-  S2S_REQUIRE(m, "finalize: null model");
-  for (auto& kv : m->slots) {
-    if (!kv.second.bound) {
-      s2s_set_error("finalize: tensor '%s' was never bound", kv.first.c_str());
-      return S2S_ERR_INVALID;
-    }
-  }
+  S2S_REQUIRE(m, "whisper finalize: null model");
+  S2S_CHECK(m->arena.check_all_bound("whisper"));
   // decode-side weight layout: fragment-major tiles (weight_tiles.cu), built once per (re)load
   {
     const auto& c = m->cfg;
@@ -443,15 +348,15 @@ int s2s_whisper_finalize(s2s_whisper* m) {
       for (int i = 0; i < c.dec_layers; ++i) {
         WhisperDecLayer& T = m->dec_t[i];
         void *a, *b, *cq, *co, *f1, *f2;
-        S2S_CHECK(dev_alloc(m, &a, tiled_weight_elems(3 * d, d) * 2));
-        S2S_CHECK(dev_alloc(m, &b, tiled_weight_elems(d, d) * 2));
-        S2S_CHECK(dev_alloc(m, &cq, tiled_weight_elems(d, d) * 2));
-        S2S_CHECK(dev_alloc(m, &co, tiled_weight_elems(d, d) * 2));
-        S2S_CHECK(dev_alloc(m, &f1, tiled_weight_elems(f, d) * 2));
-        S2S_CHECK(dev_alloc(m, &f2, tiled_weight_elems(d, f) * 2));
+        S2S_CHECK(m->arena.alloc(&a, tiled_weight_elems(3 * d, d) * 2));
+        S2S_CHECK(m->arena.alloc(&b, tiled_weight_elems(d, d) * 2));
+        S2S_CHECK(m->arena.alloc(&cq, tiled_weight_elems(d, d) * 2));
+        S2S_CHECK(m->arena.alloc(&co, tiled_weight_elems(d, d) * 2));
+        S2S_CHECK(m->arena.alloc(&f1, tiled_weight_elems(f, d) * 2));
+        S2S_CHECK(m->arena.alloc(&f2, tiled_weight_elems(d, f) * 2));
         T.w_qkv = a; T.w_o = b; T.w_cq = cq; T.w_co = co; T.w_fc1 = f1; T.w_fc2 = f2;
       }
-      S2S_CHECK(dev_alloc(m, &m->embed_t, tiled_weight_elems(c.vocab, d) * 2));
+      S2S_CHECK(m->arena.alloc(&m->embed_t, tiled_weight_elems(c.vocab, d) * 2));
       S2S_CHECK_CUDA(cudaMemcpy(m->dec_d, m->dec_t.data(), sizeof(WhisperDecLayer) * c.dec_layers, cudaMemcpyHostToDevice));
     }
     for (int i = 0; i < c.dec_layers; ++i) {

@@ -127,15 +127,7 @@ class WhisperEngine:
 
     # -- weights -----------------------------------------------------------------------------
     def load_state_dict(self, weights: Mapping[str, "np.ndarray | torch.Tensor"]) -> None:
-        for name, w in weights.items():
-            if isinstance(w, torch.Tensor):
-                w = w.detach().to("cpu", torch.float32).numpy()
-            a = np.ascontiguousarray(w)
-            if a.dtype not in (np.float32, np.float16):
-                a = a.astype(np.float32)
-            shape = (C.c_int64 * max(1, a.ndim))(*a.shape)
-            check(self.lib.s2s_whisper_bind_tensor(self.handle, name.encode(), a.ctypes.data_as(C.c_void_p), shape,
-                                                   a.ndim, _np_dtype_code(a)), f"bind_tensor({name})")
+        _bind_all(self.lib.s2s_whisper_bind_tensor, self.handle, weights, "whisper")
         check(self.lib.s2s_whisper_finalize(self.handle), "s2s_whisper_finalize")
 
     def init_random(self, seed: int = 0) -> None:
@@ -344,15 +336,7 @@ class LlamaEngine:
                   "s2s_llama_set_weight_format")
 
     def load_state_dict(self, weights: Mapping[str, "np.ndarray | torch.Tensor"]) -> None:
-        for name, w in weights.items():
-            if isinstance(w, torch.Tensor):
-                w = w.detach().to("cpu", torch.float32).numpy()
-            a = np.ascontiguousarray(w)
-            if a.dtype not in (np.float32, np.float16):
-                a = a.astype(np.float32)
-            shape = (C.c_int64 * max(1, a.ndim))(*a.shape)
-            check(self.lib.s2s_llama_bind_tensor(self.handle, name.encode(), a.ctypes.data_as(C.c_void_p), shape, a.ndim,
-                                                 _np_dtype_code(a)), f"llama bind_tensor({name})")
+        _bind_all(self.lib.s2s_llama_bind_tensor, self.handle, weights, "llama")
         check(self.lib.s2s_llama_finalize(self.handle), "s2s_llama_finalize")
 
     def init_random(self, seed: int = 0) -> None:
