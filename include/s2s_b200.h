@@ -136,6 +136,26 @@ int s2s_attention(s2s_ctx* ctx, const void* q_d, const void* k_d, const void* v_
                   int32_t Tq, int32_t Tk, int32_t heads, int32_t kv_heads, int32_t hd, int64_t ldq,
                   int64_t ldk, int64_t ldv, int64_t ldo, float scale, int32_t causal, int32_t dtype,
                   void* stream);
+/* One attention phase of the Llama-family decode by itself (exposed for tests): the production device function of the
+ * persistent decode kernel, cut into (session, head, key split) items by the same plan, run in a plain launch of `grid`
+ * CTAs.  Session b attends its first lens_h[b] cached keys (the step's own key included) with the fp32 query q[b]:
+ *   out[b][h] = sum_j softmax_j(q[b][h] . K[j]) V[j],   K / V = the kv head h / (heads / kv_heads) of slot slots_h[b].
+ * kv holds one layer of the model's cache layout, [slots][2][max_pos][kv_heads * hd] (K rows, then V rows, per slot).
+ * grid 0 = the context's decode grid (s2s_set_sm_partition); assoc_b 0 = B, else the batch whose plan fixes the split
+ * plan (the decode launch uses 8 at 13 to 16 Llama-3-8B sessions).  *plan_out_h (may be NULL) = the plan: key splits per
+ * (session, head) in bits 0-6, bit 7 set for warp-level items.  Split records and counters are allocated per call, and a
+ * counter the merge left non-zero is an error.  Synchronous: returns after the stream has finished. */
+typedef struct {
+  const float* q;        /* [B][heads][hd] fp32, softmax scale applied */
+  const void* kv;        /* 16-bit (dtype), [slots][2][max_pos][kv_heads * hd] */
+  int32_t max_pos;
+  const int32_t* slots_h; const int32_t* lens_h; int32_t B;   /* lens_h[b] in [1, max_pos]; B in [1, 16] */
+  int32_t heads, kv_heads, hd, dtype;                         /* hd 64 or 128; dtype S2S_F16 or S2S_BF16 */
+  int32_t grid;          /* CTAs; 0 = the context's decode grid */
+  int32_t assoc_b;       /* 0 = B */
+  void* out;             /* [B][heads][hd] 16-bit */
+} s2s_dec_attn_args;
+int s2s_decode_attention(s2s_ctx* ctx, const s2s_dec_attn_args* args, int32_t* plan_out_h, void* stream);
 
 /* ---- Llama-family LLM ------------------------------------------------------------------ */
 typedef struct {

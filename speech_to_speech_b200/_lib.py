@@ -19,7 +19,7 @@ EXPORTED = [
     "s2s_whisper_create", "s2s_whisper_destroy", "s2s_whisper_bind_tensor", "s2s_whisper_init_random",
     "s2s_whisper_finalize", "s2s_whisper_logmel", "s2s_whisper_encode", "s2s_whisper_decode",
     "s2s_whisper_detect_language", "s2s_whisper_transcribe", "s2s_whisper_set_trace", "s2s_whisper_max_decode_batch",
-    "s2s_gemm", "s2s_attention",
+    "s2s_gemm", "s2s_attention", "s2s_decode_attention",
     "s2s_llama_create", "s2s_llama_destroy", "s2s_llama_bind_tensor", "s2s_llama_init_random",
     "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_set_sampling", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
     "s2s_llama_set_weight_format", "s2s_llama_weight_format",
@@ -90,6 +90,16 @@ class ConvArgs(C.Structure):
     ]
 
 
+class DecAttnArgs(C.Structure):
+    """s2s_dec_attn_args: one decode attention phase by itself (s2s_decode_attention)."""
+    _fields_ = [
+        ("q", C.c_void_p), ("kv", C.c_void_p), ("max_pos", C.c_int32),
+        ("slots_h", C.POINTER(C.c_int32)), ("lens_h", C.POINTER(C.c_int32)), ("B", C.c_int32),
+        ("heads", C.c_int32), ("kv_heads", C.c_int32), ("hd", C.c_int32), ("dtype", C.c_int32),
+        ("grid", C.c_int32), ("assoc_b", C.c_int32), ("out", C.c_void_p),
+    ]
+
+
 class Qwen3TTSConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "d_model", "layers", "heads", "kv_heads", "head_dim", "ffn", "vocab",
@@ -141,6 +151,7 @@ def load() -> C.CDLL:
     lib.s2s_whisper_max_decode_batch.restype = i32
     lib.s2s_gemm.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     lib.s2s_attention.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i64, i64, i64, i64, f32, i32, i32, vp]
+    lib.s2s_decode_attention.argtypes = [vp, C.POINTER(DecAttnArgs), C.POINTER(i32), vp]
     lib.s2s_llama_create.argtypes = [vp, C.POINTER(LlamaConfig), C.POINTER(vp)]
     lib.s2s_llama_destroy.argtypes = [vp]
     lib.s2s_llama_bind_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]

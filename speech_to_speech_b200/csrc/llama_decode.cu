@@ -18,6 +18,7 @@
 // F8 instantiation: the same kernel over FP8 E4M3 weights with power-of-two row scales (7.5 GB / token), bf16 compute only.
 // Every projection of the launch, lm_head included, is FP8, so the kernel still holds one GEMV routine.
 #include <algorithm>
+#include <vector>
 
 #include "llama_decode.cuh"
 #include "llama_decode_plan.cuh"
@@ -112,6 +113,13 @@ __device__ __noinline__ void ld_attn(const LlamaDecParams& p, int layer, int ste
     }
     attn_run_item<T, HD>(wl, q, Kb, Kb + p.kv_which_stride, kvd, len, blk0, blk1, rec_s, part_bh, s, S, p.attn_cnt + bh, out16);
   }
+}
+
+// s2s_decode_attention: the attention phase of layer 0, step 0 alone (no grid barrier inside a phase: a plain launch)
+template <typename T, int HD>
+__global__ void __launch_bounds__(DEC_THREADS, 1) ld_attn_only_kernel(const __grid_constant__ LlamaDecParams p) {
+  extern __shared__ __align__(16) float rec_s[];   // DEC_WARPS records
+  ld_attn<T, HD>(p, 0, 0, rec_s);
 }
 
 
@@ -362,4 +370,70 @@ int llama_decode_max_batch(int device, int dtype, int weight_format, int d, int 
                                                       : s2s_max_dyn_smem(llama_decode_kernel<__nv_bfloat16, false>, device, &max_dyn);
   if (e != cudaSuccess) return 0;
   return llama_decode_plan_max_batch(d, ffn, qd, grid, max_dyn);
+}
+
+extern "C" int s2s_decode_attention(s2s_ctx* ctx, const s2s_dec_attn_args* args, int32_t* plan_out_h, void* stream) {
+  S2S_REQUIRE(ctx && args, "s2s_decode_attention: null argument");
+  const s2s_dec_attn_args& a = *args;
+  S2S_REQUIRE(a.q && a.kv && a.out && a.slots_h && a.lens_h, "s2s_decode_attention: null q / kv / out / slots_h / lens_h");
+  S2S_REQUIRE(a.B >= 1 && a.B <= DEC_MAX_B, "s2s_decode_attention: B %d not in [1, %d]", a.B, DEC_MAX_B);
+  S2S_REQUIRE(a.heads >= 1 && a.kv_heads >= 1 && a.heads % a.kv_heads == 0, "s2s_decode_attention: heads %d / kv_heads %d",
+              a.heads, a.kv_heads);
+  S2S_REQUIRE(a.hd == 64 || a.hd == 128, "s2s_decode_attention: hd %d (64 or 128)", a.hd);
+  S2S_REQUIRE(a.dtype == S2S_F16 || a.dtype == S2S_BF16, "s2s_decode_attention: dtype %d", a.dtype);
+  S2S_REQUIRE(a.max_pos >= 1 && a.grid >= 0 && a.assoc_b >= 0 && a.assoc_b <= DEC_MAX_B,
+              "s2s_decode_attention: max_pos %d / grid %d / assoc_b %d", a.max_pos, a.grid, a.assoc_b);
+  S2S_REQUIRE((reinterpret_cast<uintptr_t>(a.q) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.kv) & 15) == 0,
+              "s2s_decode_attention: q / kv must be 16-byte aligned");
+  int host[2 * DEC_MAX_B] = {}, max_len = 0;   // slots, then positions (len - 1)
+  for (int b = 0; b < a.B; ++b) {
+    S2S_REQUIRE(a.slots_h[b] >= 0 && a.lens_h[b] >= 1 && a.lens_h[b] <= a.max_pos,
+                "s2s_decode_attention: session %d: slot %d / len %d not in [1, %d]", b, a.slots_h[b], a.lens_h[b], a.max_pos);
+    host[b] = a.slots_h[b];
+    host[DEC_MAX_B + b] = a.lens_h[b] - 1;
+    max_len = std::max(max_len, a.lens_h[b]);
+  }
+  S2S_CHECK_CUDA(cudaSetDevice(ctx->device));
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int grid = a.grid > 0 ? a.grid : dec_grid(ctx);
+  const int kvd = a.kv_heads * a.hd, BH = a.B * a.heads;
+  LlamaDecParams p{};
+  p.heads = a.heads; p.kv_heads = a.kv_heads; p.hd = a.hd; p.B = a.B; p.max_pos = a.max_pos; p.layers = 1;
+  p.q = const_cast<float*>(a.q); p.kv = const_cast<void*>(a.kv); p.attn16 = a.out;
+  p.kv_which_stride = (long long)a.max_pos * kvd; p.kv_layer_stride = 2 * p.kv_which_stride; p.kv_slot_stride = p.kv_layer_stride;
+  p.s_max = (a.max_pos + 63) / 64;   // as llama_create sizes the records
+  p.max_len = max_len; p.assoc_b = a.assoc_b > 0 ? a.assoc_b : a.B;
+  if (plan_out_h) *plan_out_h = attn_plan(p.assoc_b * a.heads, (max_len + ATT_BLK - 1) / ATT_BLK, p.s_max, grid);
+  // per-call scratch: split records, split counters (zeroed), slots and positions
+  const size_t part_bytes = (size_t)BH * p.s_max * (a.hd + PART_PAD) * 4;
+  char* scratch = nullptr;
+  S2S_CHECK_CUDA(cudaMalloc(&scratch, part_bytes + (size_t)BH * 4 + sizeof(host)));
+  p.part = reinterpret_cast<float*>(scratch);
+  p.attn_cnt = reinterpret_cast<unsigned int*>(scratch + part_bytes);
+  int* idx_d = reinterpret_cast<int*>(scratch + part_bytes + (size_t)BH * 4);
+  p.slot = idx_d; p.pos = idx_d + DEC_MAX_B;
+  std::vector<unsigned int> cnt((size_t)BH, 0u);
+  auto run = [&]() -> int {
+    S2S_CHECK_CUDA(cudaMemsetAsync(p.attn_cnt, 0, (size_t)BH * 4, st));
+    S2S_CHECK_CUDA(cudaMemcpyAsync(idx_d, host, sizeof(host), cudaMemcpyHostToDevice, st));
+    const size_t smem = (size_t)DEC_WARPS * (a.hd + PART_PAD) * 4;
+    if (a.dtype == S2S_F16) {
+      if (a.hd == 128) ld_attn_only_kernel<__half, 128><<<grid, DEC_THREADS, smem, st>>>(p);
+      else ld_attn_only_kernel<__half, 64><<<grid, DEC_THREADS, smem, st>>>(p);
+    } else {
+      if (a.hd == 128) ld_attn_only_kernel<__nv_bfloat16, 128><<<grid, DEC_THREADS, smem, st>>>(p);
+      else ld_attn_only_kernel<__nv_bfloat16, 64><<<grid, DEC_THREADS, smem, st>>>(p);
+    }
+    S2S_LAUNCH_CHECK();
+    S2S_CHECK_CUDA(cudaMemcpyAsync(cnt.data(), p.attn_cnt, (size_t)BH * 4, cudaMemcpyDeviceToHost, st));
+    S2S_CHECK_CUDA(cudaStreamSynchronize(st));
+    for (int i = 0; i < BH; ++i)   // the decode launch reuses the counters in its next attention phase
+      S2S_REQUIRE(cnt[i] == 0u, "s2s_decode_attention: split counter of (session %d, head %d) left at %u", i / a.heads,
+                  i % a.heads, cnt[i]);
+    return S2S_OK;
+  };
+  const int rc = run();
+  cudaStreamSynchronize(st);
+  cudaFree(scratch);
+  return rc;
 }

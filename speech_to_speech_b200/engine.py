@@ -276,6 +276,29 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, kv_
     return o
 
 
+def decode_attention(q: torch.Tensor, kv: torch.Tensor, slots: Sequence[int], lens: Sequence[int], heads: int, kv_heads: int,
+                     *, grid: int = 0, assoc_b: int = 0) -> tuple[torch.Tensor, int]:
+    """One attention phase of the Llama-family decode by itself (include/s2s_b200.h s2s_decode_attention).  q: cuda f32
+    [B, heads, hd], softmax scale applied; kv: 16-bit [slots, 2, max_pos, kv_heads * hd] (K rows, then V rows, per slot);
+    session b attends the first lens[b] keys of slot slots[b].  -> (out [B, heads, hd] in kv's dtype, the split plan:
+    splits | 0x80 for warp-level items).  Synchronous."""
+    assert q.is_cuda and q.dtype == torch.float32 and q.dim() == 3 and q.is_contiguous()
+    assert kv.is_cuda and kv.dtype in (torch.float16, torch.bfloat16) and kv.dim() == 4 and kv.shape[1] == 2 and kv.is_contiguous()
+    B, H, hd = q.shape
+    assert H == heads and kv.shape[3] == kv_heads * hd and len(slots) == B and len(lens) == B
+    out = torch.empty((B, heads, hd), dtype=kv.dtype, device=q.device)
+    sl, _ = _lib.i32_array(slots)
+    ln, _ = _lib.i32_array(lens)
+    a = _lib.DecAttnArgs(q=q.data_ptr(), kv=kv.data_ptr(), max_pos=kv.shape[2], slots_h=sl, lens_h=ln, B=B, heads=heads,
+                         kv_heads=kv_heads, hd=hd, dtype={torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[kv.dtype],
+                         grid=grid, assoc_b=assoc_b, out=out.data_ptr())
+    plan = C.c_int32(0)
+    dev = q.device.index or 0
+    check(_lib.load().s2s_decode_attention(get_context(dev), C.byref(a), C.byref(plan), _stream_ptr(dev)),
+          "s2s_decode_attention")
+    return out, int(plan.value)
+
+
 def codec_contract(x: Optional[torch.Tensor], w: torch.Tensor, y: torch.Tensor, *, path: int = 0,
                    x16: Optional[torch.Tensor] = None, T_in: Optional[int] = None, T_out: Optional[int] = None, x_row0: int = 0,
                    dil: int = 1, bias: Optional[torch.Tensor] = None, bias_mod: Optional[int] = None, act: int = 0,
