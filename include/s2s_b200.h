@@ -130,6 +130,17 @@ int s2s_whisper_transcribe(s2s_whisper* m, const s2s_whisper_decode_opts* opts, 
  * out_dtype: S2S_F32 or same as dtype.  act: 0 none, 1 exact GELU.                          */
 int s2s_gemm(s2s_ctx* ctx, const void* a_d, const void* w_d, const float* bias_d, void* c_d, int32_t M,
              int32_t N, int32_t K, int32_t dtype, int32_t out_dtype, int32_t act, void* stream);
+/* The tiled weight layout the Llama-family engines store their projections in, which both the decode kernel and the
+ * prefill GEMMs read: element (row 8t+g, k 32w+8j+e) of a row-major [N, K] matrix at ((t*K/32 + w)*32 + 4g + j)*8 + e.
+ * format S2S_F16 / S2S_BF16: 16-bit elements; S2S_FP8_E4M3: one E4M3 code per element, Q = e4m3(W * 2^-e_n) with the
+ * smallest integer e_n that keeps the row's largest magnitude <= 448, followed by the N fp32 row scales 2^e_n.
+ * s2s_tiled_weight_bytes: the buffer size (0 for an invalid shape or format).  s2s_tile_weights: row-major w_d [N, K]
+ * (bf16 for FP8) -> out_d; N a multiple of 8, K of 32.  s2s_gemm_tiled: s2s_gemm with that operand; FP8 needs bf16 A,
+ * and computes exactly s2s_gemm(A, dq(Q)), dq(Q) = Q * 2^e_n.                                                       */
+int64_t s2s_tiled_weight_bytes(int32_t N, int32_t K, int32_t format);
+int s2s_tile_weights(s2s_ctx* ctx, const void* w_d, int32_t N, int32_t K, int32_t format, void* out_d, void* stream);
+int s2s_gemm_tiled(s2s_ctx* ctx, const void* a_d, const void* wt_d, int32_t format, const float* bias_d, void* c_d, int32_t M,
+                   int32_t N, int32_t K, int32_t dtype, int32_t out_dtype, int32_t act, void* stream);
 /* O = softmax(Q K^T * scale [+causal]) V ; q/k/v/o row-major [T, heads*hd] slices with row strides
  * (elements); kv_heads <= heads (GQA).  hd in {64, 128}.                                     */
 int s2s_attention(s2s_ctx* ctx, const void* q_d, const void* k_d, const void* v_d, void* o_d, int32_t B,
@@ -176,16 +187,22 @@ int s2s_llama_destroy(s2s_llama* m);
 int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, const int64_t* shape,
                           int32_t ndim, int32_t dtype);
 int s2s_llama_init_random(s2s_llama* m, uint64_t seed);
-/* Storage format of the matrices the decode launch streams (q/k/v, o, gate/up, down projections of every layer and
- * lm_head).  `format` = the model's compute_dtype (the default) or S2S_FP8_E4M3: weight-only FP8 with one power-of-two scale
- * per weight row, quantised from the bound 16-bit tensors at finalize.  The row-major matrices the prefill GEMMs read are
- * replaced by the dequantised values, so prefill and decode run ONE model: bit for bit the 16-bit engine bound to those
- * dequantised weights, and a different model from the checkpoint's.  Halves the weight bytes a decode step streams and
- * the decode copy of the weights.  Call after create and before finalize (S2S_ERR_INVALID afterwards); FP8 needs bf16
- * compute and a single-table model (S2S_ERR_UNSUPPORTED otherwise). */
+/* Storage format of the projection matrices (q/k/v, o, gate/up, down of every layer) and lm_head.  The model holds ONE copy
+ * of them, in the tiled layout of s2s_tile_weights, which both the prefill GEMMs and the decode launch read; the embedding
+ * table stays row-major, and a tied lm_head is tiled from it.  `format` = the model's compute_dtype (the default) or
+ * S2S_FP8_E4M3: weight-only FP8 with one power-of-two scale per weight row, quantised from each bound 16-bit tensor as it
+ * is bound.  Prefill expands the codes to the dequantised values, so prefill and decode run ONE model: bit for bit the
+ * 16-bit engine bound to those dequantised weights, and a different model from the checkpoint's.  Halves the weight bytes
+ * a decode step streams and the device memory of those matrices.  Call after create and before the first bind_tensor,
+ * init_random or finalize (S2S_ERR_INVALID afterwards: the matrices are allocated in the format then in force); FP8 needs
+ * bf16 compute and a single-table model (S2S_ERR_UNSUPPORTED otherwise). */
 int s2s_llama_set_weight_format(s2s_llama* m, int32_t format);
 int32_t s2s_llama_weight_format(s2s_llama* m);
 int s2s_llama_finalize(s2s_llama* m);
+/* Device bytes the model object holds: *weights = embedding table(s), norms and the tiled matrices; *total = that plus the
+ * KV cache and every workspace.  The staging buffer of bind_tensor / init_random (as large as the largest matrix tensor)
+ * is held from the first bind to finalize and is not counted. */
+int s2s_llama_device_bytes(s2s_llama* m, int64_t* weights, int64_t* total);
 /* Reset a KV-cache slot (new response).  Also empties the slot's seen-id set (repetition penalty), on the stream of the
  * slot's next prefill or decode. */
 int s2s_llama_session_reset(s2s_llama* m, int32_t slot);

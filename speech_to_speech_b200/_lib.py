@@ -19,10 +19,10 @@ EXPORTED = [
     "s2s_whisper_create", "s2s_whisper_destroy", "s2s_whisper_bind_tensor", "s2s_whisper_init_random",
     "s2s_whisper_finalize", "s2s_whisper_logmel", "s2s_whisper_encode", "s2s_whisper_decode",
     "s2s_whisper_detect_language", "s2s_whisper_transcribe", "s2s_whisper_set_trace", "s2s_whisper_max_decode_batch",
-    "s2s_gemm", "s2s_attention", "s2s_decode_attention",
+    "s2s_gemm", "s2s_tiled_weight_bytes", "s2s_tile_weights", "s2s_gemm_tiled", "s2s_attention", "s2s_decode_attention",
     "s2s_llama_create", "s2s_llama_destroy", "s2s_llama_bind_tensor", "s2s_llama_init_random",
     "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_set_sampling", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
-    "s2s_llama_set_weight_format", "s2s_llama_weight_format",
+    "s2s_llama_set_weight_format", "s2s_llama_weight_format", "s2s_llama_device_bytes",
     "s2s_tts_postproc",
     "s2s_codec_create", "s2s_codec_destroy", "s2s_codec_bind_tensor", "s2s_codec_init_random", "s2s_codec_finalize",
     "s2s_codec_decode", "s2s_codec_samples", "s2s_codec_total_upsample", "s2s_codec_contract",
@@ -150,6 +150,10 @@ def load() -> C.CDLL:
     lib.s2s_whisper_max_decode_batch.argtypes = [vp]
     lib.s2s_whisper_max_decode_batch.restype = i32
     lib.s2s_gemm.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
+    lib.s2s_tiled_weight_bytes.argtypes = [i32, i32, i32]
+    lib.s2s_tiled_weight_bytes.restype = i64
+    lib.s2s_tile_weights.argtypes = [vp, vp, i32, i32, i32, vp, vp]
+    lib.s2s_gemm_tiled.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     lib.s2s_attention.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i64, i64, i64, i64, f32, i32, i32, vp]
     lib.s2s_decode_attention.argtypes = [vp, C.POINTER(DecAttnArgs), C.POINTER(i32), vp]
     lib.s2s_llama_create.argtypes = [vp, C.POINTER(LlamaConfig), C.POINTER(vp)]
@@ -160,6 +164,7 @@ def load() -> C.CDLL:
     lib.s2s_llama_set_weight_format.argtypes = [vp, i32]
     lib.s2s_llama_weight_format.argtypes = [vp]
     lib.s2s_llama_weight_format.restype = i32
+    lib.s2s_llama_device_bytes.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     lib.s2s_llama_session_reset.argtypes = [vp, i32]
     lib.s2s_llama_set_sampling.argtypes = [vp, i32, C.POINTER(Sampling)]
     lib.s2s_llama_prefill.argtypes = [vp, i32, C.POINTER(i32), i32, vp, vp, vp]

@@ -79,6 +79,35 @@ int s2s_gemm(s2s_ctx* ctx, const void* a_d, const void* w_d, const float* bias_d
   return gemm_tc_launch(ctx, p, dtype, (cudaStream_t)stream);
 }
 
+int64_t s2s_tiled_weight_bytes(int32_t N, int32_t K, int32_t format) {
+  if (N < 1 || K < 32 || K % 32 != 0) return 0;
+  if (format == S2S_FP8_E4M3) return (int64_t)tiled_fp8_weight_bytes(N, K);
+  return (format == S2S_F16 || format == S2S_BF16) ? (int64_t)tiled_weight_elems(N, K) * 2 : 0;
+}
+
+int s2s_tile_weights(s2s_ctx* ctx, const void* w_d, int32_t N, int32_t K, int32_t format, void* out_d, void* stream) {
+  S2S_REQUIRE(ctx && w_d && out_d, "s2s_tile_weights: null argument");
+  S2S_REQUIRE(format == S2S_F16 || format == S2S_BF16 || format == S2S_FP8_E4M3, "s2s_tile_weights: unknown format %d", format);
+  S2S_REQUIRE(N >= 8 && N % 8 == 0 && K >= 32 && K % 32 == 0, "s2s_tile_weights: N=%d must be a multiple of 8, K=%d of 32", N, K);
+  S2S_REQUIRE((reinterpret_cast<uintptr_t>(w_d) & 15) == 0 && (reinterpret_cast<uintptr_t>(out_d) & 15) == 0,
+              "s2s_tile_weights: buffers must be 16-byte aligned");
+  return tile_rows_launch(w_d, N, K, out_d, N, 0, 1, format == S2S_FP8_E4M3, (cudaStream_t)stream);
+}
+
+int s2s_gemm_tiled(s2s_ctx* ctx, const void* a_d, const void* wt_d, int32_t format, const float* bias_d, void* c_d, int32_t M,
+                   int32_t N, int32_t K, int32_t dtype, int32_t out_dtype, int32_t act, void* stream) {
+  S2S_REQUIRE(ctx && a_d && wt_d && c_d, "s2s_gemm_tiled: null argument");
+  S2S_REQUIRE(format == dtype || (format == S2S_FP8_E4M3 && dtype == S2S_BF16),
+              "s2s_gemm_tiled: format %d must be the operand dtype, or FP8 with bf16 operands", format);
+  GemmProblem p{};
+  p.a = a_d; p.a_row_stride = K; p.a_batch_stride = (int64_t)K * M; p.w = wt_d;
+  p.w_layout = format == S2S_FP8_E4M3 ? GEMM_W_TILED_FP8 : GEMM_W_TILED16;
+  p.M = M; p.N = N; p.K = K; p.batch = 1; p.bias = bias_d; p.act = act;
+  if (out_dtype == S2S_F32) { p.out_f = (float*)c_d; p.ldo_f = N; }
+  else { S2S_REQUIRE(out_dtype == dtype, "s2s_gemm_tiled: out_dtype must be f32 or the operand dtype"); p.out_h = c_d; p.ldo_h = N; }
+  return gemm_tc_launch(ctx, p, dtype, (cudaStream_t)stream);
+}
+
 int s2s_attention(s2s_ctx* ctx, const void* q_d, const void* k_d, const void* v_d, void* o_d, int32_t B, int32_t Tq,
                   int32_t Tk, int32_t heads, int32_t kv_heads, int32_t hd, int64_t ldq, int64_t ldk, int64_t ldv,
                   int64_t ldo, float scale, int32_t causal, int32_t dtype, void* stream) {

@@ -9,11 +9,27 @@
 //
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = MMA + epilogue.
 //
+// The weight operand W comes in one of three layouts (GemmProblem::w_layout, a template parameter of the kernel):
+//   * row-major [N, ldw], 128-byte swizzle, as above (Whisper, the codec, s2s_gemm);
+//   * the fragment-major 16-bit tiles the decode kernels stream (weight_tiles.cu).  Each 32-k window of an 8-row tile is
+//     a contiguous 8 x 64 B block, so a 4-D TMA map {32 k, 8 rows, windows, tiles} with the 64-byte swizzle lands the
+//     k-block as [tile][window][8 rows][64 B] swizzle-64B atoms, which wgmma reads as a K-major operand (one 8-row group
+//     = BK/32 atoms = 1024 B).  The wgmma sequence and its k order are those of the row-major path, so the result is
+//     bit for bit the same;
+//   * FP8 E4M3 codes in the same tiling + one power-of-two scale per row (bf16 only).  TMA loads the codes; warps 1-3 of
+//     the producer warpgroup expand them times the row scale into the bf16 swizzle-64B buffer of the 16-bit tiled path
+//     (exact: dq(Q) is a bf16 number) and then release the stage to the MMA warpgroups.  That warpgroup is otherwise
+//     idle, so the MMA issue and the epilogue are those of the 16-bit paths.
+// The Llama-family prefill reads its projections and lm_head in the tiled layouts, the one copy the decode kernel streams.
+//
 // Used for every GEMM-shaped op with M >= 64 on the hot path: Whisper conv1/conv2 (as strided-window
 // GEMMs, no im2col), QKV / out-proj / fc1 / fc2 of the encoder, the cross-attention K/V projection and
 // the LLM prefill projections.  (Reference ops: transformers modeling_whisper.py:284-357,380-414,619-625;
 // modeling_llama.py:171-289.)
+#include <cuda_fp8.h>
+
 #include "gemm_tc.cuh"
+#include "kernels.cuh"
 #include "wgmma.cuh"
 
 namespace {
@@ -23,12 +39,16 @@ constexpr int BK = 64;  // 64 x 16-bit = 128 B = one swizzle atom
 constexpr int NTHREADS = 384;
 constexpr int CONSUMERS = 256;  // threads of the two MMA warpgroups
 
-template <int BN> struct TileCfg {
-  static constexpr int STAGES = (BN == 64) ? 8 : 6;
+constexpr int CONVERTERS = 96;  // FP8 weights: warps 1-3 of the producer warpgroup expand the codes
+
+template <int BN, int WL> struct TileCfg {
+  static constexpr bool F8 = WL == GEMM_W_TILED_FP8;
+  static constexpr int STAGES = (BN == 64) ? 8 : (F8 ? 5 : 6);
   static constexpr int A_BYTES = BM * BK * 2;
-  static constexpr int B_BYTES = BN * BK * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static constexpr int B_BYTES = BN * BK * 2;     // the 16-bit weight tile wgmma reads
+  static constexpr int Q_BYTES = F8 ? BN * BK : 0;  // FP8: the codes as loaded, expanded into the B buffer
+  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES + Q_BYTES;
+  static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/ + (F8 ? BN * 4 : 0) /*row scales*/;
 };
 
 struct EpiParams {
@@ -80,16 +100,42 @@ __device__ __forceinline__ void epilogue_pair(const EpiParams& ep, int batch, in
   }
 }
 
-template <typename T, int BN>
+// FP8 weights: expand one stage's E4M3 codes (layout [tile][window][8 rows][32 B], as loaded) into the bf16 B buffer in
+// the swizzle-64B layout TMA gives the 16-bit tiled operand, times the row scales: dq(Q) = Q * 2^e_n is a bf16 number,
+// so the values wgmma multiplies by are exactly those of the 16-bit engine bound to dq(Q).
+template <int BN>
+__device__ __forceinline__ void expand_fp8_stage(const uint8_t* sq, uint8_t* sb, const float* s_scale, int ct) {
+#pragma unroll 2
+  for (int c = ct; c < BN * BK / 16; c += CONVERTERS) {  // 16 codes = half of one 32-k row of a window
+    const uint4 q = *reinterpret_cast<const uint4*>(sq + c * 16);
+    const int r = c >> 1, h = c & 1;                      // r = (tile * BK/32 + window) * 8 + row: one 64-B line of sb
+    const float sc = s_scale[(r >> 4) * 8 + (r & 7)];
+    const uint32_t qs[4] = {q.x, q.y, q.z, q.w};
+    uint32_t o[8];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const __half2_raw hr = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(qs[i >> 1] >> (16 * (i & 1))), __NV_E4M3);
+      o[i] = DT<__nv_bfloat16>::pack2(__half2float(__half(__half_raw{hr.x})) * sc, __half2float(__half(__half_raw{hr.y})) * sc);
+    }
+    const int sw = (r >> 1) & 3;                          // swizzle-64B: 16-B chunk ^= address bits [7, 9)
+    *reinterpret_cast<uint4*>(sb + r * 64 + ((2 * h) ^ sw) * 16) = make_uint4(o[0], o[1], o[2], o[3]);
+    *reinterpret_cast<uint4*>(sb + r * 64 + ((2 * h + 1) ^ sw) * 16) = make_uint4(o[4], o[5], o[6], o[7]);
+  }
+}
+
+template <typename T, int BN, int WL>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
-               const EpiParams ep) {
-  using Cfg = TileCfg<BN>;
+               const float* __restrict__ w_scale, const EpiParams ep) {
+  using Cfg = TileCfg<BN, WL>;
+  constexpr bool F8 = Cfg::F8;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128-byte swizzle pattern (TMA and wgmma must agree)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
+  uint64_t* load_bar = empty_bar + Cfg::STAGES;   // FP8: the TMA loads of a stage; full_bar then means "codes expanded"
+  float* s_scale = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES + 256);
 
   const int wg = threadIdx.x >> 7;
   const int n_tile = blockIdx.x, m_tile = blockIdx.y, batch = blockIdx.z;
@@ -99,8 +145,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     tma_prefetch_desc(&map_a);
     tma_prefetch_desc(&map_w);
     for (int s = 0; s < Cfg::STAGES; ++s) {
-      mbar_init(&full_bar[s], 1);
+      mbar_init(&full_bar[s], F8 ? CONVERTERS : 1);
       mbar_init(&empty_bar[s], CONSUMERS);
+      if (F8) mbar_init(&load_bar[s], 1);
     }
     fence_barrier_init();
   }
@@ -115,9 +162,24 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         mbar_wait(&empty_bar[s], ph ^ 1);
         uint8_t* sa = smem + s * Cfg::STAGE_BYTES;
         uint8_t* sb = sa + Cfg::A_BYTES;
-        mbar_expect_tx(&full_bar[s], Cfg::STAGE_BYTES);
-        tma_load_3d(sa, &map_a, &full_bar[s], kb * BK, m_tile * BM, batch);
-        tma_load_2d(sb, &map_w, &full_bar[s], kb * BK, n_tile * BN);
+        uint64_t* bar = F8 ? &load_bar[s] : &full_bar[s];
+        mbar_expect_tx(bar, Cfg::A_BYTES + (F8 ? Cfg::Q_BYTES : Cfg::B_BYTES));
+        tma_load_3d(sa, &map_a, bar, kb * BK, m_tile * BM, batch);
+        if (WL == GEMM_W_ROW_MAJOR) tma_load_2d(sb, &map_w, bar, kb * BK, n_tile * BN);
+        else tma_load_4d(F8 ? sb + Cfg::B_BYTES : sb, &map_w, bar, 0, 0, kb * (BK / 32), n_tile * (BN / 8));
+      }
+    } else if (F8 && threadIdx.x >= 32) {
+      // The producer warpgroup is otherwise idle, so the expansion costs the MMA warpgroups nothing.
+      const int ct = threadIdx.x - 32;
+      for (int i = ct; i < BN; i += CONVERTERS) s_scale[i] = w_scale[n_tile * BN + i];
+      asm volatile("bar.sync 1, %0;" ::"n"(CONVERTERS) : "memory");
+      for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % Cfg::STAGES;
+        mbar_wait(&load_bar[s], (kb / Cfg::STAGES) & 1);
+        uint8_t* sb = smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES;
+        expand_fp8_stage<BN>(sb + Cfg::B_BYTES, sb, s_scale, ct);
+        fence_proxy_async();   // generic-proxy stores -> wgmma's async-proxy reads
+        mbar_arrive(&full_bar[s]);
       }
     }
     return;
@@ -130,15 +192,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
   for (int kb = 0; kb < num_kb; ++kb) {
     const int s = kb % Cfg::STAGES;
+    if (F8) mbar_wait(&load_bar[s], (kb / Cfg::STAGES) & 1);   // the A tile
     mbar_wait(&full_bar[s], (kb / Cfg::STAGES) & 1);
     const uint32_t sa = smem_u32(smem + s * Cfg::STAGE_BYTES) + cw * (64 * 128);
     const uint32_t sb = smem_u32(smem + s * Cfg::STAGE_BYTES + Cfg::A_BYTES);
     const uint64_t adesc = wgmma_desc_sw128(sa);
-    const uint64_t bdesc = wgmma_desc_sw128(sb);
     wgmma_fence_operand(acc);
     wgmma_fence();
+    if (WL == GEMM_W_ROW_MAJOR) {
+      const uint64_t bdesc = wgmma_desc_sw128(sb);
 #pragma unroll
-    for (int k = 0; k < BK / 16; ++k) wgmma_ss<T, BN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1u);
+      for (int k = 0; k < BK / 16; ++k) wgmma_ss<T, BN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)(k * 2), 1u);
+    } else {
+      // tiled: [tile][window][8 rows][64 B] swizzle-64B atoms; one tile (8 rows) = BK/32 windows = 1024 B; k16 step k
+      // reads window k/2 at byte (k%2) * 32
+      const uint64_t bdesc = wgmma_desc_sw64(sb, (BK / 32) * 512);
+#pragma unroll
+      for (int k = 0; k < BK / 16; ++k)
+        wgmma_ss<T, BN>(acc, adesc + (uint64_t)(k * 2), bdesc + (uint64_t)((k >> 1) * 32 + (k & 1) * 2), 1u);
+    }
     wgmma_commit();
     wgmma_wait<1>();  // the previous k-block's MMAs have retired: its stage may be refilled
     wgmma_fence_operand(acc);
@@ -165,7 +237,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
 }  // namespace
 
 int tma_encode_map(s2s_ctx* ctx, CUtensorMap* map, CUtensorMapDataType dt, int rank, const void* base,
-                   const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box) {
+                   const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
   cuuint32_t estr[5] = {1, 1, 1, 1, 1};
   EncodeTiledFn fn = reinterpret_cast<EncodeTiledFn>(ctx->encode_tiled);
   if (!fn) {
@@ -173,7 +245,7 @@ int tma_encode_map(s2s_ctx* ctx, CUtensorMap* map, CUtensorMapDataType dt, int r
     return S2S_ERR_CUDA;
   }
   CUresult r = fn(map, dt, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     s2s_set_error("cuTensorMapEncodeTiled failed (%d): rank %d dims [%llu,%llu,%llu] strides [%llu,%llu]", (int)r,
@@ -187,9 +259,9 @@ int tma_encode_map(s2s_ctx* ctx, CUtensorMap* map, CUtensorMapDataType dt, int r
 
 namespace {
 
-template <typename T, int BN>
+template <typename T, int BN, int WL>
 int launch_impl(s2s_ctx* ctx, const GemmProblem& p, cudaStream_t stream) {
-  using Cfg = TileCfg<BN>;
+  using Cfg = TileCfg<BN, WL>;
   CUtensorMap map_a, map_w;
   {
     cuuint64_t dims[3] = {(cuuint64_t)p.K, (cuuint64_t)p.M, (cuuint64_t)p.batch};
@@ -198,11 +270,21 @@ int launch_impl(s2s_ctx* ctx, const GemmProblem& p, cudaStream_t stream) {
     cuuint32_t box[3] = {BK, BM, 1};
     S2S_CHECK(tma_encode_map(ctx, &map_a, DT<T>::tma, 3, p.a, dims, strides, box));
   }
-  {
+  const float* w_scale = nullptr;
+  if (WL == GEMM_W_ROW_MAJOR) {
     cuuint64_t dims[2] = {(cuuint64_t)p.K, (cuuint64_t)p.N};
     cuuint64_t strides[1] = {(cuuint64_t)p.ldw * 2};
     cuuint32_t box[2] = {BK, BN};
     S2S_CHECK(tma_encode_map(ctx, &map_w, DT<T>::tma, 2, p.w, dims, strides, box));
+  } else {
+    // the tiled layout as (k in window, row in tile, window, tile): each 32-k window of an 8-row tile is an 8 x 32 block
+    const cuuint64_t esz = Cfg::F8 ? 1 : 2;
+    cuuint64_t dims[4] = {32, 8, (cuuint64_t)p.K / 32, (cuuint64_t)p.N / 8};
+    cuuint64_t strides[3] = {32 * esz, 256 * esz, (cuuint64_t)p.K / 32 * 256 * esz};
+    cuuint32_t box[4] = {32, 8, BK / 32, BN / 8};
+    S2S_CHECK(tma_encode_map(ctx, &map_w, Cfg::F8 ? CU_TENSOR_MAP_DATA_TYPE_UINT8 : DT<T>::tma, 4, p.w, dims, strides, box,
+                             Cfg::F8 ? CU_TENSOR_MAP_SWIZZLE_NONE : CU_TENSOR_MAP_SWIZZLE_64B));
+    if (Cfg::F8) w_scale = reinterpret_cast<const float*>(reinterpret_cast<const char*>(p.w) + tiled_weight_elems(p.N, p.K));
   }
   EpiParams ep;
   ep.bias = p.bias; ep.act = p.act; ep.out_h = p.out_h; ep.ldo_h = p.ldo_h; ep.out_f = p.out_f; ep.ldo_f = p.ldo_f;
@@ -210,15 +292,21 @@ int launch_impl(s2s_ctx* ctx, const GemmProblem& p, cudaStream_t stream) {
   ep.out_batch_rows = p.out_batch_rows; ep.out_row_offset = p.out_row_offset; ep.head_major_rows = p.head_major_rows;
   ep.M = p.M; ep.N = p.N; ep.K = p.K;
 
-  static bool attr_set = false;  // per (T,BN) instantiation
+  static bool attr_set = false;  // per (T,BN,WL) instantiation
   if (!attr_set) {
-    S2S_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<T, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
+    S2S_CHECK_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<T, BN, WL>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM));
     attr_set = true;
   }
   dim3 grid(p.N / BN, (p.M + BM - 1) / BM, p.batch);
-  gemm_tc_kernel<T, BN><<<grid, NTHREADS, Cfg::SMEM, stream>>>(map_a, map_w, ep);
+  gemm_tc_kernel<T, BN, WL><<<grid, NTHREADS, Cfg::SMEM, stream>>>(map_a, map_w, w_scale, ep);
   S2S_LAUNCH_CHECK();
   return S2S_OK;
+}
+
+template <typename T, int BN>
+int launch_layout(s2s_ctx* ctx, const GemmProblem& p, cudaStream_t stream) {
+  if (p.w_layout == GEMM_W_TILED16) return launch_impl<T, BN, GEMM_W_TILED16>(ctx, p, stream);
+  return launch_impl<T, BN, GEMM_W_ROW_MAJOR>(ctx, p, stream);
 }
 
 }  // namespace
@@ -226,17 +314,25 @@ int launch_impl(s2s_ctx* ctx, const GemmProblem& p, cudaStream_t stream) {
 int gemm_tc_launch(s2s_ctx* ctx, const GemmProblem& p, int dtype, cudaStream_t stream) {
   S2S_REQUIRE(p.N % 64 == 0, "gemm: N=%d must be a multiple of 64", p.N);
   S2S_REQUIRE(p.K % 8 == 0 && p.K > 0, "gemm: K=%d must be a positive multiple of 8", p.K);
-  S2S_REQUIRE(p.a_row_stride % 8 == 0 && p.ldw % 8 == 0, "gemm: row strides must be multiples of 8 elements");
+  S2S_REQUIRE(p.a_row_stride % 8 == 0, "gemm: row strides must be multiples of 8 elements");
+  S2S_REQUIRE(p.w_layout >= GEMM_W_ROW_MAJOR && p.w_layout <= GEMM_W_TILED_FP8, "gemm: unknown weight layout %d", p.w_layout);
+  if (p.w_layout == GEMM_W_ROW_MAJOR) S2S_REQUIRE(p.ldw % 8 == 0, "gemm: row strides must be multiples of 8 elements");
+  else S2S_REQUIRE(p.K % 32 == 0, "gemm: K=%d must be a multiple of 32 with a tiled weight operand", p.K);
+  S2S_REQUIRE(p.w_layout != GEMM_W_TILED_FP8 || dtype == S2S_BF16, "gemm: FP8 weights need bf16 activations");
   S2S_REQUIRE((reinterpret_cast<uintptr_t>(p.a) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.w) & 15) == 0,
               "gemm: operands must be 16-byte aligned");
   S2S_REQUIRE(p.M > 0 && p.batch > 0, "gemm: empty problem");
   // Pick the N tile so the grid covers every SM when the problem allows it.
   const long long tiles128 = (long long)(p.N / 128) * ((p.M + BM - 1) / BM) * p.batch;
   const bool use128 = (p.N % 128 == 0) && tiles128 >= ctx->num_sms;
+  if (p.w_layout == GEMM_W_TILED_FP8) {
+    return use128 ? launch_impl<__nv_bfloat16, 128, GEMM_W_TILED_FP8>(ctx, p, stream)
+                  : launch_impl<__nv_bfloat16, 64, GEMM_W_TILED_FP8>(ctx, p, stream);
+  }
   if (dtype == S2S_F16) {
-    return use128 ? launch_impl<__half, 128>(ctx, p, stream) : launch_impl<__half, 64>(ctx, p, stream);
+    return use128 ? launch_layout<__half, 128>(ctx, p, stream) : launch_layout<__half, 64>(ctx, p, stream);
   } else if (dtype == S2S_BF16) {
-    return use128 ? launch_impl<__nv_bfloat16, 128>(ctx, p, stream) : launch_impl<__nv_bfloat16, 64>(ctx, p, stream);
+    return use128 ? launch_layout<__nv_bfloat16, 128>(ctx, p, stream) : launch_layout<__nv_bfloat16, 64>(ctx, p, stream);
   }
   s2s_set_error("gemm: unsupported dtype %d", dtype);
   return S2S_ERR_UNSUPPORTED;

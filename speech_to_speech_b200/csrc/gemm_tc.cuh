@@ -30,10 +30,16 @@ struct GemmProblem {
   // > 0: out_h is written as [row / R][N / 64][R][64] (R = head_major_rows): every 64-column block (one attention head)
   // of a row range is contiguous -- the layout the decode kernels stream K/V in.  0: plain row-major with ldo_h.
   int32_t head_major_rows;
+  // layout of w: GEMM_W_ROW_MAJOR [N, ldw]; GEMM_W_TILED16 = weight_tiles.cu's fragment-major 16-bit tiles (ldw unused,
+  // K a multiple of 32); GEMM_W_TILED_FP8 = E4M3 codes in that tiling followed by the fp32 row scales (bf16 only)
+  int32_t w_layout;
 };
+
+enum GemmWeightLayout { GEMM_W_ROW_MAJOR = 0, GEMM_W_TILED16 = 1, GEMM_W_TILED_FP8 = 2 };
 
 int gemm_tc_launch(s2s_ctx* ctx, const GemmProblem& p, int dtype, cudaStream_t stream);
 
-// 128-byte-swizzled tiled TMA descriptor (cuTensorMapEncodeTiled through the runtime-resolved driver entry point)
+// tiled TMA descriptor (cuTensorMapEncodeTiled through the runtime-resolved driver entry point), 128-byte swizzle by default
 int tma_encode_map(s2s_ctx* ctx, CUtensorMap* map, CUtensorMapDataType dt, int rank, const void* base,
-                   const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box);
+                   const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box,
+                   CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B);

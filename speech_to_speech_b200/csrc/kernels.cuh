@@ -30,7 +30,8 @@ int fill_random_launch(void* dst, long long n, int dtype, float scale, float off
 // row-major 16-bit [N, K] -> fragment-major tiled layout streamed by the decode kernels (see decode_common.cuh)
 size_t tiled_weight_elems(int N, int K);
 int tile_weights_launch(const void* W, int N, int K, void* Wt, cudaStream_t stream);
-// FP8 E4M3 weight-only quantisation with a power-of-two scale per row: W (row-major bf16 [N, K]) -> Wq = tiled E4M3 codes
-// followed by roundup8(N) fp32 row scales (tiled_fp8_weight_bytes), and W is overwritten with the dequantised values
+// FP8 E4M3 weight-only storage with a power-of-two scale per row: tiled E4M3 codes followed by roundup8(N) fp32 row scales
 size_t tiled_fp8_weight_bytes(int N, int K);
-int quantize_tile_weights_fp8_launch(void* W, int N, int K, void* Wq, cudaStream_t stream);
+// the `rows` rows of a row-major 16-bit [rows, K] source -> rows row0 + r * rstride of the tiled [N, K] matrix Wt: 16-bit
+// tiles, or (fp8, bf16 source) E4M3 codes + row scales.  The other rows of Wt are left as they are.
+int tile_rows_launch(const void* src, int rows, int K, void* Wt, int N, int row0, int rstride, bool fp8, cudaStream_t stream);

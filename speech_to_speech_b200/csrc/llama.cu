@@ -130,53 +130,34 @@ int build(s2s_llama* m) {
   auto off = [&](void* base, int64_t elems) { return reinterpret_cast<char*>(base) + elems * esz; };
   m->n_tables = c.n_tables > 1 ? c.n_tables : 1;
   m->embed_table_elems = (size_t)c.vocab * d;
-  m->head_table_elems = (size_t)c.vocab * d;
-  S2S_CHECK(m->arena.alloc(&m->embed, m->n_tables * m->embed_table_elems * esz));
-  S2S_CHECK(m->arena.alloc(&m->lm_head, m->n_tables * m->head_table_elems * esz));
-  S2S_CHECK(m->arena.alloc(&m->norm_f, d * 4));
+  S2S_CHECK(m->arena.alloc_weights(&m->embed, m->n_tables * m->embed_table_elems * esz));
+  S2S_CHECK(m->arena.alloc_weights(&m->norm_f, d * 4));
   WeightArena& A = m->arena;
   if (m->n_tables == 1) {
     A.add("model.embed_tokens.weight", m->embed, true, (int64_t)c.vocab * d);
-    A.add("lm_head.weight", m->lm_head, true, (int64_t)c.vocab * d);
   } else {  // code predictor: one table / head per codebook (Qwen3OmniMoeTalkerCodePredictorModel.codec_embedding, .lm_head)
-    for (int t = 0; t < m->n_tables; ++t) {
+    for (int t = 0; t < m->n_tables; ++t)
       A.add("model.embed_tokens." + std::to_string(t) + ".weight", off(m->embed, (int64_t)t * m->embed_table_elems), true, (int64_t)c.vocab * d);
-      A.add("lm_head." + std::to_string(t) + ".weight", off(m->lm_head, (int64_t)t * m->head_table_elems), true, (int64_t)c.vocab * d);
-    }
   }
   A.add("model.norm.weight", m->norm_f, false, d, 0.1f, 1.0f);
   m->layers_h.resize(c.layers);
-  const float sd = 1.0f / sqrtf((float)d);
   for (int i = 0; i < c.layers; ++i) {
     const std::string p = "model.layers." + std::to_string(i) + ".";
-    void *w_qkv, *w_o, *w_gu, *w_down;
     float *n1, *n2, *qn = nullptr, *kn = nullptr;
-    S2S_CHECK(A.alloc(&w_qkv, (size_t)(qd + 2 * kvd) * d * esz));
-    S2S_CHECK(A.alloc(&w_o, (size_t)d * qd * esz));
-    S2S_CHECK(A.alloc(&w_gu, (size_t)2 * f * d * esz));
-    S2S_CHECK(A.alloc(&w_down, (size_t)d * f * esz));
-    S2S_CHECK(A.alloc(&n1, d * 4));
-    S2S_CHECK(A.alloc(&n2, d * 4));
-    A.add(p + "self_attn.q_proj.weight", w_qkv, true, (int64_t)qd * d, 2.0f * sd).as(W_ROPE_PERM, qd, d, 0, hd);
-    A.add(p + "self_attn.k_proj.weight", off(w_qkv, (int64_t)qd * d), true, (int64_t)kvd * d, 2.0f * sd).as(W_ROPE_PERM, kvd, d, 0, hd);
-    A.add(p + "self_attn.v_proj.weight", off(w_qkv, (int64_t)(qd + kvd) * d), true, (int64_t)kvd * d, 0.8f * sd);
-    A.add(p + "self_attn.o_proj.weight", w_o, true, (int64_t)d * qd, 1.0f * sd);
-    A.add(p + "mlp.gate_proj.weight", w_gu, true, (int64_t)f * d, 1.0f * sd).as(W_INTERLEAVE, f, d, 0, 0);
-    A.add(p + "mlp.up_proj.weight", w_gu, true, (int64_t)f * d, 1.0f * sd).as(W_INTERLEAVE, f, d, 0, 1);
-    A.add(p + "mlp.down_proj.weight", w_down, true, (int64_t)d * f, 0.7f / sqrtf((float)f));
+    S2S_CHECK(A.alloc_weights(&n1, d * 4));
+    S2S_CHECK(A.alloc_weights(&n2, d * 4));
     A.add(p + "input_layernorm.weight", n1, false, d, 0.1f, 1.0f);
     A.add(p + "post_attention_layernorm.weight", n2, false, d, 0.1f, 1.0f);
     if (c.qk_norm) {  // Qwen3Attention.q_norm / k_norm: RMSNorm(head_dim), permuted like the q/k rows
-      S2S_CHECK(A.alloc(&qn, hd * 4));
-      S2S_CHECK(A.alloc(&kn, hd * 4));
+      S2S_CHECK(A.alloc_weights(&qn, hd * 4));
+      S2S_CHECK(A.alloc_weights(&kn, hd * 4));
       A.add(p + "self_attn.q_norm.weight", qn, false, hd, 0.1f, 1.0f).as(W_ROPE_PERM, hd, 1, 0, hd);
       A.add(p + "self_attn.k_norm.weight", kn, false, hd, 0.1f, 1.0f).as(W_ROPE_PERM, hd, 1, 0, hd);
     }
     LlamaDecLayer& L = m->layers_h[i];
-    L.w_qkv = w_qkv; L.w_o = w_o; L.w_gu = w_gu; L.w_down = w_down; L.norm1 = n1; L.norm2 = n2; L.q_norm = qn; L.k_norm = kn;
+    L.norm1 = n1; L.norm2 = n2; L.q_norm = qn; L.k_norm = kn;
   }
   S2S_CHECK(m->arena.alloc(&m->layers_d, sizeof(LlamaDecLayer) * c.layers));
-  S2S_CHECK_CUDA(cudaMemcpy(m->layers_d, m->layers_h.data(), sizeof(LlamaDecLayer) * c.layers, cudaMemcpyHostToDevice));
 
   // RoPE table, float32 arithmetic like LlamaRotaryEmbedding (modeling_llama.py:73-137)
   {
@@ -239,10 +220,55 @@ int build(s2s_llama* m) {
   return S2S_OK;
 }
 
-GemmProblem lgemm(const void* a, int64_t lda, const void* w, int64_t ldw, int64_t M, int N, int K) {
+// The projections and lm_head, stored once in the tiled layout that the decode kernel streams and the prefill GEMMs read
+// (16-bit tiles, or FP8 codes + row scales).  Allocated at the first bind / init_random / finalize, which fixes the weight
+// format; bind and init_random write each tensor's rows straight into place.
+int alloc_matrices(s2s_llama* m) {
+  if (m->matrices) return S2S_OK;
+  const auto& c = m->cfg;
+  const int d = c.d_model, f = c.ffn, hd = c.head_dim, qd = c.heads * hd, kvd = c.kv_heads * hd, nqkv = qd + 2 * kvd;
+  const bool f8 = m->weight_format == S2S_FP8_E4M3;
+  auto tbytes = [f8](int N, int K) { return f8 ? tiled_fp8_weight_bytes(N, K) : tiled_weight_elems(N, K) * 2; };
+  WeightArena& A = m->arena;
+  A.tiled_format = m->weight_format;
+  const float sd = 1.0f / sqrtf((float)d);
+  for (int i = 0; i < c.layers; ++i) {
+    const std::string p = "model.layers." + std::to_string(i) + ".";
+    void *w_qkv, *w_o, *w_gu, *w_down;
+    S2S_CHECK(A.alloc_weights(&w_qkv, tbytes(nqkv, d)));
+    S2S_CHECK(A.alloc_weights(&w_o, tbytes(d, qd)));
+    S2S_CHECK(A.alloc_weights(&w_gu, tbytes(2 * f, d)));
+    S2S_CHECK(A.alloc_weights(&w_down, tbytes(d, f)));
+    A.add(p + "self_attn.q_proj.weight", w_qkv, true, (int64_t)qd * d, 2.0f * sd).as(W_ROPE_PERM, qd, d, 0, hd).tiled(nqkv, d, 0);
+    A.add(p + "self_attn.k_proj.weight", w_qkv, true, (int64_t)kvd * d, 2.0f * sd).as(W_ROPE_PERM, kvd, d, 0, hd).tiled(nqkv, d, qd);
+    A.add(p + "self_attn.v_proj.weight", w_qkv, true, (int64_t)kvd * d, 0.8f * sd).tiled(nqkv, d, qd + kvd);
+    A.add(p + "self_attn.o_proj.weight", w_o, true, (int64_t)d * qd, 1.0f * sd).tiled(d, qd);
+    A.add(p + "mlp.gate_proj.weight", w_gu, true, (int64_t)f * d, 1.0f * sd).as(W_INTERLEAVE, f, d, 0, 0).tiled(2 * f, d, 0, 2);
+    A.add(p + "mlp.up_proj.weight", w_gu, true, (int64_t)f * d, 1.0f * sd).as(W_INTERLEAVE, f, d, 0, 1).tiled(2 * f, d, 1, 2);
+    A.add(p + "mlp.down_proj.weight", w_down, true, (int64_t)d * f, 0.7f / sqrtf((float)f)).tiled(d, f);
+    LlamaDecLayer& L = m->layers_h[i];
+    L.w_qkv = w_qkv; L.w_o = w_o; L.w_gu = w_gu; L.w_down = w_down;
+  }
+  m->head_t_table_elems = tiled_weight_elems(c.vocab, d);
+  S2S_CHECK(A.alloc_weights(&m->lm_head_t, f8 ? tbytes(c.vocab, d) : m->n_tables * m->head_t_table_elems * 2));
+  if (m->n_tables == 1) {
+    A.add("lm_head.weight", m->lm_head_t, true, (int64_t)c.vocab * d).tiled(c.vocab, d);
+  } else {
+    for (int t = 0; t < m->n_tables; ++t)
+      A.add("lm_head." + std::to_string(t) + ".weight", reinterpret_cast<char*>(m->lm_head_t) + (size_t)t * m->head_t_table_elems * 2,
+            true, (int64_t)c.vocab * d).tiled(c.vocab, d);
+  }
+  S2S_CHECK_CUDA(cudaMemcpy(m->layers_d, m->layers_h.data(), sizeof(LlamaDecLayer) * c.layers, cudaMemcpyHostToDevice));
+  m->matrices = true;
+  return S2S_OK;
+}
+
+// a prefill GEMM over one of the model's tiled matrices
+GemmProblem lgemm(const s2s_llama* m, const void* a, int64_t lda, const void* w, int64_t M, int N, int K) {
   GemmProblem p{};
-  p.a = a; p.a_row_stride = lda; p.a_batch_stride = lda * M; p.w = w; p.ldw = ldw;
+  p.a = a; p.a_row_stride = lda; p.a_batch_stride = lda * M; p.w = w;
   p.M = (int32_t)M; p.N = N; p.K = K; p.batch = 1;
+  p.w_layout = m->weight_format == S2S_FP8_E4M3 ? GEMM_W_TILED_FP8 : GEMM_W_TILED16;
   return p;
 }
 
@@ -334,7 +360,7 @@ static int prefill_layers(s2s_llama* m, const PrefillSeg* segs, int nseg, int R,
     const LlamaDecLayer& L = m->layers_h[i];
     S2S_CHECK(norm_rows_launch(m->x, L.norm1, nullptr, c.rms_eps, R, d, m->xn, nullptr, dt, st));
     {
-      GemmProblem p = lgemm(m->xn, d, L.w_qkv, d, R, ldq, d);
+      GemmProblem p = lgemm(m, m->xn, d, L.w_qkv, R, ldq, d);
       p.out_h = m->qkv; p.ldo_h = ldq;
       S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
     }
@@ -361,18 +387,18 @@ static int prefill_layers(s2s_llama* m, const PrefillSeg* segs, int nseg, int R,
                                      c.heads, c.kv_heads, hd, ldq, kvd, kvd, qd, 1.0f / sqrtf((float)hd), 1, dt, m->vt, m->vt_elems, st));
     }
     {
-      GemmProblem p = lgemm(m->attn, qd, L.w_o, qd, R, d, qd);
+      GemmProblem p = lgemm(m, m->attn, qd, L.w_o, R, d, qd);
       p.out_f = m->x; p.ldo_f = d; p.resid = m->x; p.ld_resid = d; p.resid_mode = 1;
       S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
     }
     S2S_CHECK(norm_rows_launch(m->x, L.norm2, nullptr, c.rms_eps, R, d, m->xn, nullptr, dt, st));
     {
-      GemmProblem p = lgemm(m->xn, d, L.w_gu, d, R, 2 * f, d);
+      GemmProblem p = lgemm(m, m->xn, d, L.w_gu, R, 2 * f, d);
       p.act = 2; p.out_h = m->hbuf; p.ldo_h = f;
       S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
     }
     {
-      GemmProblem p = lgemm(m->hbuf, f, L.w_down, f, R, d, f);
+      GemmProblem p = lgemm(m, m->hbuf, f, L.w_down, R, d, f);
       p.out_f = m->x; p.ldo_f = d; p.resid = m->x; p.ld_resid = d; p.resid_mode = 1;
       S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
     }
@@ -393,7 +419,7 @@ int llama_prefill_rows(s2s_llama* m, int slot, int n, float* logits_out_d, int32
     S2S_CHECK_CUDA(cudaMemcpyAsync(hidden_out_d, m->x + (size_t)(n - 1) * d, (size_t)d * 4, cudaMemcpyDeviceToDevice, st));
   S2S_CHECK(norm_rows_launch(m->x, m->norm_f, nullptr, c.rms_eps, n, d, m->xn, nullptr, dt, st));
   if (logits_out_d) {
-    GemmProblem p = lgemm(m->xn, d, m->lm_head, d, n, c.vocab, d);
+    GemmProblem p = lgemm(m, m->xn, d, m->lm_head_t, n, c.vocab, d);
     p.out_f = logits_out_d; p.ldo_f = c.vocab;
     S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
   }
@@ -402,7 +428,7 @@ int llama_prefill_rows(s2s_llama* m, int slot, int n, float* logits_out_d, int32
     if (logits_out_d) {
       last = logits_out_d + (size_t)(n - 1) * c.vocab;
     } else {
-      GemmProblem p = lgemm(reinterpret_cast<char*>(m->xn) + (size_t)(n - 1) * d * 2, d, m->lm_head, d, 1, c.vocab, d);
+      GemmProblem p = lgemm(m, reinterpret_cast<char*>(m->xn) + (size_t)(n - 1) * d * 2, d, m->lm_head_t, 1, c.vocab, d);
       p.out_f = m->last_logits; p.ldo_f = c.vocab;
       S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
       last = m->last_logits;
@@ -443,7 +469,7 @@ int llama_prefill_batch(s2s_llama* m, const int32_t* slots_h, int B, const int32
   else gather_last_rows_kernel<__half><<<B, 256, 0, st>>>((const __half*)m->xn, m->slot_d, d, (__half*)m->attn);
   S2S_LAUNCH_CHECK();
   {
-    GemmProblem p = lgemm(m->attn, d, m->lm_head, d, B, c.vocab, d);
+    GemmProblem p = lgemm(m, m->attn, d, m->lm_head_t, B, c.vocab, d);
     p.out_f = m->batch_logits; p.ldo_f = c.vocab;
     S2S_CHECK(gemm_tc_launch(m->ctx, p, dt, st));
   }
@@ -488,6 +514,7 @@ int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, co
                           int32_t dtype) {
   S2S_REQUIRE(m && name && data_h && shape, "llama bind_tensor: null argument");
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
+  S2S_CHECK(alloc_matrices(m));
   S2S_CHECK(m->arena.bind("llama", name, data_h, shape, ndim, dtype, m->cfg.compute_dtype));
   if (strncmp(name, "lm_head.", 8) == 0) m->lm_head_bound = true;
   return S2S_OK;
@@ -496,6 +523,7 @@ int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, co
 int s2s_llama_init_random(s2s_llama* m, uint64_t seed) {
   S2S_REQUIRE(m, "llama init_random: null model");
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
+  S2S_CHECK(alloc_matrices(m));
   S2S_CHECK(m->arena.init_random(seed, m->cfg.compute_dtype));
   m->lm_head_bound = true;
   return S2S_OK;
@@ -503,7 +531,7 @@ int s2s_llama_init_random(s2s_llama* m, uint64_t seed) {
 
 int s2s_llama_set_weight_format(s2s_llama* m, int32_t format) {
   S2S_REQUIRE(m, "llama set_weight_format: null model");
-  S2S_REQUIRE(!m->finalized, "llama set_weight_format: the weight format is fixed once the model is finalized");
+  S2S_REQUIRE(!m->matrices, "llama set_weight_format: the weight format is fixed by the first bind, init_random or finalize");
   if (format != m->cfg.compute_dtype) {
     if (format != S2S_FP8_E4M3 || m->cfg.compute_dtype != S2S_BF16 || m->n_tables != 1) {
       // the dequantised weights are exact in bf16, not in f16; multi-table models (TTS code predictor) stay 16-bit
@@ -519,53 +547,25 @@ int32_t s2s_llama_weight_format(s2s_llama* m) { return m ? m->weight_format : S2
 
 int s2s_llama_finalize(s2s_llama* m) {
   S2S_REQUIRE(m, "llama finalize: null model");
+  S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
+  S2S_CHECK(alloc_matrices(m));
   if (m->n_tables == 1 && !m->lm_head_bound && m->arena.find("model.embed_tokens.weight")->bound) {
-    // tied embeddings (tie_word_embeddings=True): lm_head shares embed_tokens
-    S2S_CHECK_CUDA(cudaMemcpy(m->lm_head, m->embed, (size_t)m->cfg.vocab * m->cfg.d_model * 2, cudaMemcpyDeviceToDevice));
+    // tied embeddings (tie_word_embeddings=True): lm_head is tiled (or quantised) straight from embed_tokens
+    S2S_CHECK(tile_rows_launch(m->embed, m->cfg.vocab, m->cfg.d_model, m->lm_head_t, m->cfg.vocab, 0, 1,
+                               m->weight_format == S2S_FP8_E4M3, 0));
     m->arena.find("lm_head.weight")->bound = true;
   }
   S2S_CHECK(m->arena.check_all_bound("llama"));
-  // decode-side weight layout: fragment-major tiles (weight_tiles.cu), built once per (re)load.  FP8: the tiles hold E4M3
-  // codes + row scales and the row-major matrices become the dequantised values, so prefill and decode share one model.
-  {
-    const bool f8 = m->weight_format == S2S_FP8_E4M3;
-    auto tbytes = [f8](int N, int K) { return f8 ? tiled_fp8_weight_bytes(N, K) : tiled_weight_elems(N, K) * 2; };
-    auto tile = [f8](const void* W, int N, int K, const void* Wt) {
-      return f8 ? quantize_tile_weights_fp8_launch(const_cast<void*>(W), N, K, const_cast<void*>(Wt), 0)
-                : tile_weights_launch(W, N, K, const_cast<void*>(Wt), 0);
-    };
-    const auto& c = m->cfg;
-    const int d = c.d_model, qd = c.heads * c.head_dim, kvd = c.kv_heads * c.head_dim, f = c.ffn;
-    S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-    if (m->tiled_h.empty()) {
-      m->tiled_h = m->layers_h;
-      for (int i = 0; i < c.layers; ++i) {
-        LlamaDecLayer& T = m->tiled_h[i];
-        void *a, *b, *g, *dn;
-        S2S_CHECK(m->arena.alloc(&a, tbytes(qd + 2 * kvd, d)));
-        S2S_CHECK(m->arena.alloc(&b, tbytes(d, qd)));
-        S2S_CHECK(m->arena.alloc(&g, tbytes(2 * f, d)));
-        S2S_CHECK(m->arena.alloc(&dn, tbytes(d, f)));
-        T.w_qkv = a; T.w_o = b; T.w_gu = g; T.w_down = dn;
-      }
-      m->head_t_table_elems = tiled_weight_elems(c.vocab, d);
-      S2S_CHECK(m->arena.alloc(&m->lm_head_t, f8 ? tbytes(c.vocab, d) : m->n_tables * m->head_t_table_elems * 2));
-      S2S_CHECK_CUDA(cudaMemcpy(m->layers_d, m->tiled_h.data(), sizeof(LlamaDecLayer) * c.layers, cudaMemcpyHostToDevice));
-    }
-    for (int i = 0; i < c.layers; ++i) {
-      const LlamaDecLayer& R = m->layers_h[i];
-      const LlamaDecLayer& T = m->tiled_h[i];
-      S2S_CHECK(tile(R.w_qkv, qd + 2 * kvd, d, T.w_qkv));
-      S2S_CHECK(tile(R.w_o, d, qd, T.w_o));
-      S2S_CHECK(tile(R.w_gu, 2 * f, d, T.w_gu));
-      S2S_CHECK(tile(R.w_down, d, f, T.w_down));
-    }
-    for (int t = 0; t < m->n_tables; ++t)   // FP8: n_tables == 1
-      S2S_CHECK(tile(reinterpret_cast<char*>(m->lm_head) + (size_t)t * m->head_table_elems * 2, c.vocab, d,
-                     reinterpret_cast<char*>(m->lm_head_t) + (size_t)t * m->head_t_table_elems * 2));
-    S2S_CHECK_CUDA(cudaDeviceSynchronize());
-  }
+  S2S_CHECK_CUDA(cudaDeviceSynchronize());
+  m->arena.release_staging();
   m->finalized = true;
+  return S2S_OK;
+}
+
+int s2s_llama_device_bytes(s2s_llama* m, int64_t* weights, int64_t* total) {
+  S2S_REQUIRE(m && weights && total, "llama device_bytes: null argument");
+  *weights = (int64_t)m->arena.weight_bytes();
+  *total = (int64_t)m->arena.bytes();
   return S2S_OK;
 }
 

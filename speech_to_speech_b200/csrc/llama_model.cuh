@@ -11,17 +11,19 @@ struct s2s_llama {
   s2s_ctx* ctx = nullptr;
   s2s_llama_config cfg{};
   bool finalized = false;
-  int weight_format = 0;                 // storage of the matrices the decode launch streams: cfg.compute_dtype, or S2S_FP8_E4M3
+  bool matrices = false;                 // the tiled matrices are allocated: the weight format is fixed
+  int weight_format = 0;                 // storage of the projections and lm_head: cfg.compute_dtype, or S2S_FP8_E4M3
   int debug_phases = 0;
   WeightArena arena;
   bool lm_head_bound = false;
   // weights
-  void *embed = nullptr, *lm_head = nullptr;
+  void* embed = nullptr;                 // row-major (a lookup)
   float* norm_f = nullptr;
-  std::vector<LlamaDecLayer> layers_h;   // row-major weights (prefill GEMMs)
-  std::vector<LlamaDecLayer> tiled_h;    // fragment-major copies streamed by the decode kernel (16-bit, or FP8 codes + row scales)
-  LlamaDecLayer* layers_d = nullptr;     // device copy of tiled_h
-  void* lm_head_t = nullptr;
+  // the projections in the one tiled layout (weight_tiles.cu) that prefill and decode both read: 16-bit, or FP8 codes +
+  // row scales
+  std::vector<LlamaDecLayer> layers_h;
+  LlamaDecLayer* layers_d = nullptr;     // device copy of layers_h
+  void* lm_head_t = nullptr;             // tiled like the projections; n_tables heads of head_t_table_elems
   float2* rope = nullptr;
   // KV + sessions
   void* kv = nullptr;
@@ -43,7 +45,7 @@ struct s2s_llama {
   unsigned long long* trace = nullptr;
   int trace_cap = 0;
   int n_tables = 1;                      // > 1: one embedding table and one output head per codebook (code predictor)
-  size_t embed_table_elems = 0, head_table_elems = 0, head_t_table_elems = 0;
+  size_t embed_table_elems = 0, head_t_table_elems = 0;
   float* qn = nullptr;                   // qk_norm: normalised q rows of the decode step [B][H*hd]
   float* kraw = nullptr;                 // qk_norm: raw k rows of the decode step [B][KV*hd]
   // token choice per slot (s2s_llama_set_sampling); active == 0: argmax

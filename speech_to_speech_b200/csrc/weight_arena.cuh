@@ -1,6 +1,8 @@
 // weight_arena.cuh -- the host-side weight machinery every model object owns (internal to libs2s_b200): tracked device
 // allocations, the table of state-dict names -> kernel layouts, bind_tensor (convert, lay out, upload), init_random and the
-// finalize-time "every tensor was bound" check.  The layout step (weight_layout / weight_upload) is pure host code, so a
+// finalize-time "every tensor was bound" check.  A slot may live in a tiled matrix (weight_tiles.cu): its rows are laid out
+// on the host as usual, staged on the device and tiled -- or quantised to FP8 -- straight into place, so no row-major copy
+// of the matrix exists.  The layout step (weight_layout / weight_upload) is pure host code, so a
 // CPU program can check it against a numpy statement of each layout (tests/test_weight_layouts.py).
 #pragma once
 #include <string.h>
@@ -33,8 +35,15 @@ struct WeightSlot {
   uint64_t seed = 0;          // != 0: init_random draws from its seed ^ this instead of its seed ^ FNV-1a(name)
   bool bound = false;
   bool raw = false;           // written by bind / init_random since the last finalize (the model clears it)
+  // tN > 0: dst is a tiled [tN, tK] 16-bit (or FP8, WeightArena::tiled_format) matrix and the slot's n / tK laid-out rows are
+  // its rows row0 + r * rstride.  W_INTERLEAVE slots are tiled with row0 = p, rstride = 2.
+  int tN = 0, tK = 0, row0 = 0, rstride = 1;
   WeightSlot& as(int l, int a0, int a1, int a2 = 0, int pp = 0, int ldd = 0) {
     layout = l; d0 = a0; d1 = a1; d2 = a2; p = pp; ld = ldd;
+    return *this;
+  }
+  WeightSlot& tiled(int N, int K, int first_row = 0, int row_stride = 1) {
+    tN = N; tK = K; row0 = first_row; rstride = row_stride;
     return *this;
   }
 };
@@ -127,16 +136,37 @@ struct WeightArena {
   WeightArena() = default;
   WeightArena(const WeightArena&) = delete;
   WeightArena& operator=(const WeightArena&) = delete;
-  ~WeightArena() { for (void* p : allocs_) cudaFree(p); }
+  ~WeightArena() {
+    for (void* p : allocs_) cudaFree(p);
+    release_staging();
+  }
+
+  // storage of the tiled slots: the 16-bit compute dtype (tiles) or S2S_FP8_E4M3 (codes + row scales, bf16 sources)
+  int tiled_format = 0;
 
   // cudaMalloc (zeroed unless zero = false), freed with the arena
   template <typename P> int alloc(P** out, size_t bytes, bool zero = true) {
     void* p = nullptr;
     S2S_CHECK_CUDA(cudaMalloc(&p, bytes ? bytes : 16));
     allocs_.push_back(p);
+    bytes_ += bytes ? bytes : 16;
     if (zero) S2S_CHECK_CUDA(cudaMemset(p, 0, bytes ? bytes : 16));
     *out = reinterpret_cast<P*>(p);
     return S2S_OK;
+  }
+  // alloc() of weight storage: counted in weight_bytes() too
+  template <typename P> int alloc_weights(P** out, size_t bytes) {
+    S2S_CHECK(alloc(out, bytes));
+    weight_bytes_ += bytes ? bytes : 16;
+    return S2S_OK;
+  }
+  size_t bytes() const { return bytes_; }                // device bytes the arena holds (the staging buffer excluded)
+  size_t weight_bytes() const { return weight_bytes_; }
+  // the device buffer bind / init_random stage a tiled slot's rows in (as large as the largest such slot); models free it
+  // at finalize
+  void release_staging() {
+    if (staging_) cudaFree(staging_);
+    staging_ = nullptr;
   }
   WeightSlot& add(const std::string& name, void* dst, bool half, int64_t n, float rnd_scale = 0.02f, float rnd_offset = 0.f) {
     WeightSlot& s = slots[name];
@@ -156,4 +186,8 @@ struct WeightArena {
 
  private:
   std::vector<void*> allocs_;
+  size_t bytes_ = 0, weight_bytes_ = 0;
+  void* staging_ = nullptr;
+  int ensure_staging();
+  int stage_tiled(const WeightSlot& s, const void* bytes, int64_t rows, int row0, int rstride);
 };

@@ -18,6 +18,17 @@ __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   return d;
 }
 
+// K-major, 64-byte-swizzled descriptor: rows of 64 B (32 x 16-bit) in 512-byte atoms of 8 rows, 8-row groups
+// `sbo` bytes apart.  Atoms must be 512-byte aligned; within one, K advances by 16 elements per 32 B (+2 encoded).
+__device__ __forceinline__ uint64_t wgmma_desc_sw64(uint32_t smem_addr, uint32_t sbo) {
+  uint64_t d = 0;
+  d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);  // start address, bits [0,14)
+  d |= (uint64_t)1 << 16;                        // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)(sbo >> 4) << 32;               // stride byte offset
+  d |= (uint64_t)2 << 62;                        // layout: SWIZZLE_64B
+  return d;
+}
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void wgmma_wait() {

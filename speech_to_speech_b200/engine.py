@@ -257,6 +257,42 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, 
     return c
 
 
+def tile_weights(w: torch.Tensor, weight_dtype: Optional[str] = None) -> torch.Tensor:
+    """w [N, K] fp16/bf16 cuda (N a multiple of 8, K of 32) -> the tiled layout the Llama-family engines store their
+    projections in (include/s2s_b200.h s2s_tile_weights), as a flat uint8 cuda tensor: 16-bit tiles, or with
+    weight_dtype="float8_e4m3" (bf16 w) E4M3 codes followed by the fp32 row scales."""
+    assert w.is_cuda and w.dim() == 2 and w.is_contiguous() and w.dtype in (torch.float16, torch.bfloat16)
+    N, K = w.shape
+    fmt = _lib.WEIGHT_FORMAT_CODES[weight_dtype] if weight_dtype else {torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[w.dtype]
+    lib = _lib.load()
+    nbytes = int(lib.s2s_tiled_weight_bytes(N, K, fmt))
+    if nbytes <= 0:
+        raise ValueError(f"no tiled layout for a [{N}, {K}] matrix")
+    out = torch.empty((nbytes,), dtype=torch.uint8, device=w.device)
+    dev = w.device.index or 0
+    check(lib.s2s_tile_weights(get_context(dev), _ptr(w), N, K, fmt, _ptr(out), _stream_ptr(dev)), "s2s_tile_weights")
+    return out
+
+
+def gemm_tiled(a: torch.Tensor, wt: torch.Tensor, N: int, weight_dtype: Optional[str] = None, bias: Optional[torch.Tensor] = None,
+               act: str = "none", out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
+    """gemm() with the weight operand in the tiled layout of tile_weights(): a [M, K] fp16/bf16 cuda, wt from
+    tile_weights(w [N, K], weight_dtype).  FP8 computes exactly gemm(a, dq(q(w)))."""
+    assert a.is_cuda and wt.is_cuda and a.is_contiguous() and wt.is_contiguous()
+    dev = a.device.index or 0
+    M, K = a.shape
+    code = {torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[a.dtype]
+    fmt = _lib.WEIGHT_FORMAT_CODES[weight_dtype] if weight_dtype else code
+    lib = _lib.load()
+    assert wt.numel() * wt.element_size() >= int(lib.s2s_tiled_weight_bytes(N, K, fmt)), "wt is smaller than the tiled [N, K] matrix"
+    out_dtype = out_dtype or a.dtype
+    ocode = S2S_F32 if out_dtype == torch.float32 else code
+    c = torch.empty((M, N), dtype=out_dtype, device=a.device)
+    check(lib.s2s_gemm_tiled(get_context(dev), _ptr(a), _ptr(wt), fmt, _ptr(bias), _ptr(c), M, N, K, code, ocode,
+                             1 if act == "gelu" else 0, _stream_ptr(dev)), "s2s_gemm_tiled")
+    return c
+
+
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, kv_heads: int, scale: float,
               causal: bool = False) -> torch.Tensor:
     """q [B,Tq,heads*hd], k/v [B,Tk,kv_heads*hd] (last dim contiguous; row strides taken from the tensors)."""
@@ -421,6 +457,13 @@ class LlamaEngine:
     def max_decode_batch(self) -> int:
         """Sessions one decode launch can carry for this geometry (shared-memory budget of the kernel)."""
         return int(self.lib.s2s_llama_max_decode_batch(self.handle))
+
+    def device_bytes(self) -> tuple[int, int]:
+        """(weights, total): device bytes the engine holds for its weights (embedding, norms, the one tiled copy of the
+        projections and lm_head) and in all (KV cache and workspaces included)."""
+        w, t = C.c_int64(0), C.c_int64(0)
+        check(self.lib.s2s_llama_device_bytes(self.handle, C.byref(w), C.byref(t)), "s2s_llama_device_bytes")
+        return int(w.value), int(t.value)
 
     def set_trace(self, trace: Optional[torch.Tensor]) -> None:
         """trace: cuda int64 [2, capacity, 6] or None (profiling aid, see include/s2s_b200.h)."""

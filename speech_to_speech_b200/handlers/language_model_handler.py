@@ -36,6 +36,11 @@ LLAMA_GEOMETRIES = {
     "mini": dict(d_model=1024, layers=4, heads=8, kv_heads=2, head_dim=128, ffn=3584, vocab=32064),
     "llama-3-8b": dict(d_model=4096, layers=32, heads=32, kv_heads=8, head_dim=128, ffn=14336, vocab=128256,
                        rope_theta=500000.0, rms_eps=1e-5),
+    # Qwen/Qwen3-14B and Qwen/Qwen3-32B (config.json): one weight copy makes them fit one H100, 32B in FP8 only
+    "qwen3-14b": dict(d_model=5120, layers=40, heads=40, kv_heads=8, head_dim=128, ffn=17408, vocab=151936, rope_theta=1000000.0,
+                      rms_eps=1e-6, qk_norm=True),
+    "qwen3-32b": dict(d_model=5120, layers=64, heads=64, kv_heads=8, head_dim=128, ffn=25600, vocab=151936, rope_theta=1000000.0,
+                      rms_eps=1e-6, qk_norm=True),
 }
 
 
