@@ -167,6 +167,63 @@ typedef struct {
   void* out;             /* [B][heads][hd] 16-bit */
 } s2s_dec_attn_args;
 int s2s_decode_attention(s2s_ctx* ctx, const s2s_dec_attn_args* args, int32_t* plan_out_h, void* stream);
+/* The skinny GEMM of the persistent decode kernels by itself (exposed for tests): the production device functions
+ * (gemv_mma / gemv_mma_chunked, their staging routines and epilogues) in one plain launch of `grid` CTAs, running n_proj
+ * <= 3 projections back to back with one weight ring per warp, so ring slot and parity carry over between them as between
+ * the phases of a decode launch.  Projection i computes, for sessions b < B,
+ *   v[b][n] = sum_k W[n][k] x[b][k] (+ bias[n]),   W from s2s_tile_weights (16-bit, or FP8 codes + row scales),
+ * with x staged from `input`: COPY 16-bit rows x16 [B][K]; NORM fp32 rows xf [B][K] normalised (norm 1 LayerNorm with
+ * norm_w / norm_b, 2 RMSNorm with norm_w; eps; rg rows of the fp32 copy resident at a time, 0 = B, -1 = read from L2,
+ * K <= 4096); NORM_SUM xf + add_bias + sum of n_parts partials parts [n_parts][B][K], summed in that order, written to
+ * x_out by CTA 0 (may be NULL) and normalised as NORM; CHUNKED 16-bit rows x16 [B][K] staged kc columns at a time.  The
+ * epilogue `mode` is the decode kernels' (0 STORE out[b*ldo + n]; 1 GELU 16-bit out_h[b*ldh + n]; 2 RESID out += v;
+ * 3 QKV: q rows -> out, k / v rows -> the 16-bit cache kv0 + which*kv_which + b*kv_batch + c; 4 LOGITS: suppress bits
+ * 1 always / 2 at first_step set a row to -inf, optional logits_out[b*logits_ld + n], argmax (lowest id on ties) ->
+ * argmax_out[b]; 5 QKV_ROPE: rows [0, q_rows) rotated with rope[pos[b]] (fp32 (cos, sin) pairs, hd/2 per position) and
+ * scaled by q_scale -> out, [q_rows, q_rows + k_rows) rotated -> K cache, the rest -> V cache, cache element (b, c) at
+ * kv0 + which*kv_which + slot[b]*kv_slot + pos[b]*kv_ld + c; kraw != NULL stores q and k raw (q -> out, k -> kraw[b][k_rows]);
+ * 6 SWIGLU: row pairs (gate, up) -> out_h[b*ldh + n/2]).  Modes 1 and 3 exist with llama = 0 only, 5 and 6 with llama = 1.
+ * Pointers are device pointers.  The projections of one call must not read what an earlier one writes (no grid barrier).
+ * grid 0 = the context's decode grid; slots 1..4 ring slots per warp (0 = as many as fit); prefetch: issue a projection's
+ * first weight units before its input is staged, as the decode kernels' look-ahead does (not for CHUNKED); use_plans:
+ * plans computed once at kernel start, else on the fly; drain: before the last projection, issue projection 0's first
+ * units and wait for them unused (an early exit's gemv_drain).  staged (may be NULL): CTA 0's staged 16-bit operand
+ * [B][K].  plans_out_h (may be NULL): int32 [n_proj][5] = n_tiles, main_rounds, ks_log, slice, tail_rounds of CTA 0 (for
+ * CHUNKED, the plan of [N, kc] as the host recomputes it from the same inputs).
+ * Virtual clusters (cluster > 0; the per-head plans of the Whisper single-session kernel without cluster hardware): CTA i is
+ * rank i % cluster of cluster cid = i / cluster, which owns head cid when cid < heads; grid % cluster == 0 and
+ * grid / cluster >= heads.  A projection with head_plan 1 (the q, k, v rows of head cid of a [3d, d] QKV projection, K = d),
+ * 2 (the q rows of head cid of a [d, d] projection) or 3 (all d rows of a [d, d] matrix times the head's 64 columns, K = 64,
+ * N = d) runs the cluster-local plan gemv_head_plan builds; x16 and out of cluster cid are offset by cid * x_cluster_stride
+ * and cid * out_cluster_stride elements (min(cid, heads - 1) for clusters without a head).
+ * S2S_ERR_INVALID on K % 32 != 0, B outside [1, 16], FP8 with anything but bf16 / llama = 1, a mode the instantiation
+ * lacks, a kc gemv_chunk_ok rejects, odd N outside LOGITS, a bias with odd N.  Per-call scratch; synchronous. */
+#define S2S_GEMV_IN_COPY 0
+#define S2S_GEMV_IN_NORM 1
+#define S2S_GEMV_IN_NORM_SUM 2
+#define S2S_GEMV_IN_CHUNKED 3
+typedef struct {
+  const void* w; int32_t N, K; const float* bias;
+  int32_t input;
+  const void* x16; int32_t kc;
+  const float* xf; int32_t norm; const float* norm_w; const float* norm_b; float eps; int32_t rg;
+  const float* parts; int32_t n_parts; const float* add_bias; float* x_out;
+  void* staged;
+  int32_t mode;
+  float* out; int32_t ldo; void* out_h; int32_t ldh;
+  void* kv0; int64_t kv_which, kv_batch; int32_t d;
+  const int32_t* pos; const int32_t* slot; int64_t kv_slot; int32_t kv_ld; const float* rope; int32_t hd, q_rows, k_rows;
+  float q_scale; float* kraw;
+  const uint8_t* suppress; int32_t first_step; float* logits_out; int64_t logits_ld; int32_t* argmax_out;
+  int32_t head_plan; int64_t x_cluster_stride, out_cluster_stride;   /* virtual clusters only */
+} s2s_dec_gemv_proj;
+typedef struct {
+  s2s_dec_gemv_proj proj[3]; int32_t n_proj;
+  int32_t B, dtype, weight_format, llama;   /* weight_format = dtype, or S2S_FP8_E4M3 (bf16, llama = 1) */
+  int32_t grid, slots, prefetch, use_plans, drain;
+  int32_t cluster, heads;                   /* virtual clusters: 0 = whole-grid plans only */
+} s2s_dec_gemv_args;
+int s2s_decode_gemv(s2s_ctx* ctx, const s2s_dec_gemv_args* args, int32_t* plans_out_h, void* stream);
 
 /* ---- Llama-family LLM ------------------------------------------------------------------ */
 typedef struct {

@@ -19,7 +19,7 @@ EXPORTED = [
     "s2s_whisper_create", "s2s_whisper_destroy", "s2s_whisper_bind_tensor", "s2s_whisper_init_random",
     "s2s_whisper_finalize", "s2s_whisper_logmel", "s2s_whisper_encode", "s2s_whisper_decode",
     "s2s_whisper_detect_language", "s2s_whisper_transcribe", "s2s_whisper_set_trace", "s2s_whisper_max_decode_batch",
-    "s2s_gemm", "s2s_tiled_weight_bytes", "s2s_tile_weights", "s2s_gemm_tiled", "s2s_attention", "s2s_decode_attention",
+    "s2s_gemm", "s2s_tiled_weight_bytes", "s2s_tile_weights", "s2s_gemm_tiled", "s2s_attention", "s2s_decode_attention", "s2s_decode_gemv",
     "s2s_llama_create", "s2s_llama_destroy", "s2s_llama_bind_tensor", "s2s_llama_init_random",
     "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_set_sampling", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
     "s2s_llama_set_weight_format", "s2s_llama_weight_format", "s2s_llama_device_bytes",
@@ -100,6 +100,34 @@ class DecAttnArgs(C.Structure):
     ]
 
 
+class DecGemvProj(C.Structure):
+    """s2s_dec_gemv_proj: one projection of an s2s_decode_gemv call."""
+    _fields_ = [
+        ("w", C.c_void_p), ("N", C.c_int32), ("K", C.c_int32), ("bias", C.c_void_p),
+        ("input", C.c_int32),
+        ("x16", C.c_void_p), ("kc", C.c_int32),
+        ("xf", C.c_void_p), ("norm", C.c_int32), ("norm_w", C.c_void_p), ("norm_b", C.c_void_p), ("eps", C.c_float),
+        ("rg", C.c_int32),
+        ("parts", C.c_void_p), ("n_parts", C.c_int32), ("add_bias", C.c_void_p), ("x_out", C.c_void_p),
+        ("staged", C.c_void_p),
+        ("mode", C.c_int32),
+        ("out", C.c_void_p), ("ldo", C.c_int32), ("out_h", C.c_void_p), ("ldh", C.c_int32),
+        ("kv0", C.c_void_p), ("kv_which", C.c_int64), ("kv_batch", C.c_int64), ("d", C.c_int32),
+        ("pos", C.c_void_p), ("slot", C.c_void_p), ("kv_slot", C.c_int64), ("kv_ld", C.c_int32), ("rope", C.c_void_p),
+        ("hd", C.c_int32), ("q_rows", C.c_int32), ("k_rows", C.c_int32),
+        ("q_scale", C.c_float), ("kraw", C.c_void_p),
+        ("suppress", C.c_void_p), ("first_step", C.c_int32), ("logits_out", C.c_void_p), ("logits_ld", C.c_int64),
+        ("argmax_out", C.c_void_p),
+        ("head_plan", C.c_int32), ("x_cluster_stride", C.c_int64), ("out_cluster_stride", C.c_int64),
+    ]
+
+
+class DecGemvArgs(C.Structure):
+    """s2s_dec_gemv_args: 1..3 decode projections in one launch (s2s_decode_gemv)."""
+    _fields_ = [("proj", DecGemvProj * 3), ("n_proj", C.c_int32)] + [(n, C.c_int32) for n in (
+        "B", "dtype", "weight_format", "llama", "grid", "slots", "prefetch", "use_plans", "drain", "cluster", "heads")]
+
+
 class Qwen3TTSConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in (
         "d_model", "layers", "heads", "kv_heads", "head_dim", "ffn", "vocab",
@@ -156,6 +184,7 @@ def load() -> C.CDLL:
     lib.s2s_gemm_tiled.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     lib.s2s_attention.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i64, i64, i64, i64, f32, i32, i32, vp]
     lib.s2s_decode_attention.argtypes = [vp, C.POINTER(DecAttnArgs), C.POINTER(i32), vp]
+    lib.s2s_decode_gemv.argtypes = [vp, C.POINTER(DecGemvArgs), C.POINTER(i32), vp]
     lib.s2s_llama_create.argtypes = [vp, C.POINTER(LlamaConfig), C.POINTER(vp)]
     lib.s2s_llama_destroy.argtypes = [vp]
     lib.s2s_llama_bind_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]

@@ -659,6 +659,28 @@ __host__ __device__ __forceinline__ void gemv_make_plan_ex(int n_tiles, int K, i
   pl.tail_rounds = (tail > vbid) ? (tail - vbid + stride - 1) / stride : 0;
   pl.vgrid = vgrid; pl.vbid = vbid; pl.map_base = 0; pl.map_gshift = 30; pl.map_gstride = 0; pl.k_off = 0; pl.k_full = K;
 }
+// Cluster-local plans of one attention head (the Whisper single-session kernel, whisper_decode.cu): CTA `rank` of the cs CTAs
+// of cluster cid, which owns head cid when has_head (else the plan has no tiles), head_dim HD, model width d.
+//   GEMV_PLAN_QKV_HEAD  the q, k and v rows of the head of a [3d, d] projection: local tile lt -> global tile
+//                       (HD / 8) cid + (lt / (HD / 8)) * (d / 8) + lt % (HD / 8)
+//   GEMV_PLAN_Q_HEAD    the q rows of the head of a [d, d] projection
+//   GEMV_PLAN_OUT_SLICE all d rows of a [d, d] projection times the head's HD columns [HD cid, HD cid + HD) (K = HD)
+enum GemvHeadPlan { GEMV_PLAN_QKV_HEAD = 1, GEMV_PLAN_Q_HEAD = 2, GEMV_PLAN_OUT_SLICE = 3 };
+template <int HD>
+__host__ __device__ __forceinline__ void gemv_head_plan(int kind, int d, int cid, int rank, int cs, bool has_head, GemvPlan& pl) {
+  constexpr int HT = HD / 8, HT_LOG = HT == 8 ? 3 : HT == 16 ? 4 : -1;   // weight tiles per head
+  static_assert(HT_LOG > 0, "head_dim 64 or 128");
+  if (kind == GEMV_PLAN_QKV_HEAD) {
+    gemv_make_plan_ex(has_head ? 3 * HT : 0, d, cs, rank, pl);
+    pl.map_base = HT * cid; pl.map_gshift = HT_LOG; pl.map_gstride = d / 8;
+  } else if (kind == GEMV_PLAN_Q_HEAD) {
+    gemv_make_plan_ex(has_head ? HT : 0, d, cs, rank, pl);
+    pl.map_base = HT * cid; pl.map_gshift = HT_LOG; pl.map_gstride = 0;
+  } else {
+    gemv_make_plan_ex(has_head ? d / 8 : 0, HD, cs, rank, pl);
+    pl.k_off = HD * cid; pl.k_full = d;
+  }
+}
 // whole-grid projection [N, K]
 __device__ __forceinline__ void gemv_make_plan(int N, int K, GemvPlan& pl) {
   gemv_make_plan_ex((N + GV_ROWS - 1) >> 3, K, (int)gridDim.x, (int)blockIdx.x, pl);

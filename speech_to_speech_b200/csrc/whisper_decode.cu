@@ -496,15 +496,12 @@ whisper_decode_cluster_kernel(const WhisperDecParams p, int step_begin, int step
     const int i = threadIdx.x;
     const bool has_head = cx.cid < p.heads;
     GemvPlan& pl = s_plans[i];
-    if (i == 0) {         // q, k, v rows of head cid: local tile lt -> (lt >> 3) * (d / 8) + 8 cid + (lt & 7)
-      gemv_make_plan_ex(has_head ? 3 * (HD / 8) : 0, p.d, cx.cs, cx.rank, pl);
-      pl.map_base = (HD / 8) * cx.cid; pl.map_gshift = 3; pl.map_gstride = p.d / 8;
+    if (i == 0) {         // q, k, v rows of head cid
+      gemv_head_plan<HD>(GEMV_PLAN_QKV_HEAD, p.d, cx.cid, cx.rank, cx.cs, has_head, pl);
     } else if (i == 1) {  // cross-attention q rows of head cid
-      gemv_make_plan_ex(has_head ? HD / 8 : 0, p.d, cx.cs, cx.rank, pl);
-      pl.map_base = (HD / 8) * cx.cid; pl.map_gshift = 3; pl.map_gstride = 0;
+      gemv_head_plan<HD>(GEMV_PLAN_Q_HEAD, p.d, cx.cid, cx.rank, cx.cs, has_head, pl);
     } else if (i == 2) {  // all d rows x the head's 64 columns
-      gemv_make_plan_ex(has_head ? p.d / 8 : 0, HD, cx.cs, cx.rank, pl);
-      pl.k_off = HD * cx.cid; pl.k_full = p.d;
+      gemv_head_plan<HD>(GEMV_PLAN_OUT_SLICE, p.d, cx.cid, cx.rank, cx.cs, has_head, pl);
     } else {
       gemv_make_plan(i == 3 ? p.ffn : i == 5 ? p.vocab : p.d, i == 4 ? p.ffn : p.d, pl);
     }

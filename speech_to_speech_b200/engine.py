@@ -335,6 +335,40 @@ def decode_attention(q: torch.Tensor, kv: torch.Tensor, slots: Sequence[int], le
     return out, int(plan.value)
 
 
+GEMV_MODES = {"store": 0, "gelu": 1, "resid": 2, "qkv": 3, "logits": 4, "qkv_rope": 5, "swiglu": 6}
+GEMV_INPUTS = {"copy": 0, "norm": 1, "norm_sum": 2, "chunked": 3}
+
+
+def decode_gemv(projs: Sequence[Mapping[str, Any]], B: int, dtype: torch.dtype, *, weight_dtype: Optional[str] = None,
+                llama: bool = True, grid: int = 0, slots: int = 0, prefetch: bool = False, use_plans: bool = False,
+                drain: bool = False, cluster: int = 0, heads: int = 0) -> list[tuple[int, ...]]:
+    """1..3 projections of the decode kernels' skinny GEMM in one launch (include/s2s_b200.h s2s_decode_gemv).  Each entry of
+    `projs` maps s2s_dec_gemv_proj field names to values: contiguous cuda tensors are passed as their device pointers,
+    `mode` and `input` may be names (GEMV_MODES, GEMV_INPUTS); w comes from tile_weights().  The epilogues write into the
+    caller's tensors.  -> per projection (n_tiles, main_rounds, ks_log, slice, tail_rounds) of CTA 0.  Synchronous."""
+    a = _lib.DecGemvArgs()
+    for i, pr in enumerate(projs):
+        dst = a.proj[i]
+        for k, v in pr.items():
+            if isinstance(v, torch.Tensor):
+                assert v.is_cuda and v.is_contiguous(), k
+                v = v.data_ptr()
+            elif k == "mode" and isinstance(v, str):
+                v = GEMV_MODES[v]
+            elif k == "input" and isinstance(v, str):
+                v = GEMV_INPUTS[v]
+            setattr(dst, k, v)
+    code = {torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[dtype]
+    a.n_proj, a.B, a.dtype, a.llama = len(projs), B, code, int(llama)
+    a.weight_format = _lib.WEIGHT_FORMAT_CODES[weight_dtype] if weight_dtype else code
+    a.grid, a.slots, a.prefetch, a.use_plans, a.drain = grid, slots, int(prefetch), int(use_plans), int(drain)
+    a.cluster, a.heads = cluster, heads
+    plans = (C.c_int32 * (5 * 3))()
+    dev = torch.cuda.current_device()
+    check(_lib.load().s2s_decode_gemv(get_context(dev), C.byref(a), plans, _stream_ptr(dev)), "s2s_decode_gemv")
+    return [tuple(plans[5 * i: 5 * i + 5]) for i in range(len(projs))]
+
+
 def codec_contract(x: Optional[torch.Tensor], w: torch.Tensor, y: torch.Tensor, *, path: int = 0,
                    x16: Optional[torch.Tensor] = None, T_in: Optional[int] = None, T_out: Optional[int] = None, x_row0: int = 0,
                    dil: int = 1, bias: Optional[torch.Tensor] = None, bias_mod: Optional[int] = None, act: int = 0,
