@@ -131,6 +131,11 @@ template <bool F8> constexpr int gv_uk_log = F8 ? 9 : 8;                    // l
 template <bool F8> constexpr int gv_uk = 1 << gv_uk_log<F8>;
 template <bool F8> constexpr int gv_elem_bytes = F8 ? 1 : 2;
 static_assert(gv_uk<false> == GV_UK && GV_ROWS * gv_uk<true> * gv_elem_bytes<true> == GV_SLOT_BYTES, "a ring unit fills a slot");
+// element k of row r of a 16-bit tiled matrix with K columns, for row lookups (Whisper's token embedding).  Each 32-k window
+// of a row is 64 contiguous bytes, so a warp reading 32 consecutive k of a row loads one segment, as from a row-major table.
+__device__ __forceinline__ long long gv_tiled_elem(int r, int k, int K) {
+  return ((long long)(r >> 3) * (K >> 5) + (k >> 5)) * (GV_ROWS * 32) + (r & (GV_ROWS - 1)) * 32 + (k & 31);
+}
 // the row scales of an FP8 matrix [N, K] (whole rows: K = row length)
 __device__ __forceinline__ const float* gemv_f8_scales(const void* W, int N, int K) {
   return reinterpret_cast<const float*>(reinterpret_cast<const unsigned char*>(W) + (size_t)((N + GV_ROWS - 1) & ~(GV_ROWS - 1)) * K);

@@ -27,9 +27,9 @@ int convert_f32_launch(const float* src, void* dst, long long n, int dtype, cuda
 int fill_random_launch(void* dst, long long n, int dtype, float scale, float offset, uint64_t seed,
                        cudaStream_t stream);
 // ---- weight_tiles.cu ----
-// row-major 16-bit [N, K] -> fragment-major tiled layout streamed by the decode kernels (see decode_common.cuh)
+// 16-bit elements of a [N, K] matrix in the fragment-major tiled layout streamed by the decode kernels (see
+// decode_common.cuh): rows padded to a multiple of 8
 size_t tiled_weight_elems(int N, int K);
-int tile_weights_launch(const void* W, int N, int K, void* Wt, cudaStream_t stream);
 // FP8 E4M3 weight-only storage with a power-of-two scale per row: tiled E4M3 codes followed by roundup8(N) fp32 row scales
 size_t tiled_fp8_weight_bytes(int N, int K);
 // the `rows` rows of a row-major 16-bit [rows, K] source -> rows row0 + r * rstride of the tiled [N, K] matrix Wt: 16-bit

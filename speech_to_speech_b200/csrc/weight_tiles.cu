@@ -1,12 +1,12 @@
-// weight_tiles.cu -- re-lay a row-major 16-bit weight matrix [N, K] into the fragment-major "tiled" layout the
-// decode kernels stream (decode_common.cuh): tile = 8 rows, window = 32 k,
+// weight_tiles.cu -- lay row-major 16-bit weight rows [rows, K] into the fragment-major "tiled" layout of a [N, K] matrix
+// that the decode kernels stream (decode_common.cuh): tile = 8 rows, window = 32 k,
 //   element (row 8*tile + g, k 32*w + 8*t + e)  ->  ((tile * K/32 + w) * 32 + 4*g + t) * 8 + e
 // so that (a) any run of k windows of a tile is one contiguous block = one cp.async.bulk, and (b) the 16-byte
 // fragment loads of a warp read 512 consecutive bytes of shared memory, and (c) each 32-k window of a tile is an 8 x 64 B
-// row-major block, which the wgmma prefill GEMM loads with a 4-D TMA map (gemm_tc.cu).  Rows N..roundup8(N) are zero.
-// The Llama family keeps its projections and lm_head in this layout only: bind / init_random tile each tensor's rows
-// into place (tile_rows_launch), and prefill and decode read the same copy.  Whisper tiles its decoder matrices at
-// finalize (tile_weights_launch) and keeps the row-major copy for its encoder-side GEMMs.
+// row-major block, which the wgmma prefill GEMM loads with a 4-D TMA map (gemm_tc.cu).  Rows N..roundup8(N) stay zero.
+// The Llama family keeps its projections and lm_head in this layout only, and Whisper its decoder matrices and token
+// embedding: bind / init_random tile each tensor's rows into place (tile_rows_launch, weight_arena.cu), so no row-major
+// copy exists.  Llama's prefill and decode read the same copy.
 //
 // FP8 E4M3 weight-only storage (Llama-family decode, llama_decode.cu): per row n the integer exponent e_n is the smallest
 // with max_k |W[n,k]| * 2^-e_n <= 448 (not below FP8_MIN_EXP; 0 for an all-zero row), the code is
@@ -23,20 +23,6 @@
 #include "kernels.cuh"
 
 namespace {
-__global__ void tile_weights_kernel(const uint4* __restrict__ W, int N, int K, uint4* __restrict__ Wt, long long n_vec) {
-  const int wpr = K >> 5;  // windows per row
-  for (long long v = blockIdx.x * (long long)blockDim.x + threadIdx.x; v < n_vec; v += (long long)gridDim.x * blockDim.x) {
-    const int lane = (int)(v & 31);
-    const long long tw = v >> 5;
-    const int w = (int)(tw % wpr);
-    const long long tile = tw / wpr;
-    const long long row = tile * 8 + (lane >> 2);
-    uint4 val = make_uint4(0u, 0u, 0u, 0u);
-    if (row < N) val = W[(row * K + (long long)w * 32 + (lane & 3) * 8) >> 3];
-    Wt[v] = val;
-  }
-}
-
 // lowest row exponent: keeps the smallest dequantised value (2^-9 * 2^e_n) a normal bf16 number.  Rows whose largest
 // magnitude is below 448 * 2^-100 lose precision instead; trained weights are nowhere near.
 constexpr int FP8_MIN_EXP = -100;
@@ -117,12 +103,3 @@ int tile_rows_launch(const void* src, int rows, int K, void* Wt, int N, int row0
 }
 
 size_t tiled_weight_elems(int N, int K) { return (size_t)((N + 7) / 8) * 8 * (size_t)K; }
-
-int tile_weights_launch(const void* W, int N, int K, void* Wt, cudaStream_t stream) {
-  S2S_REQUIRE(K % 32 == 0, "tile_weights: K=%d must be a multiple of 32", K);
-  const long long n_vec = (long long)tiled_weight_elems(N, K) / 8;
-  const int blocks = (int)std::min<long long>((n_vec + 255) / 256, 132 * 16);
-  tile_weights_kernel<<<blocks, 256, 0, stream>>>(reinterpret_cast<const uint4*>(W), N, K, reinterpret_cast<uint4*>(Wt), n_vec);
-  S2S_LAUNCH_CHECK();
-  return S2S_OK;
-}

@@ -39,10 +39,7 @@ struct s2s_whisper {
   float *conv1_b = nullptr, *conv2_b = nullptr, *enc_pos = nullptr, *dec_pos = nullptr, *ckv_b = nullptr;
   float *enc_lnf_w = nullptr, *enc_lnf_b = nullptr, *dec_lnf_w = nullptr, *dec_lnf_b = nullptr;
   std::vector<EncLayer> enc;
-  std::vector<WhisperDecLayer> dec_h;    // row-major decoder weights as bound
-  std::vector<WhisperDecLayer> dec_t;    // fragment-major copies streamed by the decode kernel
-  WhisperDecLayer* dec_d = nullptr;      // device copy of dec_t
-  void* embed_t = nullptr;
+  WhisperDecLayer* dec_d = nullptr;      // [dec_layers] device table of the decoder layers
   // tables
   float *hann = nullptr, *twiddle = nullptr, *fb = nullptr;
   int2* fb_range = nullptr;
@@ -174,48 +171,51 @@ int alloc_weights(s2s_whisper* m) {
   }
   S2S_CHECK(add_ln("model.encoder.layer_norm", &m->enc_lnf_w, &m->enc_lnf_b));
 
-  // decoder
-  S2S_CHECK(m->arena.alloc(&m->embed, wbytes((int64_t)c.vocab * d)));
+  // decoder.  The matrices the decode kernel streams and the token embedding (looked up, and the tied output projection)
+  // are stored once, in the tiled layout (weight_tiles.cu): bind and init_random tile each tensor's rows into place.  The
+  // cross-attention K/V projections are read by the encoder-side GEMM and stay row-major.
+  auto alloc_tiled = [&](void** w, int N, int K) { return m->arena.alloc(w, tiled_weight_elems(N, K) * 2); };
+  S2S_CHECK(alloc_tiled(&m->embed, c.vocab, d));
   S2S_CHECK(m->arena.alloc(&m->dec_pos, (size_t)c.max_target_positions * d * 4));
-  A.add("model.decoder.embed_tokens.weight", m->embed, true, (int64_t)c.vocab * d);
+  A.add("model.decoder.embed_tokens.weight", m->embed, true, (int64_t)c.vocab * d).tiled(c.vocab, d);
   A.add("model.decoder.embed_positions.weight", m->dec_pos, false, (int64_t)c.max_target_positions * d);
   S2S_CHECK(m->arena.alloc(&m->ckv_w, wbytes((int64_t)c.dec_layers * 2 * d * d)));
   S2S_CHECK(m->arena.alloc(&m->ckv_b, (size_t)c.dec_layers * 2 * d * 4));
-  m->dec_h.resize(c.dec_layers);
+  std::vector<WhisperDecLayer> dec(c.dec_layers);
   for (int i = 0; i < c.dec_layers; ++i) {
-    WhisperDecLayer& L = m->dec_h[i];
+    WhisperDecLayer& L = dec[i];
     const std::string p = "model.decoder.layers." + std::to_string(i) + ".";
     void *w_qkv, *w_o, *w_cq, *w_co, *w_fc1, *w_fc2;
     float *b_qkv, *b_o, *b_cq, *b_co, *b_fc1, *b_fc2, *l1w, *l1b, *l2w, *l2b, *l3w, *l3b;
-    S2S_CHECK(m->arena.alloc(&w_qkv, wbytes((int64_t)3 * d * d)));
+    S2S_CHECK(alloc_tiled(&w_qkv, 3 * d, d));
     S2S_CHECK(m->arena.alloc(&b_qkv, 3 * d * 4));
-    S2S_CHECK(m->arena.alloc(&w_o, wbytes((int64_t)d * d)));
+    S2S_CHECK(alloc_tiled(&w_o, d, d));
     S2S_CHECK(m->arena.alloc(&b_o, d * 4));
-    S2S_CHECK(m->arena.alloc(&w_cq, wbytes((int64_t)d * d)));
+    S2S_CHECK(alloc_tiled(&w_cq, d, d));
     S2S_CHECK(m->arena.alloc(&b_cq, d * 4));
-    S2S_CHECK(m->arena.alloc(&w_co, wbytes((int64_t)d * d)));
+    S2S_CHECK(alloc_tiled(&w_co, d, d));
     S2S_CHECK(m->arena.alloc(&b_co, d * 4));
-    S2S_CHECK(m->arena.alloc(&w_fc1, wbytes((int64_t)f * d)));
+    S2S_CHECK(alloc_tiled(&w_fc1, f, d));
     S2S_CHECK(m->arena.alloc(&b_fc1, f * 4));
-    S2S_CHECK(m->arena.alloc(&w_fc2, wbytes((int64_t)d * f)));
+    S2S_CHECK(alloc_tiled(&w_fc2, d, f));
     S2S_CHECK(m->arena.alloc(&b_fc2, d * 4));
-    A.add(p + "self_attn.q_proj.weight", w_qkv, true, (int64_t)d * d, s_qk).scale = qscale;
+    A.add(p + "self_attn.q_proj.weight", w_qkv, true, (int64_t)d * d, s_qk).tiled(3 * d, d, 0).scale = qscale;
     A.add(p + "self_attn.q_proj.bias", b_qkv, false, d).scale = qscale;
-    A.add(p + "self_attn.k_proj.weight", off(w_qkv, (int64_t)d * d, esz), true, (int64_t)d * d, s_qk);
-    A.add(p + "self_attn.v_proj.weight", off(w_qkv, (int64_t)2 * d * d, esz), true, (int64_t)d * d, s_v);
+    A.add(p + "self_attn.k_proj.weight", w_qkv, true, (int64_t)d * d, s_qk).tiled(3 * d, d, d);
+    A.add(p + "self_attn.v_proj.weight", w_qkv, true, (int64_t)d * d, s_v).tiled(3 * d, d, 2 * d);
     A.add(p + "self_attn.v_proj.bias", b_qkv + 2 * d, false, d);
-    A.add(p + "self_attn.out_proj.weight", w_o, true, (int64_t)d * d, s_o);
+    A.add(p + "self_attn.out_proj.weight", w_o, true, (int64_t)d * d, s_o).tiled(d, d);
     A.add(p + "self_attn.out_proj.bias", b_o, false, d);
-    A.add(p + "encoder_attn.q_proj.weight", w_cq, true, (int64_t)d * d, s_qk).scale = qscale;
+    A.add(p + "encoder_attn.q_proj.weight", w_cq, true, (int64_t)d * d, s_qk).tiled(d, d).scale = qscale;
     A.add(p + "encoder_attn.q_proj.bias", b_cq, false, d).scale = qscale;
     A.add(p + "encoder_attn.k_proj.weight", off(m->ckv_w, (int64_t)i * 2 * d * d, esz), true, (int64_t)d * d, s_qk);
     A.add(p + "encoder_attn.v_proj.weight", off(m->ckv_w, (int64_t)(i * 2 + 1) * d * d, esz), true, (int64_t)d * d, s_v);
     A.add(p + "encoder_attn.v_proj.bias", m->ckv_b + (int64_t)(i * 2 + 1) * d, false, d);
-    A.add(p + "encoder_attn.out_proj.weight", w_co, true, (int64_t)d * d, s_o);
+    A.add(p + "encoder_attn.out_proj.weight", w_co, true, (int64_t)d * d, s_o).tiled(d, d);
     A.add(p + "encoder_attn.out_proj.bias", b_co, false, d);
-    A.add(p + "fc1.weight", w_fc1, true, (int64_t)f * d, s_fc1);
+    A.add(p + "fc1.weight", w_fc1, true, (int64_t)f * d, s_fc1).tiled(f, d);
     A.add(p + "fc1.bias", b_fc1, false, f);
-    A.add(p + "fc2.weight", w_fc2, true, (int64_t)d * f, s_fc2);
+    A.add(p + "fc2.weight", w_fc2, true, (int64_t)d * f, s_fc2).tiled(d, f);
     A.add(p + "fc2.bias", b_fc2, false, d);
     S2S_CHECK(add_ln(p + "self_attn_layer_norm", &l1w, &l1b));
     S2S_CHECK(add_ln(p + "encoder_attn_layer_norm", &l2w, &l2b));
@@ -226,7 +226,7 @@ int alloc_weights(s2s_whisper* m) {
   }
   S2S_CHECK(add_ln("model.decoder.layer_norm", &m->dec_lnf_w, &m->dec_lnf_b));
   S2S_CHECK(m->arena.alloc(&m->dec_d, sizeof(WhisperDecLayer) * c.dec_layers));
-  S2S_CHECK_CUDA(cudaMemcpy(m->dec_d, m->dec_h.data(), sizeof(WhisperDecLayer) * c.dec_layers, cudaMemcpyHostToDevice));
+  S2S_CHECK_CUDA(cudaMemcpy(m->dec_d, dec.data(), sizeof(WhisperDecLayer) * c.dec_layers, cudaMemcpyHostToDevice));
   return S2S_OK;
 }
 
@@ -337,41 +337,10 @@ int s2s_whisper_init_random(s2s_whisper* m, uint64_t seed) {
 
 int s2s_whisper_finalize(s2s_whisper* m) {
   S2S_REQUIRE(m, "whisper finalize: null model");
+  S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   S2S_CHECK(m->arena.check_all_bound("whisper"));
-  // decode-side weight layout: fragment-major tiles (weight_tiles.cu), built once per (re)load
-  {
-    const auto& c = m->cfg;
-    const int d = c.d_model, f = c.ffn;
-    S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
-    if (m->dec_t.empty()) {
-      m->dec_t = m->dec_h;
-      for (int i = 0; i < c.dec_layers; ++i) {
-        WhisperDecLayer& T = m->dec_t[i];
-        void *a, *b, *cq, *co, *f1, *f2;
-        S2S_CHECK(m->arena.alloc(&a, tiled_weight_elems(3 * d, d) * 2));
-        S2S_CHECK(m->arena.alloc(&b, tiled_weight_elems(d, d) * 2));
-        S2S_CHECK(m->arena.alloc(&cq, tiled_weight_elems(d, d) * 2));
-        S2S_CHECK(m->arena.alloc(&co, tiled_weight_elems(d, d) * 2));
-        S2S_CHECK(m->arena.alloc(&f1, tiled_weight_elems(f, d) * 2));
-        S2S_CHECK(m->arena.alloc(&f2, tiled_weight_elems(d, f) * 2));
-        T.w_qkv = a; T.w_o = b; T.w_cq = cq; T.w_co = co; T.w_fc1 = f1; T.w_fc2 = f2;
-      }
-      S2S_CHECK(m->arena.alloc(&m->embed_t, tiled_weight_elems(c.vocab, d) * 2));
-      S2S_CHECK_CUDA(cudaMemcpy(m->dec_d, m->dec_t.data(), sizeof(WhisperDecLayer) * c.dec_layers, cudaMemcpyHostToDevice));
-    }
-    for (int i = 0; i < c.dec_layers; ++i) {
-      const WhisperDecLayer& R = m->dec_h[i];
-      const WhisperDecLayer& T = m->dec_t[i];
-      S2S_CHECK(tile_weights_launch(R.w_qkv, 3 * d, d, const_cast<void*>(T.w_qkv), 0));
-      S2S_CHECK(tile_weights_launch(R.w_o, d, d, const_cast<void*>(T.w_o), 0));
-      S2S_CHECK(tile_weights_launch(R.w_cq, d, d, const_cast<void*>(T.w_cq), 0));
-      S2S_CHECK(tile_weights_launch(R.w_co, d, d, const_cast<void*>(T.w_co), 0));
-      S2S_CHECK(tile_weights_launch(R.w_fc1, f, d, const_cast<void*>(T.w_fc1), 0));
-      S2S_CHECK(tile_weights_launch(R.w_fc2, d, f, const_cast<void*>(T.w_fc2), 0));
-    }
-    S2S_CHECK(tile_weights_launch(m->embed, c.vocab, d, m->embed_t, 0));
-    S2S_CHECK_CUDA(cudaDeviceSynchronize());
-  }
+  S2S_CHECK_CUDA(cudaDeviceSynchronize());
+  m->arena.release_staging();
   m->finalized = true;
   return S2S_OK;
 }
@@ -494,7 +463,7 @@ static int decode_impl(s2s_whisper* m, const int32_t* prefix_h, const int32_t* p
     WhisperDecParams p{};
     p.d = d; p.heads = c.heads; p.layers = c.dec_layers; p.ffn = c.ffn; p.vocab = c.vocab; p.B = nb;
     p.max_pos = c.max_target_positions; p.n_ctx = c.max_source_positions;
-    p.lw = m->dec_d; p.embed = m->embed; p.embed_t = m->embed_t; p.pos = m->dec_pos; p.lnf_w = m->dec_lnf_w; p.lnf_b = m->dec_lnf_b;
+    p.lw = m->dec_d; p.embed = m->embed; p.pos = m->dec_pos; p.lnf_w = m->dec_lnf_w; p.lnf_b = m->dec_lnf_b;
     p.x = m->dx + (size_t)b0 * d; p.q = m->dq + (size_t)b0 * d; p.h = off(m->dh, (int64_t)b0 * c.ffn, esz);
     p.self_kv = off(m->self_kv, (int64_t)b0 * c.dec_layers * 2 * c.max_target_positions * d, esz);
     p.cross_kv = off(m->cross_kv, (int64_t)b0 * c.max_source_positions * c.dec_layers * 2 * d, esz);  // head-major

@@ -120,10 +120,10 @@ __device__ __noinline__ void wd_select(const WhisperDecParams& p, int g, int pos
     __syncthreads();
     const int feed = *s_feed;
     if (pos + 1 < p.max_pos) {
-      const T* e = reinterpret_cast<const T*>(p.embed) + (long long)feed * d;
+      const T* e = reinterpret_cast<const T*>(p.embed);
       const float* pe = p.pos + (long long)(pos + 1) * d;
 #pragma unroll 2
-      for (int i = threadIdx.x; i < d; i += DEC_THREADS) p.x[b * d + i] = DT<T>::to_f(e[i]) + pe[i];
+      for (int i = threadIdx.x; i < d; i += DEC_THREADS) p.x[b * d + i] = DT<T>::to_f(e[gv_tiled_elem(feed, i, d)]) + pe[i];
     }
   }
 }
@@ -181,7 +181,7 @@ struct WdModel {
     }
     const int g = step - (p.n_prefix - 1);
     if (ph == 8 * L && g >= 0) {
-      a.W = p.embed_t; a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 4; a.suppress = p.suppress; a.first_step = (g == 0);
+      a.W = p.embed; a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 4; a.suppress = p.suppress; a.first_step = (g == 0);
       a.logits_out = p.logits_out ? p.logits_out + (long long)g * B * p.vocab : nullptr; a.logits_ld = p.vocab;
     }
   }
@@ -354,7 +354,7 @@ struct WdcModel {
       }
     }
     const int g = step - (p.n_prefix - 1);
-    a.W = p.embed_t; a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 5; a.suppress = p.suppress; a.first_step = (g == 0);
+    a.W = p.embed; a.N = p.vocab; a.mode = EPI_LOGITS; a.plan_id = 5; a.suppress = p.suppress; a.first_step = (g == 0);
     a.logits_out = p.logits_out ? p.logits_out + (long long)g * B * p.vocab : nullptr; a.logits_ld = p.vocab;
   }
 
@@ -521,8 +521,8 @@ __global__ void whisper_decode_init_kernel(const WhisperDecParams p) {
   // x = E[first prompt token] + pos[0]; reset flags
   const int b = blockIdx.x;
   const int tok = p.tokens[b * p.max_pos];
-  const T* e = reinterpret_cast<const T*>(p.embed) + (long long)tok * p.d;
-  for (int i = threadIdx.x; i < p.d; i += blockDim.x) p.x[b * p.d + i] = DT<T>::to_f(e[i]) + p.pos[i];
+  const T* e = reinterpret_cast<const T*>(p.embed);
+  for (int i = threadIdx.x; i < p.d; i += blockDim.x) p.x[b * p.d + i] = DT<T>::to_f(e[gv_tiled_elem(tok, i, p.d)]) + p.pos[i];
   dec_init_session(p, b, p.max_new);
 }
 

@@ -4,7 +4,7 @@
 
 constexpr int ATT_CHUNK_KEYS = 64;  // keys per attention work item (== ATT_CHUNK in decode_common.cuh)
 
-struct WhisperDecLayer {      // all device pointers; 16-bit weights [out, in]: TILED layout (weight_tiles.cu) in the kernel's table
+struct WhisperDecLayer {      // all device pointers; 16-bit weights [out, in] in the tiled layout (weight_tiles.cu)
   const void* w_qkv; const float* b_qkv;   // [3d, d]; q rows pre-scaled by head_dim^-0.5, k bias = 0
   const void* w_o;   const float* b_o;     // [d, d]
   const void* w_cq;  const float* b_cq;    // cross-attention q [d, d] (pre-scaled)
@@ -17,8 +17,7 @@ struct WhisperDecLayer {      // all device pointers; 16-bit weights [out, in]: 
 struct WhisperDecParams {
   int d, heads, layers, ffn, vocab, B, max_pos, n_ctx;
   const WhisperDecLayer* lw;   // [layers] device
-  const void* embed;           // [vocab, d] 16-bit row-major (token embedding lookup)
-  const void* embed_t;         // the same matrix in the tiled layout (tied output projection)
+  const void* embed;           // [vocab, d] 16-bit, tiled: token embedding lookup (gv_tiled_elem) and tied output projection
   const float* pos;            // [max_pos, d]
   const float *lnf_w, *lnf_b;
   // state
