@@ -56,6 +56,24 @@ int s2s_set_sm_partition(s2s_ctx* ctx, int32_t ctas);
 const char* s2s_last_error(void);
 /* number of kernels this library launched in this process (all contexts, all host threads) since the last reset */
 int64_t s2s_launch_count(s2s_ctx* ctx, int reset);
+/* *out = device bytes the model objects of this process hold right now (all contexts, all host threads): weights,
+ * workspaces and the staging buffer of bind_tensor / init_random, counted when allocated and when freed.  Unlike the
+ * device's free memory it is not moved by other processes (tests, measurements). */
+int s2s_allocated_bytes(int64_t* out);
+
+/* ---- shared weights ---------------------------------------------------------------------
+ * s2s_{whisper,llama,qwen3tts}_create_shared make an object on `ctx` that reads the weights of `source` instead of a copy
+ * of its own -- e.g. one copy per GPU for the engines of two SM partitions (s2s_set_sm_partition) -- and keeps its own KV
+ * cache, workspaces and decode state.  It computes bit for bit what an object bound to the same weights computes.
+ * `source` must be finalized and on ctx's device; `cfg` must equal the source's configuration except for capacities
+ * (llama: max_sessions, max_positions, max_prefill; whisper: max_batch; qwen3tts: max_sessions, max_positions, max_text,
+ * codec.max_frames, codec.max_batch) -- any other difference is S2S_ERR_INVALID naming the field.  The llama weight format
+ * comes from the source.  The new object comes back finalized; its decode plans follow its own context's CTA budget.
+ * The weights are read-only while more than one object holds them: bind_tensor, init_random, finalize and
+ * s2s_llama_set_weight_format return S2S_ERR_INVALID on an object made this way, and on its source while such an object
+ * lives.  Objects are destroyed in any order; the weights are freed with the last of them.
+ * *_device_bytes: *weights = the weight bytes the object reads (its own or the shared ones), *total = that plus what the
+ * object allocated itself, so a set of objects sharing one source holds weights + sum(total - weights). */
 
 /* ---- Whisper (STT) ---------------------------------------------------------------------
  * Geometry mirrors transformers WhisperConfig.  compute_dtype: S2S_F16 (reference default
@@ -78,6 +96,10 @@ int s2s_whisper_bind_tensor(s2s_whisper* m, const char* name, const void* data_h
 /* Fill every parameter with seeded pseudo-random values on the device (bench only). */
 int s2s_whisper_init_random(s2s_whisper* m, uint64_t seed);
 int s2s_whisper_finalize(s2s_whisper* m);
+int s2s_whisper_create_shared(s2s_ctx* ctx, s2s_whisper* source, const s2s_whisper_config* cfg, s2s_whisper** out);
+/* *weights = encoder and decoder weights (the tiled decoder matrices and embedding, cross-attention K/V projections,
+ * positional tables); *total = that plus the log-mel tables, workspaces, KV caches and decode state (see shared weights) */
+int s2s_whisper_device_bytes(s2s_whisper* m, int64_t* weights, int64_t* total);
 
 /* decoding controls = what WhisperGenerationMixin.generate derives from generation_config */
 typedef struct {
@@ -256,8 +278,9 @@ int s2s_llama_init_random(s2s_llama* m, uint64_t seed);
 int s2s_llama_set_weight_format(s2s_llama* m, int32_t format);
 int32_t s2s_llama_weight_format(s2s_llama* m);
 int s2s_llama_finalize(s2s_llama* m);
+int s2s_llama_create_shared(s2s_ctx* ctx, s2s_llama* source, const s2s_llama_config* cfg, s2s_llama** out);
 /* Device bytes the model object holds: *weights = embedding table(s), norms and the tiled matrices; *total = that plus the
- * KV cache and every workspace.  The staging buffer of bind_tensor / init_random (as large as the largest matrix tensor)
+ * KV cache and every workspace (for an object sharing its weights, see shared weights).  The staging buffer of bind_tensor / init_random (as large as the largest matrix tensor)
  * is held from the first bind to finalize and is not counted. */
 int s2s_llama_device_bytes(s2s_llama* m, int64_t* weights, int64_t* total);
 /* Reset a KV-cache slot (new response).  Also empties the slot's seen-id set (repetition penalty), on the stream of the
@@ -405,6 +428,9 @@ int s2s_qwen3tts_bind_tensor(s2s_qwen3tts* m, const char* name, const void* data
                              int32_t dtype);
 int s2s_qwen3tts_init_random(s2s_qwen3tts* m, uint64_t seed);
 int s2s_qwen3tts_finalize(s2s_qwen3tts* m);
+int s2s_qwen3tts_create_shared(s2s_ctx* ctx, s2s_qwen3tts* source, const s2s_qwen3tts_config* cfg, s2s_qwen3tts** out);
+/* talker, code predictor, codec and text side together, with the meaning of s2s_llama_device_bytes (see shared weights) */
+int s2s_qwen3tts_device_bytes(s2s_qwen3tts* m, int64_t* weights, int64_t* total);
 /* Start an utterance in `slot`: builds the prompt ([im_start, assistant, newline] + text, codec prefix with the speaker
  * id), prefills the talker and stages the first frame's input.  text_ids_h: >= 1 text token ids.  Resets the slot's
  * token choice to greedy and empties its repetition-penalty set. */

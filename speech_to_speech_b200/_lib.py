@@ -15,14 +15,15 @@ DTYPE_CODES = {"float32": S2S_F32, "float16": S2S_F16, "bfloat16": S2S_BF16}
 
 # every symbol include/s2s_b200.h declares (checked by tests/test_abi.py)
 EXPORTED = [
-    "s2s_init", "s2s_destroy", "s2s_set_sm_partition", "s2s_last_error", "s2s_launch_count",
+    "s2s_init", "s2s_destroy", "s2s_set_sm_partition", "s2s_last_error", "s2s_launch_count", "s2s_allocated_bytes",
     "s2s_whisper_create", "s2s_whisper_destroy", "s2s_whisper_bind_tensor", "s2s_whisper_init_random",
     "s2s_whisper_finalize", "s2s_whisper_logmel", "s2s_whisper_encode", "s2s_whisper_decode",
     "s2s_whisper_detect_language", "s2s_whisper_transcribe", "s2s_whisper_set_trace", "s2s_whisper_max_decode_batch",
+    "s2s_whisper_create_shared", "s2s_whisper_device_bytes",
     "s2s_gemm", "s2s_tiled_weight_bytes", "s2s_tile_weights", "s2s_gemm_tiled", "s2s_attention", "s2s_decode_attention", "s2s_decode_gemv",
     "s2s_llama_create", "s2s_llama_destroy", "s2s_llama_bind_tensor", "s2s_llama_init_random",
     "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_set_sampling", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
-    "s2s_llama_set_weight_format", "s2s_llama_weight_format", "s2s_llama_device_bytes",
+    "s2s_llama_set_weight_format", "s2s_llama_weight_format", "s2s_llama_device_bytes", "s2s_llama_create_shared",
     "s2s_tts_postproc",
     "s2s_codec_create", "s2s_codec_destroy", "s2s_codec_bind_tensor", "s2s_codec_init_random", "s2s_codec_finalize",
     "s2s_codec_decode", "s2s_codec_samples", "s2s_codec_total_upsample", "s2s_codec_contract",
@@ -30,6 +31,7 @@ EXPORTED = [
     "s2s_qwen3tts_finalize", "s2s_qwen3tts_prefill", "s2s_qwen3tts_set_sampling", "s2s_qwen3tts_decode_frames",
     "s2s_qwen3tts_decode_frames_logits", "s2s_qwen3tts_decode_audio", "s2s_qwen3tts_decode_audio_batch",
     "s2s_qwen3tts_set_frames", "s2s_qwen3tts_frames", "s2s_qwen3tts_max_batch", "s2s_qwen3tts_codec", "s2s_qwen3tts_set_trace",
+    "s2s_qwen3tts_create_shared", "s2s_qwen3tts_device_bytes",
 ]
 
 
@@ -164,11 +166,14 @@ def load() -> C.CDLL:
     lib.s2s_destroy.argtypes = [C.c_void_p]
     lib.s2s_set_sm_partition.argtypes = [C.c_void_p, C.c_int32]
     vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
+    lib.s2s_allocated_bytes.argtypes = [C.POINTER(i64)]
     lib.s2s_whisper_create.argtypes = [vp, C.POINTER(WhisperConfig), C.POINTER(vp)]
     lib.s2s_whisper_destroy.argtypes = [vp]
     lib.s2s_whisper_bind_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]
     lib.s2s_whisper_init_random.argtypes = [vp, C.c_uint64]
     lib.s2s_whisper_finalize.argtypes = [vp]
+    lib.s2s_whisper_create_shared.argtypes = [vp, vp, C.POINTER(WhisperConfig), C.POINTER(vp)]
+    lib.s2s_whisper_device_bytes.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     lib.s2s_whisper_logmel.argtypes = [vp, vp, i64, C.POINTER(i32), i32, vp, vp]
     lib.s2s_whisper_encode.argtypes = [vp, vp, i32, vp, vp]
     lib.s2s_whisper_decode.argtypes = [vp, C.POINTER(WhisperDecodeOpts), i32, vp, vp, vp, vp, vp]
@@ -190,6 +195,7 @@ def load() -> C.CDLL:
     lib.s2s_llama_bind_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]
     lib.s2s_llama_init_random.argtypes = [vp, C.c_uint64]
     lib.s2s_llama_finalize.argtypes = [vp]
+    lib.s2s_llama_create_shared.argtypes = [vp, vp, C.POINTER(LlamaConfig), C.POINTER(vp)]
     lib.s2s_llama_set_weight_format.argtypes = [vp, i32]
     lib.s2s_llama_weight_format.argtypes = [vp]
     lib.s2s_llama_weight_format.restype = i32
@@ -220,6 +226,8 @@ def load() -> C.CDLL:
     lib.s2s_qwen3tts_bind_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]
     lib.s2s_qwen3tts_init_random.argtypes = [vp, C.c_uint64]
     lib.s2s_qwen3tts_finalize.argtypes = [vp]
+    lib.s2s_qwen3tts_create_shared.argtypes = [vp, vp, C.POINTER(Qwen3TTSConfig), C.POINTER(vp)]
+    lib.s2s_qwen3tts_device_bytes.argtypes = [vp, C.POINTER(i64), C.POINTER(i64)]
     lib.s2s_qwen3tts_prefill.argtypes = [vp, i32, C.POINTER(i32), i32, i32, vp]
     lib.s2s_qwen3tts_set_sampling.argtypes = [vp, i32, C.POINTER(Sampling), C.POINTER(Sampling)]
     lib.s2s_qwen3tts_decode_frames.argtypes = [vp, C.POINTER(i32), i32, i32, vp, vp, vp]

@@ -195,3 +195,31 @@ def release_shared(key: Hashable) -> None:
         if ent.refs <= 0:
             del _registry[key]
             ent.closer(ent.value)
+
+
+# ---- one weight copy per model and device (the handlers' share_weights=True) ------------------------------------
+# model key -> the live objects (engines or bundles) that hold or read that model's weights.  Any of them can be the source
+# of the next lane's: the library keeps the weights alive until the last object that reads them is destroyed.
+_weight_holders: dict = {}
+# taken inside acquire_shared factories and closers (which run under _registry_lock), never the other way round
+_weights_lock = threading.Lock()
+
+
+def weight_source(key: Hashable, load: Callable[[], Any], share: Callable[[Any], Any]) -> Any:
+    """The object of a new lane for model `key`: share(live) from a live object of that key, or load() -- which reads the
+    checkpoint -- when there is none.  Both run under the lock, so concurrent lanes read the checkpoint once.  Pair every
+    object returned with forget_weight_source(key, obj) before it is closed."""
+    with _weights_lock:
+        live = _weight_holders.setdefault(key, [])
+        obj = share(live[0]) if live else load()
+        live.append(obj)
+        return obj
+
+
+def forget_weight_source(key: Hashable, obj: Any) -> None:
+    """`obj` is about to be closed: it is no longer handed out as a source."""
+    with _weights_lock:
+        live = _weight_holders.get(key, [])
+        live[:] = [o for o in live if o is not obj]
+        if not live:
+            _weight_holders.pop(key, None)

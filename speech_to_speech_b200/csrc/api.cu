@@ -9,6 +9,7 @@
 
 static thread_local char g_err[1024] = "";
 static std::atomic<long long> g_launches{0};   // process-wide: lanes launch from several host threads
+static std::atomic<long long> g_device_bytes{0};   // process-wide: lanes create and destroy objects from several host threads
 
 void s2s_set_error(const char* fmt, ...) {
   va_list ap;
@@ -17,6 +18,7 @@ void s2s_set_error(const char* fmt, ...) {
   va_end(ap);
 }
 void s2s_count_launch(int n) { g_launches += n; }
+void s2s_count_device_bytes(long long delta) { g_device_bytes += delta; }
 
 extern "C" {
 
@@ -24,6 +26,12 @@ const char* s2s_last_error(void) { return g_err; }
 
 int64_t s2s_launch_count(s2s_ctx*, int reset) {
   return reset ? g_launches.exchange(0) : g_launches.load();
+}
+
+int s2s_allocated_bytes(int64_t* out) {
+  S2S_REQUIRE(out, "s2s_allocated_bytes: null argument");
+  *out = (int64_t)g_device_bytes.load();
+  return S2S_OK;
 }
 
 int s2s_init(int device, s2s_ctx** out) {

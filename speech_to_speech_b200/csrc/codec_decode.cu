@@ -613,7 +613,7 @@ int build(CodecDecoder* m) {
   // a tensor with an fp32 buffer of its own: d0 * max(d1, 1) * max(d2, 1) elements
   auto slot = [&](const std::string& name, float** out, int layout, int d0, int d1, int d2, int p, float rs, float ro = 0.f) -> int {
     const int64_t n = (int64_t)d0 * (d1 ? d1 : 1) * (d2 ? d2 : 1);
-    S2S_CHECK(A.alloc(out, (size_t)n * 4));
+    S2S_CHECK(A.alloc_weights(out, (size_t)n * 4));
     A.add(name, *out, false, n, rs, ro).as(layout, d0, d1, d2, p);
     return S2S_OK;
   };
@@ -624,8 +624,8 @@ int build(CodecDecoder* m) {
     const std::string p = "pre_transformer.layers." + std::to_string(l) + ".";
     CodecLayer& L = m->layers[l];
     // q, k, v share one [H][qd + 2 kvd] matrix; gate and up one [H][2 I] matrix (column blocks)
-    S2S_CHECK(A.alloc(&L.w_qkv, (size_t)H * (qd + 2 * kvd) * 4));
-    S2S_CHECK(A.alloc(&L.w_gu, (size_t)H * 2 * I * 4));
+    S2S_CHECK(A.alloc_weights(&L.w_qkv, (size_t)H * (qd + 2 * kvd) * 4));
+    S2S_CHECK(A.alloc_weights(&L.w_gu, (size_t)H * 2 * I * 4));
     A.add(p + "self_attn.q_proj.weight", L.w_qkv, false, (int64_t)qd * H, sh).as(W_LINEAR, qd, H, 0, 0, qd + 2 * kvd);
     A.add(p + "self_attn.k_proj.weight", L.w_qkv, false, (int64_t)kvd * H, sh).as(W_LINEAR, kvd, H, 0, qd, qd + 2 * kvd);
     A.add(p + "self_attn.v_proj.weight", L.w_qkv, false, (int64_t)kvd * H, sh).as(W_LINEAR, kvd, H, 0, qd + kvd, qd + 2 * kvd);
@@ -774,7 +774,7 @@ int codec_samples_for(const CodecDecoder* m, int T) {
   return L.back();
 }
 
-int codec_create(s2s_ctx* ctx, const s2s_codec_config* cfg, CodecDecoder** out) {
+static int create(s2s_ctx* ctx, const s2s_codec_config* cfg, CodecDecoder* source, CodecDecoder** out) {
   S2S_REQUIRE(ctx && cfg && out, "codec_create: null argument");
   S2S_REQUIRE(cfg->hidden % cfg->heads == 0 && cfg->heads % cfg->kv_heads == 0, "codec: bad head geometry");
   S2S_REQUIRE(cfg->n_upsample_rates >= 1 && cfg->n_upsample_rates <= 8 && cfg->n_upsampling_ratios >= 0 && cfg->n_upsampling_ratios <= 4,
@@ -785,9 +785,48 @@ int codec_create(s2s_ctx* ctx, const s2s_codec_config* cfg, CodecDecoder** out) 
   CodecDecoder* m = new s2s_codec();
   m->ctx = ctx;
   m->cfg = *cfg;
+  if (source) m->arena.borrow(source->arena);
   const int r = build(m);
   if (r != S2S_OK) { codec_destroy(m); return r; }
+  if (source) {   // the fp16 k-pair copies are weights too: keyed by the same (shared) fp32 matrices
+    m->tc_w = source->tc_w;
+    m->finalized = true;
+  }
   *out = m;
+  return S2S_OK;
+}
+
+int codec_create(s2s_ctx* ctx, const s2s_codec_config* cfg, CodecDecoder** out) { return create(ctx, cfg, nullptr, out); }
+
+int codec_create_shared(s2s_ctx* ctx, CodecDecoder* source, const s2s_codec_config* cfg, CodecDecoder** out) {
+  const char* who = "codec create_shared";
+  S2S_REQUIRE(ctx && source && cfg && out, "%s: null argument", who);
+  S2S_REQUIRE(source->finalized, "%s: the source is not finalized", who);
+  S2S_REQUIRE(source->ctx->device == ctx->device, "%s: the source is on device %d, the context on device %d", who,
+              source->ctx->device, ctx->device);
+  const s2s_codec_config& s = source->cfg;
+  S2S_REQUIRE_SAME(*cfg, s, codebook_size, who);
+  S2S_REQUIRE_SAME(*cfg, s, hidden, who);
+  S2S_REQUIRE_SAME(*cfg, s, heads, who);
+  S2S_REQUIRE_SAME(*cfg, s, kv_heads, who);
+  S2S_REQUIRE_SAME(*cfg, s, inter, who);
+  S2S_REQUIRE_SAME(*cfg, s, layers, who);
+  S2S_REQUIRE_SAME(*cfg, s, quantizers, who);
+  S2S_REQUIRE_SAME(*cfg, s, n_upsample_rates, who);
+  for (int i = 0; i < s.n_upsample_rates; ++i) S2S_REQUIRE_SAME(*cfg, s, upsample_rates[i], who);
+  S2S_REQUIRE_SAME(*cfg, s, n_upsampling_ratios, who);
+  for (int i = 0; i < s.n_upsampling_ratios; ++i) S2S_REQUIRE_SAME(*cfg, s, upsampling_ratios[i], who);
+  S2S_REQUIRE_SAME(*cfg, s, decoder_dim, who);
+  S2S_REQUIRE_SAME(*cfg, s, sliding_window, who);
+  S2S_REQUIRE_SAME(*cfg, s, rope_theta, who);
+  S2S_REQUIRE_SAME(*cfg, s, rms_eps, who);
+  S2S_REQUIRE_SAME(*cfg, s, precision, who);
+  return create(ctx, cfg, source, out);
+}
+
+int codec_device_bytes(const CodecDecoder* m, int64_t* weights, int64_t* total) {
+  *weights = (int64_t)m->arena.weight_bytes();
+  *total = (int64_t)m->arena.bytes();
   return S2S_OK;
 }
 
@@ -799,18 +838,21 @@ int codec_destroy(CodecDecoder* m) {
 
 int codec_bind_tensor(CodecDecoder* m, const char* name, const void* data_h, const int64_t* shape, int ndim, int dtype) {
   S2S_REQUIRE(m && name && data_h && shape, "codec bind_tensor: null argument");
+  S2S_CHECK(m->arena.check_writable("codec bind_tensor"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   return m->arena.bind("codec", name, data_h, shape, ndim, dtype, S2S_F32);
 }
 
 int codec_init_random(CodecDecoder* m, uint64_t seed) {
   S2S_REQUIRE(m, "codec init_random: null model");
+  S2S_CHECK(m->arena.check_writable("codec init_random"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   return m->arena.init_random(seed, S2S_F32);
 }
 
 int codec_finalize(CodecDecoder* m) {
   S2S_REQUIRE(m, "codec finalize: null model");
+  S2S_CHECK(m->arena.check_writable("codec finalize"));
   S2S_CHECK(m->arena.check_all_bound("codec"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   // SnakeBeta parameters -> (exp(alpha), 1 / (exp(beta) + 1e-9)): exactly those written since the last finalize, so a
@@ -827,7 +869,7 @@ int codec_finalize(CodecDecoder* m) {
   for (auto& kv : m->tc_w) {
     CodecDecoder::TcW& t = kv.second;
     const size_t words = (size_t)t.k * ((t.C_in + 1) / 2) * t.N;
-    if (!t.packed) S2S_CHECK(m->arena.alloc(&t.packed, words * 4, false));
+    if (!t.packed) S2S_CHECK(m->arena.alloc_weights(&t.packed, words * 4));
     pack_weight_pairs_kernel<<<(unsigned)std::min<size_t>((words + 255) / 256, 4096), 256>>>(kv.first, t.k, t.C_in, t.N,
                                                                                                reinterpret_cast<__half2*>(t.packed));
     S2S_LAUNCH_CHECK();

@@ -23,6 +23,10 @@ int conv1d_tc_launch(const ConvArgs& a, const void* w_pairs, cudaStream_t st);
 
 typedef s2s_codec CodecDecoder;   // the C-ABI handle is the model object
 int codec_create(s2s_ctx* ctx, const s2s_codec_config* cfg, CodecDecoder** out);
+// a codec that reads source's weights (source finalized; cfg equal to source's but for max_frames and max_batch), finalized
+int codec_create_shared(s2s_ctx* ctx, CodecDecoder* source, const s2s_codec_config* cfg, CodecDecoder** out);
+// s2s_llama_device_bytes' meaning: weights = the (possibly shared) weight store, total = that + the object's own state
+int codec_device_bytes(const CodecDecoder* m, int64_t* weights, int64_t* total);
 int codec_destroy(CodecDecoder* m);
 int codec_bind_tensor(CodecDecoder* m, const char* name, const void* data_h, const int64_t* shape, int ndim, int dtype);
 int codec_init_random(CodecDecoder* m, uint64_t seed);

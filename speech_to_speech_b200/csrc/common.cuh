@@ -15,6 +15,9 @@
 // ------------------------------------------------------------------------------------------
 void s2s_set_error(const char* fmt, ...);
 void s2s_count_launch(int n = 1);
+// s2s_allocated_bytes: every device allocation of a model object (WeightArena, WeightStore, staging buffer) adds its size
+// when made and subtracts it when freed
+void s2s_count_device_bytes(long long delta);
 
 #define S2S_CHECK_CUDA(expr)                                                              \
   do {                                                                                    \

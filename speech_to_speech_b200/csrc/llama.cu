@@ -483,7 +483,8 @@ int llama_prefill_batch(s2s_llama* m, const int32_t* slots_h, int B, const int32
 
 extern "C" {
 
-int s2s_llama_create(s2s_ctx* ctx, const s2s_llama_config* cfg, s2s_llama** out) {
+// source != nullptr: the new object reads source's weights (s2s_llama_create_shared) and comes back finalized
+static int create(s2s_ctx* ctx, const s2s_llama_config* cfg, s2s_llama* source, s2s_llama** out) {
   S2S_REQUIRE(ctx && cfg && out, "llama_create: null argument");
   S2S_REQUIRE(cfg->head_dim == 64 || cfg->head_dim == 128, "llama: head_dim must be 64 or 128");
   S2S_REQUIRE(cfg->heads % cfg->kv_heads == 0, "llama: heads %% kv_heads != 0");
@@ -495,13 +496,43 @@ int s2s_llama_create(s2s_ctx* ctx, const s2s_llama_config* cfg, s2s_llama** out)
   s2s_llama* m = new s2s_llama();
   m->ctx = ctx;
   m->cfg = *cfg;
-  m->weight_format = cfg->compute_dtype;
+  m->weight_format = source ? source->weight_format : cfg->compute_dtype;
+  if (source) m->arena.borrow(source->arena);
   int r = build(m);
+  if (r == S2S_OK && source) {
+    r = alloc_matrices(m);
+    m->lm_head_bound = true;
+    m->finalized = r == S2S_OK;
+  }
   if (r != S2S_OK) { s2s_llama_destroy(m); return r; }
   const char* dbg = getenv("S2S_DEBUG_PHASES");
   m->debug_phases = (dbg && dbg[0] == '1') ? 1 : 0;
   *out = m;
   return S2S_OK;
+}
+
+int s2s_llama_create(s2s_ctx* ctx, const s2s_llama_config* cfg, s2s_llama** out) { return create(ctx, cfg, nullptr, out); }
+
+int s2s_llama_create_shared(s2s_ctx* ctx, s2s_llama* source, const s2s_llama_config* cfg, s2s_llama** out) {
+  const char* who = "llama create_shared";
+  S2S_REQUIRE(ctx && source && cfg && out, "%s: null argument", who);
+  S2S_REQUIRE(source->finalized, "%s: the source is not finalized", who);
+  S2S_REQUIRE(source->ctx->device == ctx->device, "%s: the source is on device %d, the context on device %d", who,
+              source->ctx->device, ctx->device);
+  const s2s_llama_config& s = source->cfg;
+  S2S_REQUIRE_SAME(*cfg, s, d_model, who);
+  S2S_REQUIRE_SAME(*cfg, s, layers, who);
+  S2S_REQUIRE_SAME(*cfg, s, heads, who);
+  S2S_REQUIRE_SAME(*cfg, s, kv_heads, who);
+  S2S_REQUIRE_SAME(*cfg, s, head_dim, who);
+  S2S_REQUIRE_SAME(*cfg, s, ffn, who);
+  S2S_REQUIRE_SAME(*cfg, s, vocab, who);
+  S2S_REQUIRE_SAME(*cfg, s, rope_theta, who);
+  S2S_REQUIRE_SAME(*cfg, s, rms_eps, who);
+  S2S_REQUIRE_SAME(*cfg, s, compute_dtype, who);
+  S2S_REQUIRE_SAME(*cfg, s, qk_norm, who);
+  S2S_REQUIRE_SAME(*cfg, s, n_tables, who);
+  return create(ctx, cfg, source, out);
 }
 
 int s2s_llama_destroy(s2s_llama* m) {
@@ -513,6 +544,7 @@ int s2s_llama_destroy(s2s_llama* m) {
 int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, const int64_t* shape, int32_t ndim,
                           int32_t dtype) {
   S2S_REQUIRE(m && name && data_h && shape, "llama bind_tensor: null argument");
+  S2S_CHECK(m->arena.check_writable("llama bind_tensor"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   S2S_CHECK(alloc_matrices(m));
   S2S_CHECK(m->arena.bind("llama", name, data_h, shape, ndim, dtype, m->cfg.compute_dtype));
@@ -522,6 +554,7 @@ int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, co
 
 int s2s_llama_init_random(s2s_llama* m, uint64_t seed) {
   S2S_REQUIRE(m, "llama init_random: null model");
+  S2S_CHECK(m->arena.check_writable("llama init_random"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   S2S_CHECK(alloc_matrices(m));
   S2S_CHECK(m->arena.init_random(seed, m->cfg.compute_dtype));
@@ -531,6 +564,7 @@ int s2s_llama_init_random(s2s_llama* m, uint64_t seed) {
 
 int s2s_llama_set_weight_format(s2s_llama* m, int32_t format) {
   S2S_REQUIRE(m, "llama set_weight_format: null model");
+  S2S_CHECK(m->arena.check_writable("llama set_weight_format"));
   S2S_REQUIRE(!m->matrices, "llama set_weight_format: the weight format is fixed by the first bind, init_random or finalize");
   if (format != m->cfg.compute_dtype) {
     if (format != S2S_FP8_E4M3 || m->cfg.compute_dtype != S2S_BF16 || m->n_tables != 1) {
@@ -547,6 +581,7 @@ int32_t s2s_llama_weight_format(s2s_llama* m) { return m ? m->weight_format : S2
 
 int s2s_llama_finalize(s2s_llama* m) {
   S2S_REQUIRE(m, "llama finalize: null model");
+  S2S_CHECK(m->arena.check_writable("llama finalize"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   S2S_CHECK(alloc_matrices(m));
   if (m->n_tables == 1 && !m->lm_head_bound && m->arena.find("model.embed_tokens.weight")->bound) {

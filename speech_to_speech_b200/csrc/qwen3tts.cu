@@ -31,6 +31,8 @@
 
 extern "C" {
 int s2s_llama_create(s2s_ctx* ctx, const s2s_llama_config* cfg, s2s_llama** out);
+int s2s_llama_create_shared(s2s_ctx* ctx, s2s_llama* source, const s2s_llama_config* cfg, s2s_llama** out);
+int s2s_llama_device_bytes(s2s_llama* m, int64_t* weights, int64_t* total);
 int s2s_llama_destroy(s2s_llama* m);
 int s2s_llama_bind_tensor(s2s_llama* m, const char* name, const void* data_h, const int64_t* shape, int32_t ndim, int32_t dtype);
 int s2s_llama_init_random(s2s_llama* m, uint64_t seed);
@@ -196,7 +198,8 @@ int linear_f32(const float* x, int T, int K, const float* w, const float* b, int
 
 extern "C" {
 
-int s2s_qwen3tts_create(s2s_ctx* ctx, const s2s_qwen3tts_config* cfg, s2s_qwen3tts** out) {
+// source != nullptr: talker, code predictor, codec and text side read source's weights (s2s_qwen3tts_create_shared)
+static int create(s2s_ctx* ctx, const s2s_qwen3tts_config* cfg, s2s_qwen3tts* source, s2s_qwen3tts** out) {
   S2S_REQUIRE(ctx && cfg && out, "qwen3tts_create: null argument");
   S2S_REQUIRE(cfg->n_groups >= 3 && cfg->n_groups <= 32, "qwen3tts: n_groups in [3,32]");
   S2S_REQUIRE(cfg->max_sessions >= 1 && cfg->max_text >= 1 && cfg->max_positions >= 64, "qwen3tts: bad capacity");
@@ -217,25 +220,26 @@ int s2s_qwen3tts_create(s2s_ctx* ctx, const s2s_qwen3tts_config* cfg, s2s_qwen3t
     t.d_model = c.d_model; t.layers = c.layers; t.heads = c.heads; t.kv_heads = c.kv_heads; t.head_dim = c.head_dim; t.ffn = c.ffn;
     t.vocab = c.vocab; t.rope_theta = c.rope_theta; t.rms_eps = c.rms_eps; t.compute_dtype = c.compute_dtype;
     t.max_sessions = c.max_sessions; t.max_positions = c.max_positions; t.max_prefill = PROMPT_ROWS; t.qk_norm = 1; t.n_tables = 1;
-    r = s2s_llama_create(ctx, &t, &m->talker);
+    r = source ? s2s_llama_create_shared(ctx, source->talker, &t, &m->talker) : s2s_llama_create(ctx, &t, &m->talker);
   }
   if (r == S2S_OK) {
     s2s_llama_config p{};
     p.d_model = c.d_model; p.layers = c.cp_layers; p.heads = c.cp_heads; p.kv_heads = c.cp_kv_heads; p.head_dim = c.cp_head_dim;
     p.ffn = c.cp_ffn; p.vocab = c.cp_vocab; p.rope_theta = c.rope_theta; p.rms_eps = c.rms_eps; p.compute_dtype = c.compute_dtype;
     p.max_sessions = TTS_MAX_B; p.max_positions = 64; p.max_prefill = 1; p.qk_norm = 1; p.n_tables = c.n_groups - 1;
-    r = s2s_llama_create(ctx, &p, &m->pred);
+    r = source ? s2s_llama_create_shared(ctx, source->pred, &p, &m->pred) : s2s_llama_create(ctx, &p, &m->pred);
   }
-  if (r == S2S_OK) r = codec_create(ctx, &c.codec, &m->codec);
+  if (r == S2S_OK) r = source ? codec_create_shared(ctx, source->codec, &c.codec, &m->codec) : codec_create(ctx, &c.codec, &m->codec);
   if (r == S2S_OK && c.codec.quantizers != c.n_groups) { s2s_set_error("qwen3tts: codec quantizers %d != n_groups %d", c.codec.quantizers, c.n_groups); r = S2S_ERR_INVALID; }
   auto alloc_all = [&]() -> int {
     const int d = c.d_model, rows = c.max_text + 6;
     WeightArena& A = m->arena;
-    S2S_CHECK(A.alloc(&m->text_embed, (size_t)c.text_vocab * c.text_hidden * 2));
-    S2S_CHECK(A.alloc(&m->fc1_w, (size_t)c.text_hidden * c.ffn * 4));
-    S2S_CHECK(A.alloc(&m->fc1_b, (size_t)c.ffn * 4));
-    S2S_CHECK(A.alloc(&m->fc2_w, (size_t)c.ffn * d * 4));
-    S2S_CHECK(A.alloc(&m->fc2_b, (size_t)d * 4));
+    if (source) A.borrow(source->arena);
+    S2S_CHECK(A.alloc_weights(&m->text_embed, (size_t)c.text_vocab * c.text_hidden * 2));
+    S2S_CHECK(A.alloc_weights(&m->fc1_w, (size_t)c.text_hidden * c.ffn * 4));
+    S2S_CHECK(A.alloc_weights(&m->fc1_b, (size_t)c.ffn * 4));
+    S2S_CHECK(A.alloc_weights(&m->fc2_w, (size_t)c.ffn * d * 4));
+    S2S_CHECK(A.alloc_weights(&m->fc2_b, (size_t)d * 4));
     // init_random: fixed seeds (seed ^ 1 .. 5) and scales of their own
     A.add("text_embedding.weight", m->text_embed, true, (int64_t)c.text_vocab * c.text_hidden, 1.0f).seed = 1;
     A.add("text_projection.linear_fc1.weight", m->fc1_w, false, (int64_t)c.ffn * c.text_hidden, 1.0f / sqrtf((float)c.text_hidden))
@@ -279,7 +283,40 @@ int s2s_qwen3tts_create(s2s_ctx* ctx, const s2s_qwen3tts_config* cfg, s2s_qwen3t
   };
   if (r == S2S_OK) r = alloc_all();
   if (r != S2S_OK) { s2s_qwen3tts_destroy(m); return r; }
+  m->finalized = source != nullptr;
   *out = m;
+  return S2S_OK;
+}
+
+int s2s_qwen3tts_create(s2s_ctx* ctx, const s2s_qwen3tts_config* cfg, s2s_qwen3tts** out) { return create(ctx, cfg, nullptr, out); }
+
+int s2s_qwen3tts_create_shared(s2s_ctx* ctx, s2s_qwen3tts* source, const s2s_qwen3tts_config* cfg, s2s_qwen3tts** out) {
+  const char* who = "qwen3tts create_shared";
+  S2S_REQUIRE(ctx && source && cfg && out, "%s: null argument", who);
+  S2S_REQUIRE(source->finalized, "%s: the source is not finalized", who);
+  S2S_REQUIRE(source->ctx->device == ctx->device, "%s: the source is on device %d, the context on device %d", who,
+              source->ctx->device, ctx->device);
+  const s2s_qwen3tts_config& s = source->cfg;
+#define S2S_SAME(f) S2S_REQUIRE_SAME(*cfg, s, f, who)
+  S2S_SAME(d_model); S2S_SAME(layers); S2S_SAME(heads); S2S_SAME(kv_heads); S2S_SAME(head_dim); S2S_SAME(ffn); S2S_SAME(vocab);
+  S2S_SAME(cp_layers); S2S_SAME(cp_heads); S2S_SAME(cp_kv_heads); S2S_SAME(cp_head_dim); S2S_SAME(cp_ffn); S2S_SAME(cp_vocab);
+  S2S_SAME(n_groups); S2S_SAME(text_vocab); S2S_SAME(text_hidden); S2S_SAME(rope_theta); S2S_SAME(rms_eps); S2S_SAME(compute_dtype);
+  S2S_SAME(codec_eos); S2S_SAME(codec_nothink); S2S_SAME(codec_think_bos); S2S_SAME(codec_think_eos); S2S_SAME(codec_pad);
+  S2S_SAME(codec_bos); S2S_SAME(tts_bos); S2S_SAME(tts_eos); S2S_SAME(tts_pad); S2S_SAME(im_start); S2S_SAME(assistant);
+  S2S_SAME(newline);
+#undef S2S_SAME
+  // the codec's own fields (codec.precision included) are checked by codec_create_shared
+  return create(ctx, cfg, source, out);
+}
+
+int s2s_qwen3tts_device_bytes(s2s_qwen3tts* m, int64_t* weights, int64_t* total) {
+  S2S_REQUIRE(m && weights && total, "qwen3tts device_bytes: null argument");
+  int64_t w[3], t[3];
+  S2S_CHECK(s2s_llama_device_bytes(m->talker, &w[0], &t[0]));
+  S2S_CHECK(s2s_llama_device_bytes(m->pred, &w[1], &t[1]));
+  S2S_CHECK(codec_device_bytes(m->codec, &w[2], &t[2]));
+  *weights = w[0] + w[1] + w[2] + (int64_t)m->arena.weight_bytes();
+  *total = t[0] + t[1] + t[2] + (int64_t)m->arena.bytes();
   return S2S_OK;
 }
 
@@ -295,6 +332,7 @@ int s2s_qwen3tts_destroy(s2s_qwen3tts* m) {
 int s2s_qwen3tts_bind_tensor(s2s_qwen3tts* m, const char* name, const void* data_h, const int64_t* shape, int32_t ndim,
                              int32_t dtype) {
   S2S_REQUIRE(m && name && data_h && shape, "qwen3tts bind_tensor: null argument");
+  S2S_CHECK(m->arena.check_writable("qwen3tts bind_tensor"));   // the talker, predictor and codec are shared with it
   const std::string n(name);
   auto starts = [&](const char* p) { return n.rfind(p, 0) == 0; };
   if (starts("code2wav.")) return codec_bind_tensor(m->codec, name + 9, data_h, shape, ndim, dtype);
@@ -313,6 +351,7 @@ int s2s_qwen3tts_bind_tensor(s2s_qwen3tts* m, const char* name, const void* data
 
 int s2s_qwen3tts_init_random(s2s_qwen3tts* m, uint64_t seed) {
   S2S_REQUIRE(m, "qwen3tts init_random: null model");
+  S2S_CHECK(m->arena.check_writable("qwen3tts init_random"));
   S2S_CHECK(s2s_llama_init_random(m->talker, seed ^ 0x7a11ull));
   S2S_CHECK(s2s_llama_init_random(m->pred, seed ^ 0x9ed1ull));
   S2S_CHECK(codec_init_random(m->codec, seed ^ 0xc0decull));
@@ -321,6 +360,7 @@ int s2s_qwen3tts_init_random(s2s_qwen3tts* m, uint64_t seed) {
 
 int s2s_qwen3tts_finalize(s2s_qwen3tts* m) {
   S2S_REQUIRE(m, "qwen3tts finalize: null model");
+  S2S_CHECK(m->arena.check_writable("qwen3tts finalize"));
   S2S_CHECK(m->arena.check_all_bound("qwen3tts"));
   S2S_CHECK(s2s_llama_finalize(m->talker));
   S2S_CHECK(s2s_llama_finalize(m->pred));

@@ -24,6 +24,8 @@ int WeightArena::ensure_staging() {
     if (t.tN > 0) most = std::max(most, (size_t)t.n * (t.layout == W_INTERLEAVE ? 2 : 1) * 2);
   }
   S2S_CHECK_CUDA(cudaMalloc(&staging_, most ? most : 16));
+  staging_bytes_ = most ? most : 16;
+  s2s_count_device_bytes((long long)staging_bytes_);
   return S2S_OK;
 }
 

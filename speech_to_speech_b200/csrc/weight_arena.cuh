@@ -4,9 +4,14 @@
 // on the host as usual, staged on the device and tiled -- or quantised to FP8 -- straight into place, so no row-major copy
 // of the matrix exists.  The layout step (weight_layout / weight_upload) is pure host code, so a
 // CPU program can check it against a numpy statement of each layout (tests/test_weight_layouts.py).
+//
+// The weights live in a WeightStore of their own, held by std::shared_ptr: an object made by s2s_*_create_shared reads
+// the store of its source instead of allocating one, and the store is freed with its last holder.  Everything else an
+// object allocates (KV cache, workspaces, tables sized by its capacities, its device layer tables) is its own.
 #pragma once
 #include <string.h>
 
+#include <memory>
 #include <string>
 #include <unordered_map>
 #include <vector>
@@ -129,6 +134,23 @@ inline WeightUpload weight_upload(const WeightSlot& s) {
   return {0, (size_t)s.n * esz, (size_t)s.n * esz, 1};
 }
 
+// The weight allocations of one model object, in allocation order, shared by the objects that read them.
+struct WeightStore {
+  std::vector<std::pair<void*, size_t>> allocs;
+  size_t bytes = 0;
+  WeightStore() = default;
+  WeightStore(const WeightStore&) = delete;
+  WeightStore& operator=(const WeightStore&) = delete;
+  ~WeightStore() {
+    for (auto& a : allocs) cudaFree(a.first);
+    s2s_count_device_bytes(-(long long)bytes);
+  }
+};
+
+// s2s_*_create_shared: field f of the new object's configuration must equal the source's (only capacities may differ)
+#define S2S_REQUIRE_SAME(cfg, src, f, who) \
+  S2S_REQUIRE((cfg).f == (src).f, "%s: cfg." #f " differs from the source's (only capacities may differ)", who)
+
 // One per model object.  Error messages start with `who`.
 struct WeightArena {
   std::unordered_map<std::string, WeightSlot> slots;
@@ -138,35 +160,72 @@ struct WeightArena {
   WeightArena& operator=(const WeightArena&) = delete;
   ~WeightArena() {
     for (void* p : allocs_) cudaFree(p);
+    s2s_count_device_bytes(-(long long)bytes_);
     release_staging();
   }
 
   // storage of the tiled slots: the 16-bit compute dtype (tiles) or S2S_FP8_E4M3 (codes + row scales, bf16 sources)
   int tiled_format = 0;
 
-  // cudaMalloc (zeroed unless zero = false), freed with the arena
+  // cudaMalloc (zeroed unless zero = false), freed with the arena: the object's own state
   template <typename P> int alloc(P** out, size_t bytes, bool zero = true) {
     void* p = nullptr;
-    S2S_CHECK_CUDA(cudaMalloc(&p, bytes ? bytes : 16));
+    const size_t n = bytes ? bytes : 16;
+    S2S_CHECK_CUDA(cudaMalloc(&p, n));
     allocs_.push_back(p);
-    bytes_ += bytes ? bytes : 16;
-    if (zero) S2S_CHECK_CUDA(cudaMemset(p, 0, bytes ? bytes : 16));
+    bytes_ += n;
+    s2s_count_device_bytes((long long)n);
+    if (zero) S2S_CHECK_CUDA(cudaMemset(p, 0, n));
     *out = reinterpret_cast<P*>(p);
     return S2S_OK;
   }
-  // alloc() of weight storage: counted in weight_bytes() too
+  // weight storage, zeroed, in the store.  An arena that borrows another object's store (borrow()) allocates nothing: the
+  // k-th call returns the store's k-th allocation, which has the same size because the two objects' configurations differ
+  // only in capacities, and the weights' sizes do not depend on those.
   template <typename P> int alloc_weights(P** out, size_t bytes) {
-    S2S_CHECK(alloc(out, bytes));
-    weight_bytes_ += bytes ? bytes : 16;
+    const size_t n = bytes ? bytes : 16;
+    if (borrowed_) {
+      S2S_REQUIRE(next_ < store_->allocs.size() && store_->allocs[next_].second == n,
+                  "shared weights: allocation %zu of %zu bytes does not match the source's store", next_, n);
+      *out = reinterpret_cast<P*>(store_->allocs[next_++].first);
+      return S2S_OK;
+    }
+    void* p = nullptr;
+    S2S_CHECK_CUDA(cudaMalloc(&p, n));
+    store_->allocs.push_back({p, n});
+    store_->bytes += n;
+    s2s_count_device_bytes((long long)n);
+    S2S_CHECK_CUDA(cudaMemset(p, 0, n));
+    *out = reinterpret_cast<P*>(p);
     return S2S_OK;
   }
-  size_t bytes() const { return bytes_; }                // device bytes the arena holds (the staging buffer excluded)
-  size_t weight_bytes() const { return weight_bytes_; }
+  // read `src`'s weights from now on (before the first alloc_weights): the object shares its store and never writes it
+  void borrow(const WeightArena& src) {
+    store_ = src.store_;
+    borrowed_ = true;
+    next_ = 0;
+    tiled_format = src.tiled_format;
+  }
+  bool borrowed() const { return borrowed_; }
+  // bind_tensor / init_random / finalize (and anything else that writes weights) may run: the arena owns its store and no
+  // other object reads it -- another lane may be mid-launch on shared bytes
+  int check_writable(const char* who) const {
+    S2S_REQUIRE(!borrowed_, "%s: the weights are shared from another object and are read-only", who);
+    const long n = store_.use_count();
+    S2S_REQUIRE(n == 1, "%s: %ld other objects read these weights (destroy them first)", who, n - 1);
+    return S2S_OK;
+  }
+  size_t bytes() const { return bytes_ + store_->bytes; }   // device bytes the object reads (the staging buffer excluded)
+  size_t weight_bytes() const { return store_->bytes; }     // ... of them in the (possibly shared) weight store
   // the device buffer bind / init_random stage a tiled slot's rows in (as large as the largest such slot); models free it
   // at finalize
   void release_staging() {
-    if (staging_) cudaFree(staging_);
+    if (staging_) {
+      cudaFree(staging_);
+      s2s_count_device_bytes(-(long long)staging_bytes_);
+    }
     staging_ = nullptr;
+    staging_bytes_ = 0;
   }
   WeightSlot& add(const std::string& name, void* dst, bool half, int64_t n, float rnd_scale = 0.02f, float rnd_offset = 0.f) {
     WeightSlot& s = slots[name];
@@ -186,8 +245,12 @@ struct WeightArena {
 
  private:
   std::vector<void*> allocs_;
-  size_t bytes_ = 0, weight_bytes_ = 0;
+  size_t bytes_ = 0;
+  std::shared_ptr<WeightStore> store_ = std::make_shared<WeightStore>();
+  bool borrowed_ = false;
+  size_t next_ = 0;
   void* staging_ = nullptr;
+  size_t staging_bytes_ = 0;
   int ensure_staging();
   int stage_tiled(const WeightSlot& s, const void* bytes, int64_t rows, int row0, int rstride);
 };

@@ -124,11 +124,11 @@ int alloc_weights(s2s_whisper* m) {
   const float s_fc1 = 1.0f / sqrtf((float)d), s_fc2 = 0.5f / sqrtf((float)f);
   auto wbytes = [&](int64_t n) { return (size_t)n * esz; };
 
-  S2S_CHECK(m->arena.alloc(&m->conv1_w, wbytes((int64_t)d * 3 * c.n_mels)));
-  S2S_CHECK(m->arena.alloc(&m->conv1_b, d * 4));
-  S2S_CHECK(m->arena.alloc(&m->conv2_w, wbytes((int64_t)d * 3 * d)));
-  S2S_CHECK(m->arena.alloc(&m->conv2_b, d * 4));
-  S2S_CHECK(m->arena.alloc(&m->enc_pos, (size_t)c.max_source_positions * d * 4));
+  S2S_CHECK(m->arena.alloc_weights(&m->conv1_w, wbytes((int64_t)d * 3 * c.n_mels)));
+  S2S_CHECK(m->arena.alloc_weights(&m->conv1_b, d * 4));
+  S2S_CHECK(m->arena.alloc_weights(&m->conv2_w, wbytes((int64_t)d * 3 * d)));
+  S2S_CHECK(m->arena.alloc_weights(&m->conv2_b, d * 4));
+  S2S_CHECK(m->arena.alloc_weights(&m->enc_pos, (size_t)c.max_source_positions * d * 4));
   A.add("model.encoder.conv1.weight", m->conv1_w, true, (int64_t)d * c.n_mels * 3, 0.05f).as(W_CONV_ROWS, d, c.n_mels, 3);
   A.add("model.encoder.conv2.weight", m->conv2_w, true, (int64_t)d * d * 3, 0.03f).as(W_CONV_ROWS, d, d, 3);
   A.add("model.encoder.conv1.bias", m->conv1_b, false, d);
@@ -136,8 +136,8 @@ int alloc_weights(s2s_whisper* m) {
   A.add("model.encoder.embed_positions.weight", m->enc_pos, false, (int64_t)c.max_source_positions * d, 0.5f);
 
   auto add_ln = [&](const std::string& nm, float** w, float** b) -> int {
-    S2S_CHECK(m->arena.alloc(w, d * 4));
-    S2S_CHECK(m->arena.alloc(b, d * 4));
+    S2S_CHECK(m->arena.alloc_weights(w, d * 4));
+    S2S_CHECK(m->arena.alloc_weights(b, d * 4));
     A.add(nm + ".weight", *w, false, d, 0.1f, 1.0f);
     A.add(nm + ".bias", *b, false, d, 0.05f);
     return S2S_OK;
@@ -147,14 +147,14 @@ int alloc_weights(s2s_whisper* m) {
   for (int i = 0; i < c.enc_layers; ++i) {
     EncLayer& L = m->enc[i];
     const std::string p = "model.encoder.layers." + std::to_string(i) + ".";
-    S2S_CHECK(m->arena.alloc(&L.w_qkv, wbytes((int64_t)3 * d * d)));
-    S2S_CHECK(m->arena.alloc(&L.b_qkv, 3 * d * 4));
-    S2S_CHECK(m->arena.alloc(&L.w_o, wbytes((int64_t)d * d)));
-    S2S_CHECK(m->arena.alloc(&L.b_o, d * 4));
-    S2S_CHECK(m->arena.alloc(&L.w_fc1, wbytes((int64_t)f * d)));
-    S2S_CHECK(m->arena.alloc(&L.b_fc1, f * 4));
-    S2S_CHECK(m->arena.alloc(&L.w_fc2, wbytes((int64_t)d * f)));
-    S2S_CHECK(m->arena.alloc(&L.b_fc2, d * 4));
+    S2S_CHECK(m->arena.alloc_weights(&L.w_qkv, wbytes((int64_t)3 * d * d)));
+    S2S_CHECK(m->arena.alloc_weights(&L.b_qkv, 3 * d * 4));
+    S2S_CHECK(m->arena.alloc_weights(&L.w_o, wbytes((int64_t)d * d)));
+    S2S_CHECK(m->arena.alloc_weights(&L.b_o, d * 4));
+    S2S_CHECK(m->arena.alloc_weights(&L.w_fc1, wbytes((int64_t)f * d)));
+    S2S_CHECK(m->arena.alloc_weights(&L.b_fc1, f * 4));
+    S2S_CHECK(m->arena.alloc_weights(&L.w_fc2, wbytes((int64_t)d * f)));
+    S2S_CHECK(m->arena.alloc_weights(&L.b_fc2, d * 4));
     A.add(p + "self_attn.q_proj.weight", L.w_qkv, true, (int64_t)d * d, s_qk).scale = qscale;
     A.add(p + "self_attn.q_proj.bias", L.b_qkv, false, d).scale = qscale;
     A.add(p + "self_attn.k_proj.weight", off(L.w_qkv, (int64_t)d * d, esz), true, (int64_t)d * d, s_qk);
@@ -174,13 +174,13 @@ int alloc_weights(s2s_whisper* m) {
   // decoder.  The matrices the decode kernel streams and the token embedding (looked up, and the tied output projection)
   // are stored once, in the tiled layout (weight_tiles.cu): bind and init_random tile each tensor's rows into place.  The
   // cross-attention K/V projections are read by the encoder-side GEMM and stay row-major.
-  auto alloc_tiled = [&](void** w, int N, int K) { return m->arena.alloc(w, tiled_weight_elems(N, K) * 2); };
+  auto alloc_tiled = [&](void** w, int N, int K) { return m->arena.alloc_weights(w, tiled_weight_elems(N, K) * 2); };
   S2S_CHECK(alloc_tiled(&m->embed, c.vocab, d));
-  S2S_CHECK(m->arena.alloc(&m->dec_pos, (size_t)c.max_target_positions * d * 4));
+  S2S_CHECK(m->arena.alloc_weights(&m->dec_pos, (size_t)c.max_target_positions * d * 4));
   A.add("model.decoder.embed_tokens.weight", m->embed, true, (int64_t)c.vocab * d).tiled(c.vocab, d);
   A.add("model.decoder.embed_positions.weight", m->dec_pos, false, (int64_t)c.max_target_positions * d);
-  S2S_CHECK(m->arena.alloc(&m->ckv_w, wbytes((int64_t)c.dec_layers * 2 * d * d)));
-  S2S_CHECK(m->arena.alloc(&m->ckv_b, (size_t)c.dec_layers * 2 * d * 4));
+  S2S_CHECK(m->arena.alloc_weights(&m->ckv_w, wbytes((int64_t)c.dec_layers * 2 * d * d)));
+  S2S_CHECK(m->arena.alloc_weights(&m->ckv_b, (size_t)c.dec_layers * 2 * d * 4));
   std::vector<WhisperDecLayer> dec(c.dec_layers);
   for (int i = 0; i < c.dec_layers; ++i) {
     WhisperDecLayer& L = dec[i];
@@ -188,17 +188,17 @@ int alloc_weights(s2s_whisper* m) {
     void *w_qkv, *w_o, *w_cq, *w_co, *w_fc1, *w_fc2;
     float *b_qkv, *b_o, *b_cq, *b_co, *b_fc1, *b_fc2, *l1w, *l1b, *l2w, *l2b, *l3w, *l3b;
     S2S_CHECK(alloc_tiled(&w_qkv, 3 * d, d));
-    S2S_CHECK(m->arena.alloc(&b_qkv, 3 * d * 4));
+    S2S_CHECK(m->arena.alloc_weights(&b_qkv, 3 * d * 4));
     S2S_CHECK(alloc_tiled(&w_o, d, d));
-    S2S_CHECK(m->arena.alloc(&b_o, d * 4));
+    S2S_CHECK(m->arena.alloc_weights(&b_o, d * 4));
     S2S_CHECK(alloc_tiled(&w_cq, d, d));
-    S2S_CHECK(m->arena.alloc(&b_cq, d * 4));
+    S2S_CHECK(m->arena.alloc_weights(&b_cq, d * 4));
     S2S_CHECK(alloc_tiled(&w_co, d, d));
-    S2S_CHECK(m->arena.alloc(&b_co, d * 4));
+    S2S_CHECK(m->arena.alloc_weights(&b_co, d * 4));
     S2S_CHECK(alloc_tiled(&w_fc1, f, d));
-    S2S_CHECK(m->arena.alloc(&b_fc1, f * 4));
+    S2S_CHECK(m->arena.alloc_weights(&b_fc1, f * 4));
     S2S_CHECK(alloc_tiled(&w_fc2, d, f));
-    S2S_CHECK(m->arena.alloc(&b_fc2, d * 4));
+    S2S_CHECK(m->arena.alloc_weights(&b_fc2, d * 4));
     A.add(p + "self_attn.q_proj.weight", w_qkv, true, (int64_t)d * d, s_qk).tiled(3 * d, d, 0).scale = qscale;
     A.add(p + "self_attn.q_proj.bias", b_qkv, false, d).scale = qscale;
     A.add(p + "self_attn.k_proj.weight", w_qkv, true, (int64_t)d * d, s_qk).tiled(3 * d, d, d);
@@ -225,6 +225,7 @@ int alloc_weights(s2s_whisper* m) {
     L.ln1_w = l1w; L.ln1_b = l1b; L.ln2_w = l2w; L.ln2_b = l2b; L.ln3_w = l3w; L.ln3_b = l3b;
   }
   S2S_CHECK(add_ln("model.decoder.layer_norm", &m->dec_lnf_w, &m->dec_lnf_b));
+  // the device layer table is the object's own (an object sharing the weights uploads the same pointers to its own copy)
   S2S_CHECK(m->arena.alloc(&m->dec_d, sizeof(WhisperDecLayer) * c.dec_layers));
   S2S_CHECK_CUDA(cudaMemcpy(m->dec_d, dec.data(), sizeof(WhisperDecLayer) * c.dec_layers, cudaMemcpyHostToDevice));
   return S2S_OK;
@@ -289,7 +290,8 @@ GemmProblem plain_gemm(const void* a, int64_t lda, const void* w, int64_t ldw, i
 
 extern "C" {
 
-int s2s_whisper_create(s2s_ctx* ctx, const s2s_whisper_config* cfg, s2s_whisper** out) {
+// source != nullptr: the new object reads source's weights (s2s_whisper_create_shared) and comes back finalized
+static int create(s2s_ctx* ctx, const s2s_whisper_config* cfg, s2s_whisper* source, s2s_whisper** out) {
   S2S_REQUIRE(ctx && cfg && out, "whisper_create: null argument");
   S2S_REQUIRE(cfg->d_model % 64 == 0 && cfg->d_model / cfg->heads == 64, "whisper: head_dim must be 64 (d=%d heads=%d)",
               cfg->d_model, cfg->heads);
@@ -301,15 +303,46 @@ int s2s_whisper_create(s2s_ctx* ctx, const s2s_whisper_config* cfg, s2s_whisper*
   s2s_whisper* m = new s2s_whisper();
   m->ctx = ctx;
   m->cfg = *cfg;
+  if (source) m->arena.borrow(source->arena);
   int r = build_tables(m);
   if (r == S2S_OK) r = alloc_weights(m);
   if (r == S2S_OK) r = alloc_workspace(m);
   if (r != S2S_OK) { s2s_whisper_destroy(m); return r; }
+  m->finalized = source != nullptr;
   const char* dbg = getenv("S2S_DEBUG_PHASES");
   m->debug_phases = (dbg && dbg[0] == '1') ? 1 : 0;
   const char* cl = getenv("S2S_WHISPER_CLUSTER");  // "0": always use the 8-phase kernel (A/B comparisons)
   m->cluster_decode = (cl && cl[0] == '0') ? 0 : 1;
   *out = m;
+  return S2S_OK;
+}
+
+int s2s_whisper_create(s2s_ctx* ctx, const s2s_whisper_config* cfg, s2s_whisper** out) { return create(ctx, cfg, nullptr, out); }
+
+int s2s_whisper_create_shared(s2s_ctx* ctx, s2s_whisper* source, const s2s_whisper_config* cfg, s2s_whisper** out) {
+  const char* who = "whisper create_shared";
+  S2S_REQUIRE(ctx && source && cfg && out, "%s: null argument", who);
+  S2S_REQUIRE(source->finalized, "%s: the source is not finalized", who);
+  S2S_REQUIRE(source->ctx->device == ctx->device, "%s: the source is on device %d, the context on device %d", who,
+              source->ctx->device, ctx->device);
+  const s2s_whisper_config& s = source->cfg;
+  S2S_REQUIRE_SAME(*cfg, s, d_model, who);
+  S2S_REQUIRE_SAME(*cfg, s, heads, who);
+  S2S_REQUIRE_SAME(*cfg, s, enc_layers, who);
+  S2S_REQUIRE_SAME(*cfg, s, dec_layers, who);
+  S2S_REQUIRE_SAME(*cfg, s, ffn, who);
+  S2S_REQUIRE_SAME(*cfg, s, n_mels, who);
+  S2S_REQUIRE_SAME(*cfg, s, vocab, who);
+  S2S_REQUIRE_SAME(*cfg, s, max_source_positions, who);
+  S2S_REQUIRE_SAME(*cfg, s, max_target_positions, who);
+  S2S_REQUIRE_SAME(*cfg, s, compute_dtype, who);
+  return create(ctx, cfg, source, out);
+}
+
+int s2s_whisper_device_bytes(s2s_whisper* m, int64_t* weights, int64_t* total) {
+  S2S_REQUIRE(m && weights && total, "whisper device_bytes: null argument");
+  *weights = (int64_t)m->arena.weight_bytes();
+  *total = (int64_t)m->arena.bytes();
   return S2S_OK;
 }
 
@@ -324,6 +357,7 @@ int s2s_whisper_destroy(s2s_whisper* m) {
 int s2s_whisper_bind_tensor(s2s_whisper* m, const char* name, const void* data_h, const int64_t* shape, int32_t ndim,
                             int32_t dtype) {
   S2S_REQUIRE(m && name && data_h && shape, "whisper bind_tensor: null argument");
+  S2S_CHECK(m->arena.check_writable("whisper bind_tensor"));
   if (strcmp(name, "proj_out.weight") == 0) return S2S_OK;  // tied to embed_tokens
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   return m->arena.bind("whisper", name, data_h, shape, ndim, dtype, m->cfg.compute_dtype);
@@ -331,12 +365,14 @@ int s2s_whisper_bind_tensor(s2s_whisper* m, const char* name, const void* data_h
 
 int s2s_whisper_init_random(s2s_whisper* m, uint64_t seed) {
   S2S_REQUIRE(m, "whisper init_random: null model");
+  S2S_CHECK(m->arena.check_writable("whisper init_random"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   return m->arena.init_random(seed, m->cfg.compute_dtype);
 }
 
 int s2s_whisper_finalize(s2s_whisper* m) {
   S2S_REQUIRE(m, "whisper finalize: null model");
+  S2S_CHECK(m->arena.check_writable("whisper finalize"));
   S2S_CHECK_CUDA(cudaSetDevice(m->ctx->device));
   S2S_CHECK(m->arena.check_all_bound("whisper"));
   S2S_CHECK_CUDA(cudaDeviceSynchronize());

@@ -64,6 +64,21 @@ def launch_count(device: int = 0, reset: bool = False) -> int:
     return int(_lib.load().s2s_launch_count(get_context(device), 1 if reset else 0))
 
 
+def allocated_bytes(device: int = 0) -> int:
+    """Device bytes the library's model objects hold right now, counted at every allocation and free (include/s2s_b200.h
+    s2s_allocated_bytes).  The count is process-wide, over all devices and lanes; other processes on the GPU do not move it."""
+    get_context(device)
+    n = C.c_int64(0)
+    check(_lib.load().s2s_allocated_bytes(C.byref(n)), "s2s_allocated_bytes")
+    return int(n.value)
+
+
+def _device_bytes(fn, handle, what: str) -> tuple[int, int]:
+    w, t = C.c_int64(0), C.c_int64(0)
+    check(fn(handle, C.byref(w), C.byref(t)), what)
+    return int(w.value), int(t.value)
+
+
 def _stream_ptr(device: int) -> C.c_void_p:
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
@@ -133,6 +148,27 @@ class WhisperEngine:
     def init_random(self, seed: int = 0) -> None:
         check(self.lib.s2s_whisper_init_random(self.handle, seed), "s2s_whisper_init_random")
         check(self.lib.s2s_whisper_finalize(self.handle), "s2s_whisper_finalize")
+
+    def share(self, lane: int, lanes: int, max_batch: Optional[int] = None) -> "WhisperEngine":
+        """A new engine on lane `lane` of `lanes` that reads this engine's weights (one copy per GPU): its own workspaces and
+        caches, sized by max_batch (default: this engine's).  This engine must be loaded; neither can be reloaded while both
+        live.  Bit for bit what an engine loaded with the same weights computes (include/s2s_b200.h shared weights)."""
+        eng = object.__new__(WhisperEngine)
+        eng.lib, eng.device, eng.geometry, eng.dtype = self.lib, self.device, dict(self.geometry), self.dtype
+        eng.ctx = get_context(self.device, lane, lanes)
+        eng.cfg = WhisperConfig.from_buffer_copy(self.cfg)
+        if max_batch is not None:
+            eng.cfg.max_batch = max_batch
+        eng.max_batch = eng.cfg.max_batch
+        eng.handle = C.c_void_p()
+        check(self.lib.s2s_whisper_create_shared(eng.ctx, self.handle, C.byref(eng.cfg), C.byref(eng.handle)),
+              "s2s_whisper_create_shared")
+        return eng
+
+    def device_bytes(self) -> tuple[int, int]:
+        """(weights, total): device bytes of the weights the engine reads (its own, or those it shares) and that plus
+        what the engine allocated itself (log-mel tables, workspaces, KV caches)."""
+        return _device_bytes(self.lib.s2s_whisper_device_bytes, self.handle, "s2s_whisper_device_bytes")
 
     # -- device-resident API -------------------------------------------------------------------
     def logmel(self, pcm: torch.Tensor, n_samples: Sequence[int], return_mel: bool = False) -> Optional[torch.Tensor]:
@@ -436,6 +472,27 @@ class LlamaEngine:
         check(self.lib.s2s_llama_init_random(self.handle, seed), "s2s_llama_init_random")
         check(self.lib.s2s_llama_finalize(self.handle), "s2s_llama_finalize")
 
+    def share(self, lane: int, lanes: int, max_sessions: Optional[int] = None, max_positions: Optional[int] = None,
+              max_prefill: Optional[int] = None) -> "LlamaEngine":
+        """A new engine on lane `lane` of `lanes` that reads this engine's weights (one copy per GPU) in their format: its
+        own KV cache, workspaces and sampling state, sized by the given capacities (default: this engine's).  This engine
+        must be loaded; neither can be reloaded while both live, and they may be closed in any order.  Bit for bit what an
+        engine loaded with the same weights computes (include/s2s_b200.h shared weights)."""
+        eng = object.__new__(LlamaEngine)
+        eng.lib, eng.device, eng.geometry, eng.weight_dtype = self.lib, self.device, dict(self.geometry), self.weight_dtype
+        eng.ctx = get_context(self.device, lane, lanes)
+        cfg = LlamaConfig.from_buffer_copy(self.cfg)
+        if max_sessions is not None:
+            cfg.max_sessions = max_sessions
+        if max_positions is not None:
+            cfg.max_positions = min(max_positions, int(self.geometry.get("max_positions", max_positions)))
+        if max_prefill is not None:
+            cfg.max_prefill = max_prefill
+        eng.cfg, eng.max_positions = cfg, cfg.max_positions
+        eng.handle = C.c_void_p()
+        check(self.lib.s2s_llama_create_shared(eng.ctx, self.handle, C.byref(cfg), C.byref(eng.handle)), "s2s_llama_create_shared")
+        return eng
+
     def reset(self, slot: int = 0) -> None:
         check(self.lib.s2s_llama_session_reset(self.handle, slot), "s2s_llama_session_reset")
 
@@ -494,10 +551,9 @@ class LlamaEngine:
 
     def device_bytes(self) -> tuple[int, int]:
         """(weights, total): device bytes the engine holds for its weights (embedding, norms, the one tiled copy of the
-        projections and lm_head) and in all (KV cache and workspaces included)."""
-        w, t = C.c_int64(0), C.c_int64(0)
-        check(self.lib.s2s_llama_device_bytes(self.handle, C.byref(w), C.byref(t)), "s2s_llama_device_bytes")
-        return int(w.value), int(t.value)
+        projections and lm_head) and in all (KV cache and workspaces included).  An engine made by share() reports the
+        weights it reads, so total - weights is what it allocated itself."""
+        return _device_bytes(self.lib.s2s_llama_device_bytes, self.handle, "s2s_llama_device_bytes")
 
     def set_trace(self, trace: Optional[torch.Tensor]) -> None:
         """trace: cuda int64 [2, capacity, 6] or None (profiling aid, see include/s2s_b200.h)."""
@@ -636,12 +692,46 @@ class Qwen3TTSEngine:
                   "tts_bos", "tts_eos", "tts_pad", "im_start", "assistant", "newline"):
             setattr(cfg, k, int(g[k]))
         cfg.codec = codec_config(codec_geometry, codec_max_frames, codec_precision, max_batch=min(16, max_sessions))
+        self._create(cfg, dict(codec_geometry), None)
+
+    def _create(self, cfg: Qwen3TTSConfig, codec_geometry: dict, source: Optional["Qwen3TTSEngine"]) -> None:
         self.cfg = cfg
         self.n_groups = cfg.n_groups
         self.codec_eos = cfg.codec_eos
         self.handle = C.c_void_p()
-        check(self.lib.s2s_qwen3tts_create(self.ctx, C.byref(cfg), C.byref(self.handle)), "s2s_qwen3tts_create")
-        self.codec = CodecEngine(codec_geometry, device=device, _handle=C.c_void_p(self.lib.s2s_qwen3tts_codec(self.handle)), _owner=self)
+        if source is None:
+            check(self.lib.s2s_qwen3tts_create(self.ctx, C.byref(cfg), C.byref(self.handle)), "s2s_qwen3tts_create")
+        else:
+            check(self.lib.s2s_qwen3tts_create_shared(self.ctx, source.handle, C.byref(cfg), C.byref(self.handle)),
+                  "s2s_qwen3tts_create_shared")
+        self.codec = CodecEngine(codec_geometry, device=self.device, _handle=C.c_void_p(self.lib.s2s_qwen3tts_codec(self.handle)),
+                                 _owner=self)
+
+    def share(self, lane: int, lanes: int, max_sessions: Optional[int] = None, max_positions: Optional[int] = None,
+              max_text: Optional[int] = None, codec_max_frames: Optional[int] = None) -> "Qwen3TTSEngine":
+        """A new engine on lane `lane` of `lanes` that reads this engine's weights -- talker, code predictor, codec and text
+        side, one copy per GPU -- with its own sessions, history and workspaces, sized by the given capacities (default:
+        this engine's; the codec batches min(16, max_sessions) sequences).  This engine must be loaded; neither can be
+        reloaded while both live.  Bit for bit what an engine loaded with the same weights computes."""
+        eng = object.__new__(Qwen3TTSEngine)
+        eng.lib, eng.device, eng.geometry = self.lib, self.device, dict(self.geometry)
+        eng.ctx = get_context(self.device, lane, lanes)
+        cfg = Qwen3TTSConfig.from_buffer_copy(self.cfg)
+        if max_sessions is not None:
+            cfg.max_sessions = max_sessions
+            cfg.codec.max_batch = min(16, max_sessions)
+        if max_positions is not None:
+            cfg.max_positions = max_positions
+        if max_text is not None:
+            cfg.max_text = max_text
+        if codec_max_frames is not None:
+            cfg.codec.max_frames = codec_max_frames
+        eng._create(cfg, dict(self.codec.geometry), self)
+        return eng
+
+    def device_bytes(self) -> tuple[int, int]:
+        """(weights, total) of talker, code predictor, codec and text side together, as LlamaEngine.device_bytes."""
+        return _device_bytes(self.lib.s2s_qwen3tts_device_bytes, self.handle, "s2s_qwen3tts_device_bytes")
 
     def load_state_dict(self, weights, codec_weights) -> None:
         _bind_all(self.lib.s2s_qwen3tts_bind_tensor, self.handle, weights, "qwen3tts")

@@ -11,7 +11,11 @@ launches, so cancellation is polled every `stream_chunk_tokens` tokens.  No CPU 
 `gen_kwargs["max_sessions"] = N` (N = number of pipeline units) makes all handler instances of the process with the same
 (model, dtype, device) share ONE engine -- one copy of the weights, N KV-cache slots -- and merges the decode chunks of
 concurrent sessions into one persistent launch through the SessionBatcher (`batcher.py`): the kernel serves up to
-`engine.max_decode_batch()` sessions of different lengths per launch at the cost of one weight stream."""
+`engine.max_decode_batch()` sessions of different lengths per launch at the cost of one weight stream.
+
+`gen_kwargs["share_weights"] = True` goes one step further with lanes: the engines of all lanes of a (model, dtype,
+weight_dtype, device) read ONE copy of the weights (LlamaEngine.share) and the checkpoint is read once per process; each
+lane keeps its own engine, KV-cache slots, batcher and stream."""
 from __future__ import annotations
 
 import contextlib
@@ -21,7 +25,7 @@ import random
 import threading
 from typing import Any, Callable, Iterator, Optional, Sequence
 
-from ..batcher import SessionBatcher, acquire_shared, assign_lane, release_shared
+from ..batcher import SessionBatcher, acquire_shared, assign_lane, forget_weight_source, release_shared, weight_source
 from ..host import _stub_optional
 
 logger = logging.getLogger(__name__)
@@ -276,6 +280,13 @@ class _LlamaBundle:
             self.batcher.close()
         self.engine.close()
 
+    def share(self, lane: int, lanes: int, max_sessions: int, max_positions: int, batch_wait_s: float,
+              batch_gap_s: Optional[float]) -> "_LlamaBundle":
+        """A bundle for another lane whose engine reads this bundle's weights (LlamaEngine.share), same tokenizer and EOS ids."""
+        engine = self.engine.share(lane, lanes, max_sessions=max_sessions, max_positions=max_positions)
+        return _LlamaBundle(engine, self.tokenizer, self.eos_ids, max_sessions, batch_wait_s, lane, lanes, batch_gap_s,
+                            self.generation_config)
+
 
 def geometry_from_hf_config(c: Any, max_positions: int) -> dict:
     """Engine geometry from a transformers config, REJECTING everything the kernels do not implement instead of loading
@@ -354,8 +365,10 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
         if weight_dtype not in (None, "float8_e4m3"):
             raise ValueError(f"weight_dtype={weight_dtype!r}: supported values are None (weights stored as torch_dtype) and 'float8_e4m3'")
         fmt = {"weight_dtype": weight_dtype} if weight_dtype else {}
+        # one weight copy for all lanes of the model (LlamaEngine.share): off unless asked for
+        share_weights = bool(self.gen_kwargs.pop("share_weights", False))
 
-        def build() -> _LlamaBundle:
+        def load() -> _LlamaBundle:
             if model_name.startswith("random:"):
                 parts = model_name.split(":")
                 geom = LLAMA_GEOMETRIES[parts[1]]
@@ -380,10 +393,18 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
             del hf
             return _LlamaBundle(engine, tokenizer, eos_ids, max_sessions, batch_wait_s, lane, lanes, batch_gap_s, ckpt_gen)
 
+        self._weights_key = ("llama", model_name, torch_dtype, weight_dtype, dev) if share_weights else None
+
+        def build() -> _LlamaBundle:
+            if self._weights_key is None:
+                return load()
+            return weight_source(self._weights_key, load,
+                                 lambda src: src.share(lane, lanes, max_sessions, max_pos, batch_wait_s, batch_gap_s))
+
         if model_name.startswith("random:"):
             resolve_generation(self.gen_kwargs)
         self._shared_key = ("llama", model_name, torch_dtype, weight_dtype, dev, max_sessions, max_pos, lane, lanes) if max_sessions > 1 else None
-        self.bundle = acquire_shared(self._shared_key, build, lambda b: b.close()) if self._shared_key else build()
+        self.bundle = acquire_shared(self._shared_key, build, self._close_bundle) if self._shared_key else build()
         self.engine, self.tokenizer, self.eos_ids = self.bundle.engine, self.bundle.tokenizer, self.bundle.eos_ids
         self.sampling = resolve_generation(self.gen_kwargs, getattr(self.bundle, "generation_config", None))
         self.slot = self.bundle.acquire_slot()
@@ -437,6 +458,11 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
         for _ in self.generate_text_stream([1, 2, 3, 4], max_new_tokens=4):
             pass
 
+    def _close_bundle(self, bundle: _LlamaBundle) -> None:
+        if getattr(self, "_weights_key", None) is not None:   # never handed out as a weight source once closing
+            forget_weight_source(self._weights_key, bundle)
+        bundle.close()
+
     def cleanup(self) -> None:
         bundle = getattr(self, "bundle", None)
         if bundle is None:
@@ -446,7 +472,7 @@ class B200LanguageModelHandler(_Base if _Base is not None else _StandaloneBase):
         if self._shared_key is not None:
             release_shared(self._shared_key)  # the last handler of the process closes the shared engine
         else:
-            bundle.close()
+            self._close_bundle(bundle)
 
 
 class _IdTokenizer:

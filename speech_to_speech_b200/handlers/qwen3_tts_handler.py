@@ -17,6 +17,8 @@ session-voice logic unchanged; on a machine without the reference it subclasses 
 
 `gen_kwargs["max_sessions"] = N` (or setup kwarg `max_sessions`) shares ONE engine between the N pipeline units of the
 process and merges the chunk requests of concurrently speaking sessions into one launch sequence (tts_model.py).
+`share_weights=True` (setup kwarg or gen_kwargs) lets the engines of all lanes of a (model, dtype, device, codec precision)
+read ONE copy of the weights (B200Qwen3TTS.share); each lane keeps its own engine, sessions and batcher.
 
 Sampling: the qwen-tts generation keywords in gen_kwargs (`do_sample, temperature, top_k, top_p, repetition_penalty,
 subtalker_dosample, subtalker_temperature, subtalker_top_k, subtalker_top_p`, tts_model.SAMPLING_KEYWORDS) and
@@ -33,7 +35,7 @@ from typing import Any, Optional
 
 import numpy as np
 
-from ..batcher import acquire_shared, assign_lane, release_shared
+from ..batcher import acquire_shared, assign_lane, forget_weight_source, release_shared, weight_source
 from ..tts_model import _UNSUPPORTED_SAMPLING, SAMPLING_KEYWORDS, B200Qwen3TTS, DeviceAudio, resolve_sampling
 
 logger = logging.getLogger(__name__)
@@ -73,8 +75,10 @@ class B200Qwen3TTSHandler(_Base):  # type: ignore[misc, valid-type]
     _b200_shared_key: Optional[tuple] = None
 
     def setup(self, *args: Any, max_sessions: Optional[int] = None, lane: Optional[int] = None, lanes: Optional[int] = None,
-              **kwargs: Any) -> None:
+              share_weights: Optional[bool] = None, **kwargs: Any) -> None:
         gk = dict(kwargs.get("gen_kwargs") or {})
+        self._b200_share_weights = bool(share_weights if share_weights is not None else gk.pop("share_weights", False))
+        gk.pop("share_weights", None)
         self._b200_max_sessions = int(max_sessions if max_sessions is not None else gk.pop("max_sessions", 1))
         # SM partition: the handler instances of lane i share lane i's engine (engine.get_context); see INTEGRATION.md section 4
         self._b200_lanes = max(1, int(lanes if lanes is not None else gk.pop("lanes", 1)))
@@ -110,15 +114,24 @@ class B200Qwen3TTSHandler(_Base):  # type: ignore[misc, valid-type]
         prec = 0 if getattr(self, "parity_mode", False) else 1
         lane, lanes = getattr(self, "_b200_lane", 0), getattr(self, "_b200_lanes", 1)
         key = ("qwen3tts", model_name, dt, dev, n, prec, lane, lanes)
+        wkey = ("qwen3tts", model_name, dt, dev, prec) if getattr(self, "_b200_share_weights", False) else None
 
-        def build() -> B200Qwen3TTS:
+        def load() -> B200Qwen3TTS:
             if model_name.startswith("random:"):
                 return B200Qwen3TTS.from_random(model_name.split(":", 1)[1], seed=self._b200_seed, dtype=dt, device=dev, max_sessions=n,
                                                 codec_precision=prec, lane=lane, lanes=lanes)
             return B200Qwen3TTS.from_pretrained(model_name, device=device, dtype=self.dtype, attn_implementation=attn_implementation,
                                                 backend=backend, max_sessions=n, codec_precision=prec, lane=lane, lanes=lanes)
 
-        self.model = acquire_shared(key, build, lambda m: m.close())
+        def build() -> B200Qwen3TTS:
+            return load() if wkey is None else weight_source(wkey, load, lambda src: src.share(lane, lanes, max_sessions=n))
+
+        def close(m: B200Qwen3TTS) -> None:
+            if wkey is not None:   # never handed out as a weight source once closing
+                forget_weight_source(wkey, m)
+            m.close()
+
+        self.model = acquire_shared(key, build, close)
         if getattr(self, "_b200_sampling", None) or getattr(self, "_b200_sampling_seed", None) is not None:
             self.model = HandlerModelView(self.model, self._b200_sampling, self._b200_sampling_seed)
         self._b200_shared_key = key

@@ -21,7 +21,7 @@ from typing import Any, Iterator, Optional
 import numpy as np
 
 from ..host import resolve
-from ..batcher import SessionBatcher, acquire_shared, assign_lane, release_shared
+from ..batcher import SessionBatcher, acquire_shared, assign_lane, forget_weight_source, release_shared, weight_source
 
 logger = logging.getLogger(__name__)
 _api = resolve()
@@ -130,6 +130,13 @@ class _EngineBundle:
             self.batcher.close()
         self.engine.close()
 
+    def share(self, lane: int, lanes: int, max_batch: int, batch_wait_s: float, batch_gap_s: Optional[float]) -> "_EngineBundle":
+        """A bundle for another lane whose engine reads this bundle's weights (WhisperEngine.share), same tokens and processor."""
+        bundle = _EngineBundle(self.E, self.engine.share(lane, lanes, max_batch=max_batch), self.tokens, self.decode_text, max_batch,
+                               batch_wait_s, lane, lanes, batch_gap_s)
+        bundle.processor = getattr(self, "processor", None)
+        return bundle
+
 
 class B200WhisperSTTHandler(_api.BaseSTTHandler):
     """Speech-to-text on the H100 engine.  `model_name`: a local transformers Whisper checkpoint directory / hub id
@@ -141,7 +148,10 @@ class B200WhisperSTTHandler(_api.BaseSTTHandler):
 
     def setup(self, model_name: str = "distil-whisper/distil-large-v3", device: str = "cuda", torch_dtype: str = "float16",
               compile_mode: Optional[str] = None, language: Optional[str] = None, gen_kwargs: dict[str, Any] = {},
-              max_batch: int = 1, batch_wait_ms: float = 6.0, lane: Optional[int] = None, lanes: int = 1, batch_gap_ms: float = 0.8) -> None:
+              max_batch: int = 1, batch_wait_ms: float = 6.0, lane: Optional[int] = None, lanes: int = 1, batch_gap_ms: float = 0.8,
+              share_weights: bool = False) -> None:
+        """share_weights: the engines of all lanes of a (model, dtype, device) read ONE copy of the weights
+        (WhisperEngine.share) and the checkpoint is read once per process; each lane keeps its own engine and batcher."""
         if not str(device).startswith("cuda"):
             raise ValueError(f"B200WhisperSTTHandler runs on CUDA (sm_90a) only, got device={device!r}; there is no CPU fallback")
         from .. import engine as E  # raises ImportError if libs2s_b200.so is not built
@@ -167,11 +177,19 @@ class B200WhisperSTTHandler(_api.BaseSTTHandler):
             lane = assign_lane(("whisper", model_name, self.device_index), self.lanes)
         self.lane = int(lane) % self.lanes
         self._shared_key = None
+        self._weights_key = ("whisper", model_name, torch_dtype, self.device_index) if share_weights else None
+
+        def build() -> _EngineBundle:
+            if self._weights_key is None:
+                return self._load(model_name)
+            return weight_source(self._weights_key, lambda: self._load(model_name),
+                                 lambda src: src.share(self.lane, self.lanes, self.max_batch, self.batch_wait_s, self.batch_gap_s))
+
         if self.max_batch > 1:
             self._shared_key = ("whisper", model_name, torch_dtype, self.device_index, self.max_batch, self.lane, self.lanes)
-            self.bundle = acquire_shared(self._shared_key, lambda: self._load(model_name), lambda b: b.close())
+            self.bundle = acquire_shared(self._shared_key, build, self._close_bundle)
         else:
-            self.bundle = self._load(model_name)
+            self.bundle = build()
         self.engine, self.tokens, self._decode_text = self.bundle.engine, self.bundle.tokens, self.bundle.decode_text
         self.processor = getattr(self.bundle, "processor", None)
         self.warmup()
@@ -298,7 +316,12 @@ class B200WhisperSTTHandler(_api.BaseSTTHandler):
         if self._shared_key is not None:
             release_shared(self._shared_key)  # the last handler of the process closes the shared engine
         else:
-            bundle.close()
+            self._close_bundle(bundle)
+
+    def _close_bundle(self, bundle: _EngineBundle) -> None:
+        if getattr(self, "_weights_key", None) is not None:   # never handed out as a weight source once closing
+            forget_weight_source(self._weights_key, bundle)
+        bundle.close()
 
 
 # Whisper geometries (transformers WhisperConfig values of the public checkpoints; SURVEY.md Appendix A)

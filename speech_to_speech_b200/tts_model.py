@@ -182,6 +182,9 @@ class B200Qwen3TTS:
         # alternate in half-full launches (measured: mean batch 7.8 of 16 with a 0.6 ms gap)
         self.engine = engine
         self.lane, self.lanes = int(lane), int(lanes)
+        self.max_sessions = int(max_sessions)
+        self._options = dict(batch_wait_s=batch_wait_s, tts_model_type=tts_model_type, batch_gap_s=batch_gap_s,
+                             prefetch_chunks=prefetch_chunks, sampling=sampling, sampling_seed=sampling_seed)
         self.prefetch_chunks = bool(prefetch_chunks)   # False: request chunk k + 1 only after the consumer took chunk k (A/B, tests)
         self.tokenize = tokenize
         # default token choice of generate_custom_voice_streaming (None = greedy; COUSIN_SAMPLING = the cousin's) and one
@@ -256,6 +259,13 @@ class B200Qwen3TTS:
         tok = AutoTokenizer.from_pretrained(model_name)
         return cls(eng, lambda text: tok.encode(text, add_special_tokens=False), cfg.get("speaker_id") or DEFAULT_SPEAKERS,
                    max_sessions=max_sessions, lane=lane, lanes=lanes, sampling=sampling, sampling_seed=sampling_seed)
+
+    def share(self, lane: int, lanes: int, max_sessions: Optional[int] = None) -> "B200Qwen3TTS":
+        """The same model on lane `lane` of `lanes` (default: as many session slots as this one) with the same speakers,
+        tokenizer and options, on an engine that reads this model's weights (Qwen3TTSEngine.share): one weight copy per GPU."""
+        n = int(max_sessions if max_sessions is not None else self.max_sessions)
+        eng = self.engine.share(lane, lanes, max_sessions=n)
+        return type(self)(eng, self.tokenize, self.speakers, max_sessions=n, lane=lane, lanes=lanes, **self._options)
 
     # ---- the calls the handler makes ------------------------------------------------------------------------------------
     def get_supported_speakers(self) -> list:
