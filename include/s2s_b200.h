@@ -147,22 +147,46 @@ int s2s_whisper_transcribe(s2s_whisper* m, const s2s_whisper_decode_opts* opts, 
                            int64_t pcm_stride, const int32_t* n_samples_h, int32_t B, int32_t* ids_out_h,
                            int32_t* len_out_h, void* stream);
 
-/* ---- generic GEMM (exposed for tests / roofline benches) --------------------------------
- * C[M,N] = A[M,K] * W[N,K]^T (+bias), wgmma + TMA; dtype S2S_F16 or S2S_BF16, fp32 accumulate.
- * out_dtype: S2S_F32 or same as dtype.  act: 0 none, 1 exact GELU.                          */
-int s2s_gemm(s2s_ctx* ctx, const void* a_d, const void* w_d, const float* bias_d, void* c_d, int32_t M,
-             int32_t N, int32_t K, int32_t dtype, int32_t out_dtype, int32_t act, void* stream);
+/* ---- the prefill / encoder GEMM by itself (exposed for tests / roofline benches) ----------
+ * The wgmma + TMA kernel every Whisper encoder op and every Llama-family prefill projection runs, in any form those call
+ * sites use (fields as the library's own GemmProblem):
+ *   v[b][m][n] = sum_k A[b][m][k] W[n][k] (+ bias[n]),   A[b][m][k] at a + b*a_batch_stride + m*a_row_stride + k,
+ * fp32 accumulation; a_row_stride < K reads overlapping windows (Whisper's convolutions without im2col).  W: w_layout 0
+ * row-major [N][ldw]; 1 the 16-bit tiles of s2s_tile_weights (K % 32 == 0); 2 its FP8 codes + row scales (bf16 only),
+ * computing exactly the bf16 GEMM over dq(Q).  Epilogue per output row orow = b*out_batch_rows + out_row_offset + m:
+ * act 1 exact GELU, act 2 SwiGLU over interleaved (gate, up) columns -> out_h[orow*ldo_h + n/2] (16-bit only); fp32
+ * out_f[orow*ldo_f + n] = v + resid (resid_mode 1: resid row orow, may be out_f itself; 2: resid row m, a table broadcast
+ * over the batch); 16-bit out_h[orow*ldo_h + n], or with head_major_rows R > 0 at
+ * ((orow/R * N/64 + n/64) * R + orow%R) * 64 + n%64.  dtype S2S_F16 / S2S_BF16 (A, W and out_h).  bn: the N tile,
+ * 0 = the library's rule, 64 or 128 to force one (128 needs N % 128 == 0).  S2S_ERR_INVALID, with nothing launched, on
+ * N % 64, K % 8 (K % 32 tiled), a row stride that is not a multiple of 8, operands not 16-byte aligned, FP8 without bf16,
+ * no output, a residual without out_f or with resid_mode outside {1, 2}, act 2 with out_f / head_major_rows or without
+ * out_h, head_major_rows without out_h, bn outside {0, 64, 128}.  Asynchronous on `stream`. */
+#define S2S_GEMM_W_ROW_MAJOR 0
+#define S2S_GEMM_W_TILED16 1
+#define S2S_GEMM_W_TILED_FP8 2
+typedef struct {
+  const void* a; int64_t a_row_stride, a_batch_stride;
+  const void* w; int64_t ldw;
+  int32_t w_layout;
+  int32_t M, N, K, batch;
+  const float* bias; int32_t act;
+  void* out_h; int64_t ldo_h;
+  float* out_f; int64_t ldo_f;
+  const float* resid; int64_t ld_resid; int32_t resid_mode;
+  int64_t out_batch_rows, out_row_offset;
+  int32_t head_major_rows;
+  int32_t dtype, bn;
+} s2s_gemm_args;
+int s2s_gemm_ex(s2s_ctx* ctx, const s2s_gemm_args* args, void* stream);
 /* The tiled weight layout the Llama-family engines store their projections in, which both the decode kernel and the
  * prefill GEMMs read: element (row 8t+g, k 32w+8j+e) of a row-major [N, K] matrix at ((t*K/32 + w)*32 + 4g + j)*8 + e.
  * format S2S_F16 / S2S_BF16: 16-bit elements; S2S_FP8_E4M3: one E4M3 code per element, Q = e4m3(W * 2^-e_n) with the
  * smallest integer e_n that keeps the row's largest magnitude <= 448, followed by the N fp32 row scales 2^e_n.
  * s2s_tiled_weight_bytes: the buffer size (0 for an invalid shape or format).  s2s_tile_weights: row-major w_d [N, K]
- * (bf16 for FP8) -> out_d; N a multiple of 8, K of 32.  s2s_gemm_tiled: s2s_gemm with that operand; FP8 needs bf16 A,
- * and computes exactly s2s_gemm(A, dq(Q)), dq(Q) = Q * 2^e_n.                                                       */
+ * (bf16 for FP8) -> out_d; N a multiple of 8, K of 32.  s2s_gemm_ex reads it with w_layout 1 / 2. */
 int64_t s2s_tiled_weight_bytes(int32_t N, int32_t K, int32_t format);
 int s2s_tile_weights(s2s_ctx* ctx, const void* w_d, int32_t N, int32_t K, int32_t format, void* out_d, void* stream);
-int s2s_gemm_tiled(s2s_ctx* ctx, const void* a_d, const void* wt_d, int32_t format, const float* bias_d, void* c_d, int32_t M,
-                   int32_t N, int32_t K, int32_t dtype, int32_t out_dtype, int32_t act, void* stream);
 /* O = softmax(Q K^T * scale [+causal]) V ; q/k/v/o row-major [T, heads*hd] slices with row strides
  * (elements); kv_heads <= heads (GQA).  hd in {64, 128}.                                     */
 int s2s_attention(s2s_ctx* ctx, const void* q_d, const void* k_d, const void* v_d, void* o_d, int32_t B,

@@ -20,7 +20,7 @@ EXPORTED = [
     "s2s_whisper_finalize", "s2s_whisper_logmel", "s2s_whisper_encode", "s2s_whisper_decode",
     "s2s_whisper_detect_language", "s2s_whisper_transcribe", "s2s_whisper_set_trace", "s2s_whisper_max_decode_batch",
     "s2s_whisper_create_shared", "s2s_whisper_device_bytes",
-    "s2s_gemm", "s2s_tiled_weight_bytes", "s2s_tile_weights", "s2s_gemm_tiled", "s2s_attention", "s2s_decode_attention", "s2s_decode_gemv",
+    "s2s_gemm_ex", "s2s_tiled_weight_bytes", "s2s_tile_weights", "s2s_attention", "s2s_decode_attention", "s2s_decode_gemv",
     "s2s_llama_create", "s2s_llama_destroy", "s2s_llama_bind_tensor", "s2s_llama_init_random",
     "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_set_sampling", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
     "s2s_llama_set_weight_format", "s2s_llama_weight_format", "s2s_llama_device_bytes", "s2s_llama_create_shared",
@@ -89,6 +89,23 @@ class ConvArgs(C.Structure):
         ("y", C.c_void_p), ("ldy", C.c_int64), ("T_out", C.c_int32),
         ("t0", C.c_int32),
         ("batch", C.c_int32), ("x_bs", C.c_int64), ("y_bs", C.c_int64), ("r_bs", C.c_int64),
+    ]
+
+
+class GemmArgs(C.Structure):
+    """s2s_gemm_args: one call of the prefill / encoder GEMM (s2s_gemm_ex)."""
+    _fields_ = [
+        ("a", C.c_void_p), ("a_row_stride", C.c_int64), ("a_batch_stride", C.c_int64),
+        ("w", C.c_void_p), ("ldw", C.c_int64),
+        ("w_layout", C.c_int32),
+        ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("batch", C.c_int32),
+        ("bias", C.c_void_p), ("act", C.c_int32),
+        ("out_h", C.c_void_p), ("ldo_h", C.c_int64),
+        ("out_f", C.c_void_p), ("ldo_f", C.c_int64),
+        ("resid", C.c_void_p), ("ld_resid", C.c_int64), ("resid_mode", C.c_int32),
+        ("out_batch_rows", C.c_int64), ("out_row_offset", C.c_int64),
+        ("head_major_rows", C.c_int32),
+        ("dtype", C.c_int32), ("bn", C.c_int32),
     ]
 
 
@@ -182,11 +199,10 @@ def load() -> C.CDLL:
     lib.s2s_whisper_set_trace.argtypes = [vp, vp, i32]
     lib.s2s_whisper_max_decode_batch.argtypes = [vp]
     lib.s2s_whisper_max_decode_batch.restype = i32
-    lib.s2s_gemm.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
+    lib.s2s_gemm_ex.argtypes = [vp, C.POINTER(GemmArgs), vp]
     lib.s2s_tiled_weight_bytes.argtypes = [i32, i32, i32]
     lib.s2s_tiled_weight_bytes.restype = i64
     lib.s2s_tile_weights.argtypes = [vp, vp, i32, i32, i32, vp, vp]
-    lib.s2s_gemm_tiled.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, vp]
     lib.s2s_attention.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i64, i64, i64, i64, f32, i32, i32, vp]
     lib.s2s_decode_attention.argtypes = [vp, C.POINTER(DecAttnArgs), C.POINTER(i32), vp]
     lib.s2s_decode_gemv.argtypes = [vp, C.POINTER(DecGemvArgs), C.POINTER(i32), vp]

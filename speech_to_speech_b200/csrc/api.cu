@@ -76,15 +76,18 @@ int s2s_destroy(s2s_ctx* ctx) {
   return S2S_OK;
 }
 
-int s2s_gemm(s2s_ctx* ctx, const void* a_d, const void* w_d, const float* bias_d, void* c_d, int32_t M, int32_t N,
-             int32_t K, int32_t dtype, int32_t out_dtype, int32_t act, void* stream) {
-  S2S_REQUIRE(ctx && a_d && w_d && c_d, "s2s_gemm: null argument");
+int s2s_gemm_ex(s2s_ctx* ctx, const s2s_gemm_args* g, void* stream) {
+  S2S_REQUIRE(ctx && g && g->a && g->w, "s2s_gemm_ex: null argument");
   GemmProblem p{};
-  p.a = a_d; p.a_row_stride = K; p.a_batch_stride = (int64_t)K * M; p.w = w_d; p.ldw = K;
-  p.M = M; p.N = N; p.K = K; p.batch = 1; p.bias = bias_d; p.act = act;
-  if (out_dtype == S2S_F32) { p.out_f = (float*)c_d; p.ldo_f = N; }
-  else { S2S_REQUIRE(out_dtype == dtype, "s2s_gemm: out_dtype must be f32 or the operand dtype"); p.out_h = c_d; p.ldo_h = N; }
-  return gemm_tc_launch(ctx, p, dtype, (cudaStream_t)stream);
+  p.a = g->a; p.a_row_stride = g->a_row_stride; p.a_batch_stride = g->a_batch_stride;
+  p.w = g->w; p.ldw = g->ldw; p.w_layout = g->w_layout;
+  p.M = g->M; p.N = g->N; p.K = g->K; p.batch = g->batch;
+  p.bias = g->bias; p.act = g->act;
+  p.out_h = g->out_h; p.ldo_h = g->ldo_h; p.out_f = g->out_f; p.ldo_f = g->ldo_f;
+  p.resid = g->resid; p.ld_resid = g->ld_resid; p.resid_mode = g->resid_mode;
+  p.out_batch_rows = g->out_batch_rows; p.out_row_offset = g->out_row_offset; p.head_major_rows = g->head_major_rows;
+  p.bn = g->bn;
+  return gemm_tc_launch(ctx, p, g->dtype, (cudaStream_t)stream);
 }
 
 int64_t s2s_tiled_weight_bytes(int32_t N, int32_t K, int32_t format) {
@@ -100,20 +103,6 @@ int s2s_tile_weights(s2s_ctx* ctx, const void* w_d, int32_t N, int32_t K, int32_
   S2S_REQUIRE((reinterpret_cast<uintptr_t>(w_d) & 15) == 0 && (reinterpret_cast<uintptr_t>(out_d) & 15) == 0,
               "s2s_tile_weights: buffers must be 16-byte aligned");
   return tile_rows_launch(w_d, N, K, out_d, N, 0, 1, format == S2S_FP8_E4M3, (cudaStream_t)stream);
-}
-
-int s2s_gemm_tiled(s2s_ctx* ctx, const void* a_d, const void* wt_d, int32_t format, const float* bias_d, void* c_d, int32_t M,
-                   int32_t N, int32_t K, int32_t dtype, int32_t out_dtype, int32_t act, void* stream) {
-  S2S_REQUIRE(ctx && a_d && wt_d && c_d, "s2s_gemm_tiled: null argument");
-  S2S_REQUIRE(format == dtype || (format == S2S_FP8_E4M3 && dtype == S2S_BF16),
-              "s2s_gemm_tiled: format %d must be the operand dtype, or FP8 with bf16 operands", format);
-  GemmProblem p{};
-  p.a = a_d; p.a_row_stride = K; p.a_batch_stride = (int64_t)K * M; p.w = wt_d;
-  p.w_layout = format == S2S_FP8_E4M3 ? GEMM_W_TILED_FP8 : GEMM_W_TILED16;
-  p.M = M; p.N = N; p.K = K; p.batch = 1; p.bias = bias_d; p.act = act;
-  if (out_dtype == S2S_F32) { p.out_f = (float*)c_d; p.ldo_f = N; }
-  else { S2S_REQUIRE(out_dtype == dtype, "s2s_gemm_tiled: out_dtype must be f32 or the operand dtype"); p.out_h = c_d; p.ldo_h = N; }
-  return gemm_tc_launch(ctx, p, dtype, (cudaStream_t)stream);
 }
 
 int s2s_attention(s2s_ctx* ctx, const void* q_d, const void* k_d, const void* v_d, void* o_d, int32_t B, int32_t Tq,

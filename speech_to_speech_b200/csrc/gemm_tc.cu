@@ -10,7 +10,7 @@
 // Warp roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = MMA + epilogue.
 //
 // The weight operand W comes in one of three layouts (GemmProblem::w_layout, a template parameter of the kernel):
-//   * row-major [N, ldw], 128-byte swizzle, as above (Whisper, the codec, s2s_gemm);
+//   * row-major [N, ldw], 128-byte swizzle, as above (Whisper, the codec, s2s_gemm_ex);
 //   * the fragment-major 16-bit tiles the decode kernels stream (weight_tiles.cu).  Each 32-k window of an 8-row tile is
 //     a contiguous 8 x 64 B block, so a 4-D TMA map {32 k, 8 rows, windows, tiles} with the 64-byte swizzle lands the
 //     k-block as [tile][window][8 rows][64 B] swizzle-64B atoms, which wgmma reads as a K-major operand (one 8-row group
@@ -322,9 +322,19 @@ int gemm_tc_launch(s2s_ctx* ctx, const GemmProblem& p, int dtype, cudaStream_t s
   S2S_REQUIRE((reinterpret_cast<uintptr_t>(p.a) & 15) == 0 && (reinterpret_cast<uintptr_t>(p.w) & 15) == 0,
               "gemm: operands must be 16-byte aligned");
   S2S_REQUIRE(p.M > 0 && p.batch > 0, "gemm: empty problem");
+  // epilogue combinations epilogue_pair would silently ignore
+  S2S_REQUIRE(p.out_h || p.out_f, "gemm: no output");
+  S2S_REQUIRE(p.act >= 0 && p.act <= 2, "gemm: unknown act %d", p.act);
+  S2S_REQUIRE(p.act != 2 || (p.out_h && !p.out_f && p.head_major_rows == 0),
+              "gemm: SwiGLU (act 2) writes a plain 16-bit out_h only");
+  S2S_REQUIRE(!p.resid || p.out_f, "gemm: a residual needs the fp32 output");
+  S2S_REQUIRE(!p.resid || p.resid_mode == 1 || p.resid_mode == 2, "gemm: resid_mode %d (1 or 2 with a residual)", p.resid_mode);
+  S2S_REQUIRE(p.head_major_rows >= 0 && (p.head_major_rows == 0 || p.out_h), "gemm: head_major_rows needs out_h");
+  S2S_REQUIRE(p.bn == 0 || p.bn == 64 || (p.bn == 128 && p.N % 128 == 0), "gemm: bn=%d (0, 64, or 128 with N %% 128 == 0; N=%d)",
+              p.bn, p.N);
   // Pick the N tile so the grid covers every SM when the problem allows it.
   const long long tiles128 = (long long)(p.N / 128) * ((p.M + BM - 1) / BM) * p.batch;
-  const bool use128 = (p.N % 128 == 0) && tiles128 >= ctx->num_sms;
+  const bool use128 = p.bn ? p.bn == 128 : (p.N % 128 == 0) && tiles128 >= ctx->num_sms;
   if (p.w_layout == GEMM_W_TILED_FP8) {
     return use128 ? launch_impl<__nv_bfloat16, 128, GEMM_W_TILED_FP8>(ctx, p, stream)
                   : launch_impl<__nv_bfloat16, 64, GEMM_W_TILED_FP8>(ctx, p, stream);

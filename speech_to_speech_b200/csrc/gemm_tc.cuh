@@ -33,6 +33,9 @@ struct GemmProblem {
   // layout of w: GEMM_W_ROW_MAJOR [N, ldw]; GEMM_W_TILED16 = weight_tiles.cu's fragment-major 16-bit tiles (ldw unused,
   // K a multiple of 32); GEMM_W_TILED_FP8 = E4M3 codes in that tiling followed by the fp32 row scales (bf16 only)
   int32_t w_layout;
+  // N tile: 0 = the launch's rule (128 when N % 128 == 0 and the 128-wide grid covers every SM, else 64); 64 or 128 forces
+  // that instantiation (128 needs N % 128 == 0).  The engines leave it 0; tests force both.
+  int32_t bn;
 };
 
 enum GemmWeightLayout { GEMM_W_ROW_MAJOR = 0, GEMM_W_TILED16 = 1, GEMM_W_TILED_FP8 = 2 };

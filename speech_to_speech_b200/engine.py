@@ -276,20 +276,54 @@ class WhisperEngine:
 
 
 # ---------------------------------------------------------------------------------------------
+GEMM_W_LAYOUTS = {"row_major": 0, "tiled": 1, "float8_e4m3": 2}
+GEMM_ACTS = {"none": 0, "gelu": 1, "swiglu": 2}
+
+
+def gemm_ex(a: torch.Tensor, w: torch.Tensor, M: int, N: int, K: int, *, dtype: Optional[torch.dtype] = None,
+            **fields: Any) -> None:
+    """One call of the prefill / encoder GEMM in any form the engines use (include/s2s_b200.h s2s_gemm_ex), written into
+    the caller's tensors.  `fields` maps the other s2s_gemm_args field names to values: cuda tensors are passed as their
+    device pointers (a view's pointer is its first element), `w_layout` and `act` may be names (GEMM_W_LAYOUTS,
+    GEMM_ACTS).  Defaults: a_row_stride = ldw = K, a_batch_stride = M * a_row_stride, batch 1, dtype = a's 16-bit type
+    (a uint8 view of the operand needs dtype).  Asynchronous on the current stream."""
+    assert a.is_cuda and w.is_cuda
+    g = _lib.GemmArgs()
+    g.a, g.w, g.M, g.N, g.K = a.data_ptr(), w.data_ptr(), M, N, K
+    g.a_row_stride, g.ldw, g.batch = K, K, 1
+    for k, v in fields.items():
+        if isinstance(v, torch.Tensor):
+            assert v.is_cuda, k
+            v = v.data_ptr()
+        elif k == "w_layout" and isinstance(v, str):
+            v = GEMM_W_LAYOUTS[v]
+        elif k == "act" and isinstance(v, str):
+            v = GEMM_ACTS[v]
+        elif v is None:
+            v = 0
+        setattr(g, k, v)
+    if "a_batch_stride" not in fields:
+        g.a_batch_stride = M * g.a_row_stride
+    g.dtype = {torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[dtype or a.dtype]
+    dev = a.device.index or 0
+    check(_lib.load().s2s_gemm_ex(get_context(dev), C.byref(g), _stream_ptr(dev)), "s2s_gemm_ex")
+
+
+def _gemm_out(M: int, N: int, a: torch.Tensor, out_dtype: Optional[torch.dtype]) -> tuple[torch.Tensor, dict]:
+    out_dtype = out_dtype or a.dtype
+    assert out_dtype in (torch.float32, a.dtype), "out_dtype must be float32 or the operand dtype"
+    c = torch.empty((M, N), dtype=out_dtype, device=a.device)
+    return c, (dict(out_f=c, ldo_f=N) if out_dtype == torch.float32 else dict(out_h=c, ldo_h=N))
+
+
 def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, act: str = "none",
          out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
     """C = A @ W^T (+bias) through the wgmma kernel; a [M,K], w [N,K] fp16/bf16 cuda tensors."""
     assert a.is_cuda and w.is_cuda and a.dtype == w.dtype and a.is_contiguous() and w.is_contiguous()
-    dev = a.device.index or 0
     M, K = a.shape
     N = w.shape[0]
-    code = {torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[a.dtype]
-    out_dtype = out_dtype or a.dtype
-    ocode = S2S_F32 if out_dtype == torch.float32 else code
-    c = torch.empty((M, N), dtype=out_dtype, device=a.device)
-    lib = _lib.load()
-    check(lib.s2s_gemm(get_context(dev), _ptr(a), _ptr(w), _ptr(bias), _ptr(c), M, N, K, code, ocode,
-                       1 if act == "gelu" else 0, _stream_ptr(dev)), "s2s_gemm")
+    c, out = _gemm_out(M, N, a, out_dtype)
+    gemm_ex(a, w, M, N, K, bias=bias, act=act, **out)
     return c
 
 
@@ -315,17 +349,11 @@ def gemm_tiled(a: torch.Tensor, wt: torch.Tensor, N: int, weight_dtype: Optional
     """gemm() with the weight operand in the tiled layout of tile_weights(): a [M, K] fp16/bf16 cuda, wt from
     tile_weights(w [N, K], weight_dtype).  FP8 computes exactly gemm(a, dq(q(w)))."""
     assert a.is_cuda and wt.is_cuda and a.is_contiguous() and wt.is_contiguous()
-    dev = a.device.index or 0
     M, K = a.shape
-    code = {torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[a.dtype]
-    fmt = _lib.WEIGHT_FORMAT_CODES[weight_dtype] if weight_dtype else code
-    lib = _lib.load()
-    assert wt.numel() * wt.element_size() >= int(lib.s2s_tiled_weight_bytes(N, K, fmt)), "wt is smaller than the tiled [N, K] matrix"
-    out_dtype = out_dtype or a.dtype
-    ocode = S2S_F32 if out_dtype == torch.float32 else code
-    c = torch.empty((M, N), dtype=out_dtype, device=a.device)
-    check(lib.s2s_gemm_tiled(get_context(dev), _ptr(a), _ptr(wt), fmt, _ptr(bias), _ptr(c), M, N, K, code, ocode,
-                             1 if act == "gelu" else 0, _stream_ptr(dev)), "s2s_gemm_tiled")
+    fmt = _lib.WEIGHT_FORMAT_CODES[weight_dtype] if weight_dtype else {torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[a.dtype]
+    assert wt.numel() * wt.element_size() >= int(_lib.load().s2s_tiled_weight_bytes(N, K, fmt)), "wt is smaller than the tiled [N, K] matrix"
+    c, out = _gemm_out(M, N, a, out_dtype)
+    gemm_ex(a, wt, M, N, K, w_layout=weight_dtype or "tiled", bias=bias, act=act, **out)
     return c
 
 

@@ -42,28 +42,6 @@ def _opts(E, G, max_new=None):
                                   begin_suppress=G["begin_suppress"].tolist())
 
 
-# ------------------------------------------------------------------------------------------ kernels
-@pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
-@pytest.mark.parametrize("shape", [(128, 64, 64), (1500, 768, 768), (200, 64, 240), (3000, 2304, 768), (333, 512, 3072),
-                                   (1, 128, 8), (129, 192, 72)])
-def test_gemm_tcgen05_matches_fp32_matmul(E, dt, shape):
-    """The tensor-core GEMM (csrc/gemm_tc.cu, wgmma on sm_90a) against an fp32 matmul."""
-    M, N, K = shape
-    gen = torch.Generator(device="cuda").manual_seed(M * 7 + N)
-    a = (torch.randn(M, K, device="cuda", generator=gen) * 0.5).to(dt)
-    w = (torch.randn(N, K, device="cuda", generator=gen) * 0.05).to(dt)
-    bias = torch.randn(N, device="cuda", generator=gen) * 0.1
-    ref = a.float() @ w.float().T + bias
-    out = E.gemm(a, w, bias, out_dtype=torch.float32)
-    assert (out - ref).abs().max().item() < 1e-4 * max(1.0, K / 256)
-    out_h = E.gemm(a, w, bias, act="gelu")
-    ref_h = torch.nn.functional.gelu(ref)
-    tol = 2e-3 if dt == torch.float16 else 2e-2
-    assert (out_h.float() - ref_h).abs().max().item() < tol
-    out_nb = E.gemm(a, w, None, out_dtype=torch.float32)
-    assert (out_nb - (ref - bias)).abs().max().item() < 1e-4 * max(1.0, K / 256)
-
-
 # ------------------------------------------------------------------------------------------ log-mel
 @pytest.mark.parametrize("seed,n", [(0, 160000), (2, 480000), (3, 12345), (4, 500000), (5, 0), (6, 200), (7, 479999)])
 def test_logmel_matches_oracle(E, seed, n):
