@@ -201,16 +201,29 @@ int s2s_attention(s2s_ctx* ctx, const void* q_d, const void* k_d, const void* v_
  * grid 0 = the context's decode grid (s2s_set_sm_partition); assoc_b 0 = B, else the batch whose plan fixes the split
  * plan (the decode launch uses 8 at 13 to 16 Llama-3-8B sessions).  *plan_out_h (may be NULL) = the plan: key splits per
  * (session, head) in bits 0-6, bit 7 set for warp-level items.  Split records and counters are allocated per call, and a
- * counter the merge left non-zero is an error.  Synchronous: returns after the stream has finished. */
+ * counter the merge left non-zero is an error.  Synchronous: returns after the stream has finished.
+ * Qwen3 mode (qk_norm = 1), the attention phase of the Qwen3 / Qwen3-TTS decode: q is the RAW q row, the cache holds keys
+ * [0, len - 1) and kraw[b] the raw key of the step.  At the head of every item the kernel's ld_qk_prepare normalises
+ * (RMSNorm over hd with q_norm / k_norm and eps, fp32 statistics), rotates (rope [max_pos][hd / 2] fp32 (cos, sin) at
+ * position len - 1) and scales (1 / sqrt(hd)) q; the item whose key split holds key len - 1 normalises and rotates kraw and
+ * writes it to cache row len - 1 first.  q_norm / k_norm are stored pair-adjacent like the q / k rows (the model's layout).
+ * qn_out (may be NULL): the normalised, rotated, scaled q [B][heads][hd].  Pointers 16-byte aligned. */
 typedef struct {
-  const float* q;        /* [B][heads][hd] fp32, softmax scale applied */
-  const void* kv;        /* 16-bit (dtype), [slots][2][max_pos][kv_heads * hd] */
+  const float* q;        /* [B][heads][hd] fp32, softmax scale applied (qk_norm: raw) */
+  void* kv;              /* 16-bit (dtype), [slots][2][max_pos][kv_heads * hd]; qk_norm: K row len - 1 is written */
   int32_t max_pos;
   const int32_t* slots_h; const int32_t* lens_h; int32_t B;   /* lens_h[b] in [1, max_pos]; B in [1, 16] */
   int32_t heads, kv_heads, hd, dtype;                         /* hd 64 or 128; dtype S2S_F16 or S2S_BF16 */
   int32_t grid;          /* CTAs; 0 = the context's decode grid */
   int32_t assoc_b;       /* 0 = B */
   void* out;             /* [B][heads][hd] 16-bit */
+  int32_t qk_norm;       /* 0: q is final (the fields below are ignored); 1: Qwen3 mode */
+  const float* kraw;     /* [B][kv_heads][hd] fp32 raw keys of the step */
+  const float* q_norm;   /* [hd] */
+  const float* k_norm;   /* [hd] */
+  const float* rope;     /* [max_pos][hd / 2] (cos, sin) pairs */
+  float eps;
+  float* qn_out;         /* [B][heads][hd] fp32 or NULL */
 } s2s_dec_attn_args;
 int s2s_decode_attention(s2s_ctx* ctx, const s2s_dec_attn_args* args, int32_t* plan_out_h, void* stream);
 /* The skinny GEMM of the persistent decode kernels by itself (exposed for tests): the production device functions
@@ -270,6 +283,31 @@ typedef struct {
   int32_t cluster, heads;                   /* virtual clusters: 0 = whole-grid plans only */
 } s2s_dec_gemv_args;
 int s2s_decode_gemv(s2s_ctx* ctx, const s2s_dec_gemv_args* args, int32_t* plans_out_h, void* stream);
+/* The prefill / encoder row norm by itself (exposed for tests): the launch every Whisper encoder layer and every
+ * Llama-family prefill layer runs.  For each of `rows` fp32 rows x[r][0..d), two-pass fp32 statistics:
+ *   bias != NULL: LayerNorm   y = (x - mean) / sqrt(var + eps) * w + bias
+ *   bias == NULL: RMSNorm     y = x / sqrt(mean(x^2) + eps) * w
+ * -> out_h [rows][d] 16-bit (dtype) and / or out_f [rows][d] fp32.  S2S_ERR_INVALID, with nothing launched, on d % 4 != 0,
+ * rows < 1, no output, x / w / bias / out_f not 16-byte aligned, out_h not 8-byte aligned, dtype not S2S_F16 / S2S_BF16.
+ * Asynchronous on `stream`. */
+int s2s_norm_rows(s2s_ctx* ctx, const float* x, const float* w, const float* bias, float eps, int64_t rows, int32_t d,
+                  void* out_h, float* out_f, int32_t dtype, void* stream);
+/* The RoPE / KV-append step of a Llama-family prefill layer by itself (exposed for tests): the launch the prefill runs for
+ * each segment.  qkv: n 16-bit rows [heads * hd | kv_heads * hd | kv_heads * hd] (q, k, v; q and k rows and q_norm / k_norm
+ * stored pair-adjacent, element 2j, 2j + 1 of a head = rotate_half partners j, j + hd / 2).  Token t sits at position past + t:
+ * with q_norm == k_norm == NULL (Llama) q and k are rotated with rope[past + t] ((cos, sin) fp32 pairs [max_pos][hd / 2]);
+ * with both given (Qwen3) each q / k head is first RMS-normalised over hd (fp32 statistics, eps).  q is rewritten in place,
+ * the rotated k row goes to kcache[past + t] and the v row to vcache[past + t] (caches [max_pos][kv_heads * hd]); the k and v
+ * columns of qkv are left as they were.  S2S_ERR_INVALID, with nothing launched, on hd not 64 / 128, n < 1, past < 0,
+ * past + n > max_pos, heads % kv_heads, one norm weight without the other, pointers not 16-byte aligned, dtype not
+ * S2S_F16 / S2S_BF16.  Asynchronous on `stream`. */
+int s2s_prefill_rope(s2s_ctx* ctx, void* qkv, int32_t n, int32_t heads, int32_t kv_heads, int32_t hd, int32_t past,
+                     const float* rope, int32_t max_pos, const float* q_norm, const float* k_norm, float eps, void* kcache,
+                     void* vcache, int32_t dtype, void* stream);
+/* The greedy token choice after a prefill by itself (exposed for tests): *out_d = the argmax of logits_d[0..n), the lowest
+ * id among equal maxima; NaN entries count as -inf, so a row without a number above -inf gives 0.  S2S_ERR_INVALID on
+ * n < 1 or a null pointer.  Asynchronous on `stream`. */
+int s2s_argmax_row(s2s_ctx* ctx, const float* logits_d, int32_t n, int32_t* out_d, void* stream);
 
 /* ---- Llama-family LLM ------------------------------------------------------------------ */
 typedef struct {

@@ -21,6 +21,7 @@ EXPORTED = [
     "s2s_whisper_detect_language", "s2s_whisper_transcribe", "s2s_whisper_set_trace", "s2s_whisper_max_decode_batch",
     "s2s_whisper_create_shared", "s2s_whisper_device_bytes",
     "s2s_gemm_ex", "s2s_tiled_weight_bytes", "s2s_tile_weights", "s2s_attention", "s2s_decode_attention", "s2s_decode_gemv",
+    "s2s_norm_rows", "s2s_prefill_rope", "s2s_argmax_row",
     "s2s_llama_create", "s2s_llama_destroy", "s2s_llama_bind_tensor", "s2s_llama_init_random",
     "s2s_llama_finalize", "s2s_llama_session_reset", "s2s_llama_set_sampling", "s2s_llama_prefill", "s2s_llama_prefill_batch", "s2s_llama_decode", "s2s_llama_generate", "s2s_llama_set_trace", "s2s_llama_max_decode_batch",
     "s2s_llama_set_weight_format", "s2s_llama_weight_format", "s2s_llama_device_bytes", "s2s_llama_create_shared",
@@ -116,6 +117,8 @@ class DecAttnArgs(C.Structure):
         ("slots_h", C.POINTER(C.c_int32)), ("lens_h", C.POINTER(C.c_int32)), ("B", C.c_int32),
         ("heads", C.c_int32), ("kv_heads", C.c_int32), ("hd", C.c_int32), ("dtype", C.c_int32),
         ("grid", C.c_int32), ("assoc_b", C.c_int32), ("out", C.c_void_p),
+        ("qk_norm", C.c_int32), ("kraw", C.c_void_p), ("q_norm", C.c_void_p), ("k_norm", C.c_void_p), ("rope", C.c_void_p),
+        ("eps", C.c_float), ("qn_out", C.c_void_p),
     ]
 
 
@@ -206,6 +209,9 @@ def load() -> C.CDLL:
     lib.s2s_attention.argtypes = [vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, i64, i64, i64, i64, f32, i32, i32, vp]
     lib.s2s_decode_attention.argtypes = [vp, C.POINTER(DecAttnArgs), C.POINTER(i32), vp]
     lib.s2s_decode_gemv.argtypes = [vp, C.POINTER(DecGemvArgs), C.POINTER(i32), vp]
+    lib.s2s_norm_rows.argtypes = [vp, vp, vp, vp, f32, i64, i32, vp, vp, i32, vp]
+    lib.s2s_prefill_rope.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, f32, vp, vp, i32, vp]
+    lib.s2s_argmax_row.argtypes = [vp, vp, i32, vp, vp]
     lib.s2s_llama_create.argtypes = [vp, C.POINTER(LlamaConfig), C.POINTER(vp)]
     lib.s2s_llama_destroy.argtypes = [vp]
     lib.s2s_llama_bind_tensor.argtypes = [vp, C.c_char_p, vp, C.POINTER(i64), i32, i32]

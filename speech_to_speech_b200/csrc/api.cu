@@ -90,6 +90,18 @@ int s2s_gemm_ex(s2s_ctx* ctx, const s2s_gemm_args* g, void* stream) {
   return gemm_tc_launch(ctx, p, g->dtype, (cudaStream_t)stream);
 }
 
+int s2s_norm_rows(s2s_ctx* ctx, const float* x, const float* w, const float* bias, float eps, int64_t rows, int32_t d,
+                  void* out_h, float* out_f, int32_t dtype, void* stream) {
+  auto al = [](const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; };
+  S2S_REQUIRE(ctx && x && w, "s2s_norm_rows: null argument");
+  S2S_REQUIRE(out_h || out_f, "s2s_norm_rows: no output");
+  S2S_REQUIRE(rows >= 1 && d >= 4 && d % 4 == 0, "s2s_norm_rows: rows %lld, d %d (a multiple of 4)", (long long)rows, d);
+  S2S_REQUIRE(dtype == S2S_F16 || dtype == S2S_BF16, "s2s_norm_rows: dtype %d", dtype);
+  S2S_REQUIRE(al(x, 16) && al(w, 16) && al(bias, 16) && al(out_f, 16) && al(out_h, 8),
+              "s2s_norm_rows: x / w / bias / out_f must be 16-byte aligned, out_h 8-byte aligned");
+  return norm_rows_launch(x, w, bias, eps, rows, d, out_h, out_f, dtype, (cudaStream_t)stream);
+}
+
 int64_t s2s_tiled_weight_bytes(int32_t N, int32_t K, int32_t format) {
   if (N < 1 || K < 32 || K % 32 != 0) return 0;
   if (format == S2S_FP8_E4M3) return (int64_t)tiled_fp8_weight_bytes(N, K);

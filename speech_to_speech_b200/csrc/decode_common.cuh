@@ -1047,10 +1047,11 @@ __device__ __forceinline__ void gemv_argmax_candidates(float (&best_v)[2], int (
 }
 
 // ---- token choice of the select phase (one warp per session) ----------------------------------------------------
-// the argmax over the grid's per-CTA candidates of session b (the lowest id on ties), in every lane
+// the argmax over the grid's per-CTA candidates of session b (the lowest id on ties), in every lane.  NaN never compares
+// greater, so it counts as -inf; starting from (-inf, id 0) makes a row with nothing above -inf give id 0, a valid id.
 __device__ __forceinline__ int dec_argmax_merge(const float* cand_val, const int* cand_idx, int b) {
   const int lane = threadIdx.x & 31;
-  float bv = -INFINITY; int bi = 0x7fffffff;
+  float bv = -INFINITY; int bi = 0;
 #pragma unroll 1
   for (int c = lane; c < (int)gridDim.x; c += 32) {
     const float v = __ldcg(cand_val + b * gridDim.x + c); const int i = __ldcg(cand_idx + b * gridDim.x + c);

@@ -85,10 +85,12 @@ __global__ void qknorm_rope_prefill_kernel(T* __restrict__ qkv, int H, int KV, i
     *reinterpret_cast<uint32_t*>(vcache + (long long)(past + t) * kvd + i) = *reinterpret_cast<const uint32_t*>(row + qd + kvd + i);
 }
 
+// the lowest id among the maxima; NaN never compares greater, so it counts as -inf: starting from (-inf, id 0) makes a row with
+// nothing above -inf (all -inf and / or NaN) give id 0, a valid id, instead of the start value
 __global__ void argmax_row_kernel(const float* __restrict__ logits, int n, int* __restrict__ out) {
   __shared__ float sv[32];
   __shared__ int si[32];
-  float bv = -INFINITY; int bi = 0x7fffffff;
+  float bv = -INFINITY; int bi = 0;
   for (int i = threadIdx.x; i < n; i += blockDim.x) {
     const float v = logits[i];
     if (v > bv || (v == bv && i < bi)) { bv = v; bi = i; }
@@ -344,6 +346,28 @@ static int prefill_choose(s2s_llama* m, int slot, const float* row, int pred_pos
   return S2S_OK;
 }
 
+// RoPE / Qwen3 q/k norm + RoPE and the K/V append of one prefill segment: n rows of qkv at positions [past, past + n).
+// q_norm == nullptr: Llama (rope_prefill_kernel), else Qwen3 (qknorm_rope_prefill_kernel).  prefill_layers and
+// s2s_prefill_rope both launch through here.
+static int prefill_rope_launch(void* qkv, int n, int heads, int kv_heads, int hd, int past, const float2* rope, const float* q_norm,
+                               const float* k_norm, float eps, void* kc, void* vc, int dt, cudaStream_t st) {
+  const bool bf = dt == S2S_BF16;
+  if (q_norm) {
+#define S2S_QKN(T, HD) qknorm_rope_prefill_kernel<T, HD><<<n, 256, 0, st>>>((T*)qkv, heads, kv_heads, past, rope, q_norm, k_norm, \
+                                                                             eps, (T*)kc, (T*)vc)
+    if (bf) { if (hd == 128) S2S_QKN(__nv_bfloat16, 128); else S2S_QKN(__nv_bfloat16, 64); }
+    else { if (hd == 128) S2S_QKN(__half, 128); else S2S_QKN(__half, 64); }
+#undef S2S_QKN
+  } else {
+    const int qd = heads * hd, kvd = kv_heads * hd;
+    if (bf) rope_prefill_kernel<__nv_bfloat16><<<n, 256, 0, st>>>((__nv_bfloat16*)qkv, n, qd, kvd, hd, past, rope, (__nv_bfloat16*)kc,
+                                                                  (__nv_bfloat16*)vc);
+    else rope_prefill_kernel<__half><<<n, 256, 0, st>>>((__half*)qkv, n, qd, kvd, hd, past, rope, (__half*)kc, (__half*)vc);
+  }
+  S2S_LAUNCH_CHECK();
+  return S2S_OK;
+}
+
 // One pass of all decoder layers over R = sum of the segments' rows, already embedded in m->x.  A segment is the new rows of
 // one session (rows [off, off + n) of the buffers, positions [past, past + n) of its KV slot): the projections and the MLP
 // run over all R rows at once -- ONE pass over the weights for every session of a batched prefill -- while RoPE / cache
@@ -354,7 +378,6 @@ static int prefill_layers(s2s_llama* m, const PrefillSeg* segs, int nseg, int R,
   const auto& c = m->cfg;
   const int d = c.d_model, f = c.ffn, hd = c.head_dim, qd = c.heads * hd, kvd = c.kv_heads * hd, dt = c.compute_dtype;
   const int ldq = qd + 2 * kvd;
-  const bool bf = dt == S2S_BF16;
   const size_t esz = 2;
   for (int i = 0; i < c.layers; ++i) {
     const LlamaDecLayer& L = m->layers_h[i];
@@ -370,19 +393,8 @@ static int prefill_layers(s2s_llama* m, const PrefillSeg* segs, int nseg, int R,
       char* vc = kc + (size_t)m->kv_which_stride * esz;
       char* qrow = reinterpret_cast<char*>(m->qkv) + (size_t)sg.off * ldq * esz;
       const int n = sg.n, past = sg.past;
-      if (c.qk_norm) {
-#define S2S_QKN(T, HD) qknorm_rope_prefill_kernel<T, HD><<<n, 256, 0, st>>>((T*)qrow, c.heads, c.kv_heads, past, m->rope, \
-                                                                             L.q_norm, L.k_norm, c.rms_eps, (T*)kc, (T*)vc)
-        if (bf) { if (hd == 128) S2S_QKN(__nv_bfloat16, 128); else S2S_QKN(__nv_bfloat16, 64); }
-        else { if (hd == 128) S2S_QKN(__half, 128); else S2S_QKN(__half, 64); }
-#undef S2S_QKN
-      } else if (bf) {
-        rope_prefill_kernel<__nv_bfloat16><<<n, 256, 0, st>>>((__nv_bfloat16*)qrow, n, qd, kvd, hd, past, m->rope,
-                                                              (__nv_bfloat16*)kc, (__nv_bfloat16*)vc);
-      } else {
-        rope_prefill_kernel<__half><<<n, 256, 0, st>>>((__half*)qrow, n, qd, kvd, hd, past, m->rope, (__half*)kc, (__half*)vc);
-      }
-      S2S_LAUNCH_CHECK();
+      S2S_CHECK(prefill_rope_launch(qrow, n, c.heads, c.kv_heads, hd, past, m->rope, c.qk_norm ? L.q_norm : nullptr,
+                                    c.qk_norm ? L.k_norm : nullptr, c.rms_eps, kc, vc, dt, st));
       S2S_CHECK(attention_tc_launch(m->ctx, qrow, kc, vc, reinterpret_cast<char*>(m->attn) + (size_t)sg.off * qd * esz, 1, n, past + n,
                                      c.heads, c.kv_heads, hd, ldq, kvd, kvd, qd, 1.0f / sqrtf((float)hd), 1, dt, m->vt, m->vt_elems, st));
     }
@@ -752,6 +764,29 @@ int s2s_llama_generate(s2s_llama* m, int32_t slot, const int32_t* prompt_h, int3
   } else {
     *len_out_h = 1 + n_dec;
   }
+  return S2S_OK;
+}
+
+int s2s_prefill_rope(s2s_ctx* ctx, void* qkv, int32_t n, int32_t heads, int32_t kv_heads, int32_t hd, int32_t past,
+                     const float* rope, int32_t max_pos, const float* q_norm, const float* k_norm, float eps, void* kcache,
+                     void* vcache, int32_t dtype, void* stream) {
+  auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  S2S_REQUIRE(ctx && qkv && rope && kcache && vcache, "s2s_prefill_rope: null argument");
+  S2S_REQUIRE(hd == 64 || hd == 128, "s2s_prefill_rope: hd %d (64 or 128)", hd);
+  S2S_REQUIRE(heads >= 1 && kv_heads >= 1 && heads % kv_heads == 0, "s2s_prefill_rope: heads %d / kv_heads %d", heads, kv_heads);
+  S2S_REQUIRE(n >= 1 && past >= 0 && (int64_t)past + n <= max_pos, "s2s_prefill_rope: rows [%d, %d + %d) outside [0, max_pos %d)",
+              past, past, n, max_pos);
+  S2S_REQUIRE(!q_norm == !k_norm, "s2s_prefill_rope: q_norm and k_norm go together (both: Qwen3, neither: Llama)");
+  S2S_REQUIRE(dtype == S2S_F16 || dtype == S2S_BF16, "s2s_prefill_rope: dtype %d", dtype);
+  S2S_REQUIRE(al(qkv) && al(rope) && al(q_norm) && al(k_norm) && al(kcache) && al(vcache), "s2s_prefill_rope: pointers must be 16-byte aligned");
+  return prefill_rope_launch(qkv, n, heads, kv_heads, hd, past, reinterpret_cast<const float2*>(rope), q_norm, k_norm, eps, kcache,
+                             vcache, dtype, (cudaStream_t)stream);
+}
+
+int s2s_argmax_row(s2s_ctx* ctx, const float* logits_d, int32_t n, int32_t* out_d, void* stream) {
+  S2S_REQUIRE(ctx && logits_d && out_d && n >= 1, "s2s_argmax_row: null argument or n %d < 1", n);
+  argmax_row_kernel<<<1, 1024, 0, (cudaStream_t)stream>>>(logits_d, n, out_d);   // as prefill_choose launches it
+  S2S_LAUNCH_CHECK();
   return S2S_OK;
 }
 

@@ -383,8 +383,14 @@ extern "C" int s2s_decode_attention(s2s_ctx* ctx, const s2s_dec_attn_args* args,
   S2S_REQUIRE(a.dtype == S2S_F16 || a.dtype == S2S_BF16, "s2s_decode_attention: dtype %d", a.dtype);
   S2S_REQUIRE(a.max_pos >= 1 && a.grid >= 0 && a.assoc_b >= 0 && a.assoc_b <= DEC_MAX_B,
               "s2s_decode_attention: max_pos %d / grid %d / assoc_b %d", a.max_pos, a.grid, a.assoc_b);
-  S2S_REQUIRE((reinterpret_cast<uintptr_t>(a.q) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.kv) & 15) == 0,
-              "s2s_decode_attention: q / kv must be 16-byte aligned");
+  auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  S2S_REQUIRE(al(a.q) && al(a.kv), "s2s_decode_attention: q / kv must be 16-byte aligned");
+  S2S_REQUIRE(a.qk_norm == 0 || a.qk_norm == 1, "s2s_decode_attention: qk_norm %d", a.qk_norm);
+  if (a.qk_norm) {
+    S2S_REQUIRE(a.kraw && a.q_norm && a.k_norm && a.rope, "s2s_decode_attention: qk_norm needs kraw / q_norm / k_norm / rope");
+    S2S_REQUIRE(al(a.kraw) && al(a.q_norm) && al(a.k_norm) && al(a.rope) && al(a.qn_out),
+                "s2s_decode_attention: kraw / q_norm / k_norm / rope / qn_out must be 16-byte aligned");
+  }
   int host[2 * DEC_MAX_B] = {}, max_len = 0;   // slots, then positions (len - 1)
   for (int b = 0; b < a.B; ++b) {
     S2S_REQUIRE(a.slots_h[b] >= 0 && a.lens_h[b] >= 1 && a.lens_h[b] <= a.max_pos,
@@ -399,23 +405,35 @@ extern "C" int s2s_decode_attention(s2s_ctx* ctx, const s2s_dec_attn_args* args,
   const int kvd = a.kv_heads * a.hd, BH = a.B * a.heads;
   LlamaDecParams p{};
   p.heads = a.heads; p.kv_heads = a.kv_heads; p.hd = a.hd; p.B = a.B; p.max_pos = a.max_pos; p.layers = 1;
-  p.q = const_cast<float*>(a.q); p.kv = const_cast<void*>(a.kv); p.attn16 = a.out;
+  p.q = const_cast<float*>(a.q); p.kv = a.kv; p.attn16 = a.out;
   p.kv_which_stride = (long long)a.max_pos * kvd; p.kv_layer_stride = 2 * p.kv_which_stride; p.kv_slot_stride = p.kv_layer_stride;
   p.s_max = (a.max_pos + 63) / 64;   // as llama_create sizes the records
   p.max_len = max_len; p.assoc_b = a.assoc_b > 0 ? a.assoc_b : a.B;
   if (plan_out_h) *plan_out_h = attn_plan(p.assoc_b * a.heads, (max_len + ATT_BLK - 1) / ATT_BLK, p.s_max, grid);
-  // per-call scratch: split records, split counters (zeroed), slots and positions
+  // per-call scratch: split records, split counters (zeroed), slots and positions; Qwen3: the one-layer weight table and,
+  // without qn_out, the normalised q
   const size_t part_bytes = (size_t)BH * p.s_max * (a.hd + PART_PAD) * 4;
+  const size_t idx_off = part_bytes + (size_t)BH * 4, layer_off = (idx_off + sizeof(host) + 15) / 16 * 16;
+  const size_t qn_off = layer_off + (sizeof(LlamaDecLayer) + 15) / 16 * 16;
+  const size_t scratch_bytes = a.qk_norm ? qn_off + (a.qn_out ? 0 : (size_t)BH * a.hd * 4) : idx_off + sizeof(host);
   char* scratch = nullptr;
-  S2S_CHECK_CUDA(cudaMalloc(&scratch, part_bytes + (size_t)BH * 4 + sizeof(host)));
+  S2S_CHECK_CUDA(cudaMalloc(&scratch, scratch_bytes));
   p.part = reinterpret_cast<float*>(scratch);
   p.attn_cnt = reinterpret_cast<unsigned int*>(scratch + part_bytes);
-  int* idx_d = reinterpret_cast<int*>(scratch + part_bytes + (size_t)BH * 4);
+  int* idx_d = reinterpret_cast<int*>(scratch + idx_off);
   p.slot = idx_d; p.pos = idx_d + DEC_MAX_B;
+  LlamaDecLayer layer{};
+  if (a.qk_norm) {   // ld_attn's Qwen3 path reads the norm weights from layer 0 of the model's table
+    layer.q_norm = a.q_norm; layer.k_norm = a.k_norm;
+    p.lw = reinterpret_cast<const LlamaDecLayer*>(scratch + layer_off);
+    p.qk_norm = 1; p.kraw = const_cast<float*>(a.kraw); p.rope = reinterpret_cast<const float2*>(a.rope); p.eps = a.eps;
+    p.qn = a.qn_out ? a.qn_out : reinterpret_cast<float*>(scratch + qn_off);
+  }
   std::vector<unsigned int> cnt((size_t)BH, 0u);
   auto run = [&]() -> int {
     S2S_CHECK_CUDA(cudaMemsetAsync(p.attn_cnt, 0, (size_t)BH * 4, st));
     S2S_CHECK_CUDA(cudaMemcpyAsync(idx_d, host, sizeof(host), cudaMemcpyHostToDevice, st));
+    if (a.qk_norm) S2S_CHECK_CUDA(cudaMemcpyAsync(scratch + layer_off, &layer, sizeof(layer), cudaMemcpyHostToDevice, st));
     const size_t smem = (size_t)DEC_WARPS * (a.hd + PART_PAD) * 4;
     if (a.dtype == S2S_F16) {
       if (a.hd == 128) ld_attn_only_kernel<__half, 128><<<grid, DEC_THREADS, smem, st>>>(p);

@@ -377,11 +377,16 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, heads: int, kv_
 
 
 def decode_attention(q: torch.Tensor, kv: torch.Tensor, slots: Sequence[int], lens: Sequence[int], heads: int, kv_heads: int,
-                     *, grid: int = 0, assoc_b: int = 0) -> tuple[torch.Tensor, int]:
+                     *, grid: int = 0, assoc_b: int = 0, kraw: Optional[torch.Tensor] = None, q_norm: Optional[torch.Tensor] = None,
+                     k_norm: Optional[torch.Tensor] = None, rope: Optional[torch.Tensor] = None, eps: float = 1e-6,
+                     qn_out: Optional[torch.Tensor] = None) -> tuple[torch.Tensor, int]:
     """One attention phase of the Llama-family decode by itself (include/s2s_b200.h s2s_decode_attention).  q: cuda f32
     [B, heads, hd], softmax scale applied; kv: 16-bit [slots, 2, max_pos, kv_heads * hd] (K rows, then V rows, per slot);
     session b attends the first lens[b] keys of slot slots[b].  -> (out [B, heads, hd] in kv's dtype, the split plan:
-    splits | 0x80 for warp-level items).  Synchronous."""
+    splits | 0x80 for warp-level items).  Synchronous.
+    Qwen3 mode (kraw given): q is the raw q, kraw f32 [B, kv_heads, hd] the step's raw keys, q_norm / k_norm f32 [hd]
+    (pair-adjacent), rope f32 [max_pos, hd / 2, 2] (cos, sin); the kernel normalises, rotates and scales q (into qn_out
+    [B, heads, hd] when given) and writes key lens[b] - 1 of every session into kv before it attends."""
     assert q.is_cuda and q.dtype == torch.float32 and q.dim() == 3 and q.is_contiguous()
     assert kv.is_cuda and kv.dtype in (torch.float16, torch.bfloat16) and kv.dim() == 4 and kv.shape[1] == 2 and kv.is_contiguous()
     B, H, hd = q.shape
@@ -392,11 +397,60 @@ def decode_attention(q: torch.Tensor, kv: torch.Tensor, slots: Sequence[int], le
     a = _lib.DecAttnArgs(q=q.data_ptr(), kv=kv.data_ptr(), max_pos=kv.shape[2], slots_h=sl, lens_h=ln, B=B, heads=heads,
                          kv_heads=kv_heads, hd=hd, dtype={torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}[kv.dtype],
                          grid=grid, assoc_b=assoc_b, out=out.data_ptr())
+    if kraw is not None:
+        for t in (kraw, q_norm, k_norm, rope, qn_out):
+            assert t is None or (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous())
+        a.qk_norm, a.kraw, a.q_norm, a.k_norm, a.rope = 1, kraw.data_ptr(), _ptr(q_norm), _ptr(k_norm), _ptr(rope)
+        a.eps, a.qn_out = float(eps), _ptr(qn_out)
     plan = C.c_int32(0)
     dev = q.device.index or 0
     check(_lib.load().s2s_decode_attention(get_context(dev), C.byref(a), C.byref(plan), _stream_ptr(dev)),
           "s2s_decode_attention")
     return out, int(plan.value)
+
+
+_CODE16 = {torch.float16: S2S_F16, torch.bfloat16: S2S_BF16}
+
+
+def norm_rows(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, eps: float = 1e-5, *,
+              out_h: Optional[torch.Tensor] = None, out_f: Optional[torch.Tensor] = None, dtype: Optional[torch.dtype] = None) -> None:
+    """The prefill / encoder row norm (include/s2s_b200.h s2s_norm_rows) over x f32 [rows, d]: LayerNorm with `bias`, RMSNorm
+    without, written into out_h (16-bit) and / or out_f (f32), [rows, d] each.  dtype: the 16-bit type (default out_h's,
+    else bfloat16).  Asynchronous on the current stream."""
+    for t in (x, w, bias, out_h, out_f):
+        assert t is None or (t.is_cuda and t.is_contiguous())
+    rows, d = x.shape
+    code = _CODE16[dtype or (out_h.dtype if out_h is not None else torch.bfloat16)]
+    dev = x.device.index or 0
+    check(_lib.load().s2s_norm_rows(get_context(dev), _ptr(x), _ptr(w), _ptr(bias), float(eps), rows, d, _ptr(out_h), _ptr(out_f),
+                                    code, _stream_ptr(dev)), "s2s_norm_rows")
+
+
+def prefill_rope(qkv: torch.Tensor, heads: int, kv_heads: int, past: int, rope: torch.Tensor, kcache: torch.Tensor,
+                 vcache: torch.Tensor, *, q_norm: Optional[torch.Tensor] = None, k_norm: Optional[torch.Tensor] = None,
+                 eps: float = 1e-6) -> None:
+    """The RoPE / KV-append step of a Llama-family prefill (include/s2s_b200.h s2s_prefill_rope): qkv 16-bit [n, (heads +
+    2 kv_heads) hd] (pair-adjacent q / k), rope f32 [max_pos, hd / 2, 2], caches 16-bit [max_pos, kv_heads * hd]; q_norm /
+    k_norm f32 [hd] select the Qwen3 q/k norm.  q is rewritten in place, rows [past, past + n) of the caches are written.
+    Asynchronous on the current stream."""
+    for t in (qkv, rope, kcache, vcache, q_norm, k_norm):
+        assert t is None or (t.is_cuda and t.is_contiguous())
+    n = qkv.shape[0]
+    hd = qkv.shape[1] // (heads + 2 * kv_heads)
+    dev = qkv.device.index or 0
+    check(_lib.load().s2s_prefill_rope(get_context(dev), _ptr(qkv), n, heads, kv_heads, hd, past, _ptr(rope), kcache.shape[0],
+                                       _ptr(q_norm), _ptr(k_norm), float(eps), _ptr(kcache), _ptr(vcache), _CODE16[qkv.dtype],
+                                       _stream_ptr(dev)), "s2s_prefill_rope")
+
+
+def argmax_row(logits: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The greedy token choice after a prefill (include/s2s_b200.h s2s_argmax_row) over logits f32 [n] -> int32 [1]
+    (into `out` when given).  Asynchronous on the current stream."""
+    assert logits.is_cuda and logits.dtype == torch.float32 and logits.is_contiguous()
+    out = torch.empty((1,), dtype=torch.int32, device=logits.device) if out is None else out
+    dev = logits.device.index or 0
+    check(_lib.load().s2s_argmax_row(get_context(dev), _ptr(logits), logits.numel(), _ptr(out), _stream_ptr(dev)), "s2s_argmax_row")
+    return out
 
 
 GEMV_MODES = {"store": 0, "gelu": 1, "resid": 2, "qkv": 3, "logits": 4, "qkv_rope": 5, "swiglu": 6}

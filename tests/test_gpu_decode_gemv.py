@@ -790,6 +790,26 @@ def test_argmax_all_but_one_suppressed(E):
         assert (out[:, N - 1] == -100).all() and torch.isneginf(out[:, : N - 1]).all() and torch.isnan(out[:, N:]).all()
 
 
+def test_argmax_all_nan_row_gives_a_valid_id(E):
+    """a session whose logits are all NaN (a NaN input row) gets id 0 -- NaN counts as -inf, so nothing beats the lowest id
+    -- and the other sessions keep their argmax"""
+    N, K, B = 128256, 64, 3
+    gen = torch.Generator(device="cuda").manual_seed(3)
+    wi = torch.randint(-8, 9, (N, K), device="cuda", generator=gen).double()
+    tiled, _ = weights(E, N, K, "bf16", None, ints=wi)
+    x = nan_like((16, K), torch.bfloat16)
+    x[:B] = torch.randint(-1, 2, (B, K), device="cuda", generator=gen).bfloat16()
+    x[1] = float("nan")
+    for grid in (132, 37):
+        out = nan_like((B, N), torch.float32)
+        ids = torch.full((16,), -7, dtype=torch.int32, device="cuda")
+        E.decode_gemv([dict(w=tiled, N=N, K=K, mode="logits", input="copy", x16=x, logits_out=out, logits_ld=N, argmax_out=ids)],
+                      B, torch.bfloat16, grid=grid)
+        ref = x[:B].double() @ wi.T
+        assert torch.isnan(out[1]).all()
+        assert ids[:B].tolist() == [int(ref[0].argmax()), 0, int(ref[2].argmax())], ids[:B].tolist()
+
+
 # ---- arguments the entry point rejects -----------------------------------------------------------------------------------
 def test_rejects_bad_arguments(E):
     from speech_to_speech_b200._lib import S2SError
