@@ -390,8 +390,7 @@ int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int3
                      const int32_t* forced_d, float* logits_out_d, void* stream);
 /* Profiling aid: the stamps of s2s_whisper_set_trace, trace_d[2][capacity][6] (stamp 1, inputs staged, stays 0). */
 int s2s_llama_set_trace(s2s_llama* m, uint64_t* trace_d, int32_t capacity);
-/* Largest B accepted by s2s_llama_decode for this geometry (shared-memory budget of the decode kernel, <= 16); the
- * environment variable S2S_LLAMA_MAX_DECODE_B lowers the value reported here (A/B measurements). */
+/* Largest B accepted by s2s_llama_decode for this geometry (shared-memory budget of the decode kernel, <= 16). */
 int32_t s2s_llama_max_decode_batch(s2s_llama* m);
 /* End-to-end with HOST buffers: (chunked) prefill + decode with the slot's token choice, synchronous.  ids_out_h[0] is
  * the token chosen from the prompt's last position, n_steps tokens in total (generate() semantics of the reference's pipeline call). */

@@ -752,7 +752,6 @@ int snake_launch_h(const float* x, const float* a, const float* ib, int C, int B
 // may the contraction with weights w (C_in = C, N outputs) take an fp16 operand?  (tensor-core mode, packed weights, 16-byte tiles)
 bool fp16_operand_ok(const CodecDecoder* m, const float* w, int C, int N) {
   if (m->cfg.precision == 0 || C % 8 != 0 || N % 4 != 0) return false;
-  if (const char* e = getenv("S2S_CODEC_FP16_OPERANDS")) { if (e[0] == '0') return false; }   // A/B switch (tests: bit-identical)
   auto it = m->tc_w.find(w);
   return it != m->tc_w.end() && it->second.packed != nullptr;
 }

@@ -45,10 +45,9 @@ __device__ __forceinline__ unsigned int ld_relaxed_gpu(const unsigned int* p) {
 // quarter round trip apart; the pipeline is self-clocking (each consumed load is re-issued at once), so the counter
 // is sampled several times per round trip.  After the successful sample thread 0 executes fence.acq_rel.gpu: relaxed load + fence is
 // the PTX acquire pattern, it synchronises with every producer's red.release, and the bar.sync that follows extends
-// the ordering to the CTA's other threads (causality order is transitive over barriers).  `relaxed` != 0 skips the
-// fence (A/B measurements only, S2S_SYNC_RELAXED=1): without it the cross-CTA reads race under the PTX memory model
-// even when every one of them is an L2 access.
-__device__ __forceinline__ void grid_wait(unsigned int* counter, unsigned int epoch_thread0, int relaxed = 0) {
+// the ordering to the CTA's other threads (causality order is transitive over barriers).  Without the fence the
+// cross-CTA reads would race under the PTX memory model even when every one of them is an L2 access.
+__device__ __forceinline__ void grid_wait(unsigned int* counter, unsigned int epoch_thread0) {
   if (threadIdx.x == 0) {
     const unsigned int target = epoch_thread0 * gridDim.x;
     unsigned int v0 = ld_relaxed_gpu(counter), v1 = 0, v2 = 0, v3 = 0;
@@ -75,18 +74,13 @@ __device__ __forceinline__ void grid_wait(unsigned int* counter, unsigned int ep
         if (++spins > (1u << 26)) __trap();
       }
     }
-    if (!relaxed) asm volatile("fence.acq_rel.gpu;" ::: "memory");
+    asm volatile("fence.acq_rel.gpu;" ::: "memory");
   }
   __syncthreads();
 }
 __device__ __forceinline__ void grid_sync(unsigned int* counter, unsigned int& epoch) {
   grid_arrive(counter, epoch);
   grid_wait(counter, epoch);
-}
-// host: S2S_SYNC_RELAXED=1 selects the unfenced barrier waits (measurement aid, never the default)
-inline int dec_sync_relaxed_env() {
-  const char* e = getenv("S2S_SYNC_RELAXED");  // read per launch so one process can A/B
-  return (e && e[0] == '1') ? 1 : 0;
 }
 
 // Warp w of CTA c takes work items  w * gridDim.x + c, then + total_warps ...: consecutive items land on
@@ -1395,7 +1389,7 @@ __device__ __forceinline__ void dec_run(const P& p, const Model& m, const DecVie
           }
         }
         if (tracing && Model::stamps_barrier) tr[3] = dec_clock_ns();  // next phase prepared
-        grid_wait(p.sync_counter, epoch, p.sync_relaxed);
+        grid_wait(p.sync_counter, epoch);
       }
       if (tracing) tr[5] = dec_clock_ns();
       if (!skip) ++trace_i;

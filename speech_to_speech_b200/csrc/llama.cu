@@ -716,17 +716,7 @@ int s2s_llama_decode(s2s_llama* m, const int32_t* slots_h, int32_t B, const int3
   return S2S_OK;
 }
 
-int32_t s2s_llama_max_decode_batch(s2s_llama* m) {
-  if (!m) return 0;
-  int b = llama_max_decode_batch_of(m);
-  // developer knob: a smaller batch per launch than the shared-memory plan allows, so that one build can time both (e.g. 12:
-  // the Llama-3-8B limit before the third plan tier).  Only what the engine reports changes; the TTS slot is unaffected.
-  if (const char* e = getenv("S2S_LLAMA_MAX_DECODE_B")) {
-    const int v = atoi(e);
-    if (v >= 1 && v < b) b = v;
-  }
-  return b;
-}
+int32_t s2s_llama_max_decode_batch(s2s_llama* m) { return m ? llama_max_decode_batch_of(m) : 0; }
 
 int s2s_llama_set_trace(s2s_llama* m, uint64_t* trace_d, int32_t capacity) {
   S2S_REQUIRE(m, "llama set_trace: null model");

@@ -321,11 +321,7 @@ __global__ void llama_decode_init_kernel(const LlamaDecParams p) {
 
 template <typename T, bool F8>
 int launch_t(s2s_ctx* ctx, const LlamaDecParams& p, int debug_phases, cudaStream_t stream) {
-  int grid = dec_grid(ctx);                          // the context's SM partition (s2s_set_sm_partition)
-  if (const char* e = getenv("S2S_DECODE_CTAS")) {   // developer knob: override for experiments (tests/dev/dev_lanes.py)
-    const int v = atoi(e);
-    if (v >= 8 && v < ctx->num_sms) grid = v;
-  }
+  const int grid = dec_grid(ctx);  // the context's SM partition (s2s_set_sm_partition)
   auto kern = llama_decode_kernel<T, F8>;
   long long max_dyn = 0;
   S2S_CHECK_CUDA(s2s_max_dyn_smem(kern, ctx->device, &max_dyn));
@@ -334,7 +330,6 @@ int launch_t(s2s_ctx* ctx, const LlamaDecParams& p, int debug_phases, cudaStream
               "llama decode: batch %d does not fit shared memory for d %d, ffn %d", p.B, p.d, p.ffn);
   const DecSmem lay = dec_smem_layout(p.B, p.d, pl.kmax, p.d, pl.rg);
   LlamaDecParams pr = p;
-  pr.sync_relaxed = dec_sync_relaxed_env();
   pr.ring_slots = pl.slots; pr.norm_rg = pl.rg; pr.down_kc = pl.kc; pr.assoc_b = pl.assoc_b;
   const size_t smem = dec_smem_bytes(lay, pl.slots);
   S2S_REQUIRE((long long)smem <= max_dyn, "llama decode: plan of batch %d needs %zu B of shared memory, %lld available", p.B, smem,

@@ -64,7 +64,6 @@ struct LlamaDecParams {
   int assoc_b;                  // the batch whose plan fixes the attention split plan (set by the launcher, see LlamaDecPlan)
   unsigned long long* trace;    // optional [2][cap][6] globaltimer stamps (profiling aid, dec_run)
   int trace_cap;
-  int sync_relaxed;             // 1: barrier waits without the acquire fence (A/B measurement aid)
   // ---- per-session token choice (sampling.cuh); samp == null: every session takes the argmax-candidate path ----
   const SampSlot* samp;         // [B] or null
   float* samp_rows;             // [B][vocab] fp32 logits rows of the step (used when logits_out is null)

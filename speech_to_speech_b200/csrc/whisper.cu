@@ -519,7 +519,6 @@ static int decode_impl(s2s_whisper* m, const int32_t* prefix_h, const int32_t* p
     p.done = m->done + b0; p.n_done = m->n_done; p.cand_val = m->cand_val + (size_t)b0 * m->ctx->num_sms;
     p.cand_idx = m->cand_idx + (size_t)b0 * m->ctx->num_sms; p.sync_counter = m->sync_counter;
     p.trace = m->trace; p.trace_cap = m->trace_cap;
-    { const char* tm = getenv("S2S_TRACE_MODE"); p.trace_mode = (tm && tm[0] == '1') ? 1 : 0; }
     S2S_CHECK(whisper_decode_launch(m->ctx, p, c.compute_dtype, m->debug_phases, st));
   }
   return S2S_OK;

@@ -286,14 +286,13 @@ __device__ __forceinline__ unsigned int cluster_nctaid_x() {
 // ONE thread publishes the CTA's writes (bar.sync + fence by thread 0: cumulative, like grid_arrive); the hardware barrier
 // itself is relaxed -- barrier.cluster.arrive.release makes EVERY thread execute MEMBAR.ALL.GPU, which serialises
 // with 256 threads.  Readers use L2 accesses (ld.global.cg) after the wait.
-__device__ __forceinline__ void cluster_barrier(int relaxed) {
+__device__ __forceinline__ void cluster_barrier() {
   __syncthreads();
   if (threadIdx.x == 0) asm volatile("fence.acq_rel.gpu;" ::: "memory");
   asm volatile("barrier.cluster.arrive.relaxed.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory");
-  if (!relaxed) {  // acquire side, mirrored: one fencing thread, then the CTA barrier extends the order to the others
-    if (threadIdx.x == 0) asm volatile("fence.acq_rel.gpu;" ::: "memory");
-    __syncthreads();
-  }
+  // acquire side, mirrored: one fencing thread, then the CTA barrier extends the order to the others
+  if (threadIdx.x == 0) asm volatile("fence.acq_rel.gpu;" ::: "memory");
+  __syncthreads();
 }
 
 struct WdcCtx { int cid, rank, cs; };
@@ -306,7 +305,7 @@ __device__ __forceinline__ void wdc_out_args(const WhisperDecParams& p, const Wd
 }
 
 // The cluster kernel's phases for dec_run (decode_common.cuh): the kernel's shared copy of the parameters and the cluster
-// identity.  Stamps 2 and 3 of the trace are the block's intra-phase milestones (S2S_TRACE_MODE selects which).
+// identity.  Stamps 2 and 3 of the trace are the block's intra-phase milestones: q/k/v rows done, cluster barrier 1 passed.
 template <typename T>
 struct WdcModel {
   static constexpr bool stamps_barrier = false;
@@ -386,12 +385,12 @@ struct WdcModel {
     }
     __syncthreads();
     gemv_mma<T, false>(a, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
-    if (tr && p.trace_mode == 0) tr[2] = dec_clock_ns();
+    if (tr) tr[2] = dec_clock_ns();
     // C. start streaming the head's out-projection slice
     gemv_prefetch<T>(ao, ring);
     // D. q (and the new k, v cache rows) of the head are visible to the whole cluster
-    cluster_barrier(p.sync_relaxed);
-    if (tr && p.trace_mode == 0) tr[3] = dec_clock_ns();
+    cluster_barrier();
+    if (tr) tr[3] = dec_clock_ns();
     // E. attention: 32-key blocks over (CTA rank, warp); one record per CTA
     float* rec_s = reinterpret_cast<float*>(sm.red);
     {
@@ -420,12 +419,10 @@ struct WdcModel {
       }
     }
     // F. every CTA's record of the head is visible to the cluster
-    cluster_barrier(p.sync_relaxed);
-    if (tr && p.trace_mode == 1) tr[2] = dec_clock_ns();
+    cluster_barrier();
     // G. merge the CS records (redundantly in every CTA: one L2 round trip, no further hand-off) -> o_h as x operand
     if (warp < B) attn_merge_records<T, HD>(p.part + (long long)(warp * H + h) * p.s_max * REC, cx.cs, sm.xh + warp * (HD + GV_XPAD));
     __syncthreads();
-    if (tr && p.trace_mode == 1) tr[3] = dec_clock_ns();
     // H. the head's slice of the out-projection -> partial residual update
     gemv_mma<T, false>(ao, smem_u32(sm.xh), B, best_v, best_i, ring, sm.red);
   }
@@ -560,7 +557,6 @@ int launch_cluster_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, 
   cached_smem = smem; cached_heads = p.heads; cached_cs = cs; cached_n = n_clusters; cached_grid = lane_grid;
   if (!cs) return S2S_OK;
   WhisperDecParams pr = p;
-  pr.sync_relaxed = dec_sync_relaxed_env();
   pr.ring_slots = slots;
   pr.cluster_size = cs;
   whisper_decode_init_kernel<T><<<p.B, 256, 0, stream>>>(pr);
@@ -581,7 +577,6 @@ int launch_t(s2s_ctx* ctx, const WhisperDecParams& p, int debug_phases, cudaStre
   }
   const DecSmem lay = dec_smem_layout(p.B, p.d, std::max(p.d, p.ffn), 2 * p.d);
   WhisperDecParams pr = p;
-  pr.sync_relaxed = dec_sync_relaxed_env();
   pr.ring_slots = dec_ring_slots(lay, WD_SMEM_BUDGET);
   {
     const int BH = p.B * p.heads, grid = dec_grid(ctx);

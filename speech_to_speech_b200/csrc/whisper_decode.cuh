@@ -52,8 +52,6 @@ struct WhisperDecParams {
   int ring_slots;               // weight-ring slots per warp (set by the launcher from the shared-memory budget)
   unsigned long long* trace;   // optional [2][trace_cap][6] globaltimer stamps (profiling aid, dec_run)
   int trace_cap;
-  int trace_mode;              // which intra-phase stamps the cluster kernel records (profiling aid)
-  int sync_relaxed;            // 1: barrier waits without the acquire fence (A/B measurement aid, S2S_SYNC_RELAXED=1)
 };
 
 int whisper_decode_launch(s2s_ctx* ctx, const WhisperDecParams& p, int dtype, int debug_phases, cudaStream_t stream);

@@ -175,8 +175,7 @@ def byte_tokenizer(text_vocab: int, reserved: int = 16) -> Callable[[str], list]
 class B200Qwen3TTS:
     def __init__(self, engine: Any, tokenize: Callable[[str], Sequence[int]], speakers: Mapping[str, int], max_sessions: int = 1,
                  batch_wait_s: float = 0.012, tts_model_type: str = "custom_voice", lane: int = 0, lanes: int = 1,
-                 batch_gap_s: Optional[float] = 0.003, prefetch_chunks: bool = True, sampling: Optional[Mapping] = None,
-                 sampling_seed: Optional[int] = None):
+                 batch_gap_s: Optional[float] = 0.003, sampling: Optional[Mapping] = None, sampling_seed: Optional[int] = None):
         # batch_gap_s: a session needs a few ms of host work between two chunk requests (resample + int16 + D2H of the chunk it
         # just received); the gap must cover it, or the sessions of the launch that just ended miss the next one and two groups
         # alternate in half-full launches (measured: mean batch 7.8 of 16 with a 0.6 ms gap)
@@ -184,8 +183,7 @@ class B200Qwen3TTS:
         self.lane, self.lanes = int(lane), int(lanes)
         self.max_sessions = int(max_sessions)
         self._options = dict(batch_wait_s=batch_wait_s, tts_model_type=tts_model_type, batch_gap_s=batch_gap_s,
-                             prefetch_chunks=prefetch_chunks, sampling=sampling, sampling_seed=sampling_seed)
-        self.prefetch_chunks = bool(prefetch_chunks)   # False: request chunk k + 1 only after the consumer took chunk k (A/B, tests)
+                             sampling=sampling, sampling_seed=sampling_seed)
         self.tokenize = tokenize
         # default token choice of generate_custom_voice_streaming (None = greedy; COUSIN_SAMPLING = the cousin's) and one
         # 64-bit Philox seed per sampled utterance, drawn from a generator seeded by sampling_seed (OS entropy when None)
@@ -370,13 +368,10 @@ class B200Qwen3TTS:
                 valid, finished, wav = pending.result()
                 pending = None
                 done += valid
-                more = not finished and done < budget
-                if more and self.prefetch_chunks:
+                if not finished and done < budget:
                     pending = self.batcher.submit(min(chunk, budget - done), slot)
                 if wav is not None and wav.numel() > 0:
                     yield DeviceAudio(wav), SAMPLE_RATE, {"frames": done, "elapsed_s": perf_counter() - t0}
-                if more and not self.prefetch_chunks:
-                    pending = self.batcher.submit(min(chunk, budget - done), slot)
         finally:
             if pending is not None and not pending.cancel():     # consumer stopped early: the slot is in use until the launch ends
                 try:

@@ -28,8 +28,8 @@ for cta in (0, 1):
         sel = [idx + s * nph + l * 4 + k for s in range(4) for l in range(L)]
         def rel(j):
             v = t[cta, sel, j]; return np.where(v > 0, v - t[cta, sel, 0], 0).mean()
-        lab = ("q/k/v rows done", "cluster barrier 1 passed") if os.environ.get("S2S_TRACE_MODE", "0") != "1" else ("attention + cluster barrier 2 passed", "records merged")
-        print(f"  {names[k]:10s} body {body[sel].mean():8.0f}  barrier {bar[sel].mean():8.0f}   [staged {rel(1):6.0f} | {lab[0]} {rel(2):6.0f} | {lab[1]} {rel(3):6.0f}]")
+        print(f"  {names[k]:10s} body {body[sel].mean():8.0f}  barrier {bar[sel].mean():8.0f}   [staged {rel(1):6.0f} | "
+              f"q/k/v rows done {rel(2):6.0f} | cluster barrier 1 passed {rel(3):6.0f}]")
     sel = [idx + s * nph + 4 * L for s in range(4)]
     print(f"  {'logits':10s} body {body[sel].mean():8.0f}  barrier {bar[sel].mean():8.0f}")
     sel = [idx + s * nph + 4 * L + 1 for s in range(4)]

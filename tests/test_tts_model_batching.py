@@ -2,16 +2,12 @@
 SessionBatcher.  The case that matters is two groups of sessions out of phase by half a launch whose consumers need longer
 than the batch gap to digest a chunk (on the GPU: waiting for the chunk's codec kernels + resample + D2H, ~10 ms): without the
 prefetched request they lock into alternating half-full launches, with it they merge into full ones."""
-import os
-import sys
 import threading
 import time
 import types
 
 import pytest
 import torch
-
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))   # `python tests/test_tts_model_batching.py`
 
 from speech_to_speech_b200.tts_model import B200Qwen3TTS
 
@@ -56,9 +52,9 @@ class FakeEngine:
         pass
 
 
-def _run(prefetch: bool):
+def _run():
     eng = FakeEngine()
-    tts = B200Qwen3TTS(eng, lambda text: [1, 2, 3], {"a": 0}, max_sessions=16, batch_wait_s=0.06, batch_gap_s=0.004, prefetch_chunks=prefetch)
+    tts = B200Qwen3TTS(eng, lambda text: [1, 2, 3], {"a": 0}, max_sessions=16, batch_wait_s=0.06, batch_gap_s=0.004)
     got = {}
 
     def session(i, delay):
@@ -78,7 +74,7 @@ def _run(prefetch: bool):
 
 
 def test_prefetched_requests_merge_two_groups_into_full_launches():
-    eng, got = _run(prefetch=True)
+    eng, got = _run()
     for i in range(16):   # every session got its chunks in order, each decoded from its own frame counter
         assert [f for f, _ in got[i]] == [8 * (k + 1) for k in range(CHUNKS)]
         assert [v for _, v in got[i]] == [float(8 * (k + 1)) for k in range(CHUNKS)]
@@ -87,8 +83,8 @@ def test_prefetched_requests_merge_two_groups_into_full_launches():
 
 
 # Without the prefetch the two groups alternate in half-full launches (what the handler wave measured on the GPU: mean batch 7.8
-# of 16): `python tests/test_tts_model_batching.py` prints both launch sequences.  Not a test: the alternation is an unstable
-# equilibrium under host-thread jitter, on a busy CPU box the groups sometimes fall into step by chance.
+# of 16).  That is not asserted: the alternation is an unstable equilibrium under host-thread jitter, on a busy CPU box the
+# groups sometimes fall into step by chance.
 
 
 def test_consumer_that_stops_early_releases_the_slot_after_the_prefetched_launch():
@@ -100,8 +96,3 @@ def test_consumer_that_stops_early_releases_the_slot_after_the_prefetched_launch
     assert sorted(tts._free) == [0, 1]
     assert eng.n[0] in (8, 16)                     # at most one chunk ahead of the consumer
     tts.close()
-
-
-if __name__ == "__main__":
-    for pf in (False, True):
-        print("prefetch" if pf else "no prefetch", _run(pf)[0].launches)
